@@ -55,30 +55,19 @@ CPU_SAMPLE = 131072
 
 
 def _peaks():
-    """Roofline denominators: MEASURED_PEAKS.json (driver-written).  The tensor figure used is the BURST one: the
-    timed region is a fraction of a second at full clocks (VERDICT r1); the sustained figure is reported beside it."""
+    """Roofline denominators: MEASURED_PEAKS.json when present (measured on the machine; the tensor figure used is the
+    BURST one, the sustained figure is reported beside it), else NVIDIA's H100 SXM data-sheet figures (700 W card)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained"), "src": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "src": "fallback (B200_PROFILING.md)"}
-
-
-def _measured_traffic():
-    """dram bytes per launch of this build's kernels, from the ncu --set full pass committed under profiles/
-    (tools/ncu_traffic.py writes the file); None when no pass of the current round exists."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": None,
+            "src": "H100 SXM data sheet (dense, 700 W), not measured"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -324,7 +313,7 @@ def timed_graph(fn, n=8, reps=5):
 
 def encoder_rooflines(dev, peaks, netG):
     """Tensor-bound kernels of the encoders: the ResnetBlock convolution (80 % of NormalNet's FLOPs) and the whole
-    forwards, algorithmic FLOPs / time against the measured bf16 burst peak (the kernels execute 3 fp16 MMAs per
+    forwards, algorithmic FLOPs / time against the bf16 peak of _peaks() (the kernels execute 3 fp16 MMAs per
     algorithmic one)."""
     import torch
     import torch.nn as nn
@@ -336,12 +325,10 @@ def encoder_rooflines(dev, peaks, netG):
         op, _ = T.act(raw, halo=1)
         ms = timed_graph(lambda: T.conv(op, m))
         flop = 2.0 * 1024 * 9 * 1024 * 32 * 32
-        out.append({"kernel": "k_conv_nhwc<256,2> + k_splitk_nhwc: ResnetBlock conv 1024->1024 3x3 reflect @32x32 (TMA + tcgen05, "
+        out.append({"kernel": "k_conv_nhwc<256,2> + k_splitk_nhwc: ResnetBlock conv 1024->1024 3x3 reflect @32x32 (TMA + wgmma, "
                               "fp16 hi/lo x3, split-K 4)", "bound": "tensor", "ms": ms, "achieved": flop / ms / 1e9,
                     "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": flop / ms / 1e9 / peaks["bf16_tflops"],
-                    "executed_frac": 3 * flop / ms / 1e9 / peaks["bf16_tflops"],
-                    "note": "operand traffic L2 -> SM is 96 KB per 64-channel chunk = 59 B/clk/SM at the MMA rate, above the "
-                            "~43 B/clk/SM the L2 sustains chip-wide (B300_MICROARCH.md: ~6300 B/clk): L2-bound, not MMA-bound"})
+                    "executed_frac": 3 * flop / ms / 1e9 / peaks["bf16_tflops"]})
         batch = {k: v.to(dev) for k, v in S.encoder_inputs_512(seed=5).items()}
         for _ in range(3):
             netG.normal_filter(batch)
@@ -365,7 +352,7 @@ def encoder_rooflines(dev, peaks, netG):
 
 
 def secondary_rooflines(dev, peaks, flush):
-    """HBM-bound kernels of the path at their real sizes: algorithmic bytes / CUDA-event time / measured HBM peak."""
+    """HBM-bound kernels of the path at their real sizes: algorithmic bytes / CUDA-event time / HBM peak of _peaks()."""
     import torch
     from icon_b200 import ops
     out = []
@@ -497,6 +484,27 @@ def reference_gpu_encoders(dev, netG, reps=3):
     return out
 
 
+def dump_sample(n_points, n_images):
+    """The lattice points whose occupancies --dump-outputs writes: a fixed seeded sample, the same on every rank and in
+    every run, of at most 2^22 points over ALL images of the run (<= 16 MB of float32 occupancies + 32 MB of indices)."""
+    import numpy as np
+    per = min(n_points, (1 << 22) // max(1, n_images))
+    if per == n_points:
+        return np.arange(n_points)
+    return np.sort(np.random.default_rng(0).choice(n_points, size=per, replace=False))
+
+
+def dump_outputs(out_dir, kept, image_ids, idx, write_index):
+    """occupancy_img<id>.npy per image of this rank (float32, occupancies at the sampled points) and, from one rank,
+    sample_index.npy (float64) -- so that two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    if write_index:
+        np.save(os.path.join(out_dir, "sample_index.npy"), idx.astype(np.float64))
+    for i, occ in zip(image_ids, kept):
+        np.save(os.path.join(out_dir, f"occupancy_img{i}.npy"), occ.float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -508,6 +516,9 @@ def main():
     ap.add_argument("--grid", type=int, default=None, help=argparse.SUPPRESS)
     ap.add_argument("--no-cpu-baseline", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--no-extras", action="store_true", help="metric + e2e only (skip recon / rooflines / baselines)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the occupancies of the last timed step as DIR/occupancy_img<id>.npy (float32; a fixed "
+                         "seeded sample of at most 2^22 points over all images, indices in DIR/sample_index.npy as float64)")
     args = ap.parse_args()
     wl = dict(WORKLOADS[args.workload])
     if args.grid:
@@ -544,7 +555,7 @@ def main():
     grid = wl["grid"]
     pts_cpu = S.lattice_points(grid)                                      # [1, N, 3]: 201 MB at 256^3, 1.6 GB at 512^3
     N = pts_cpu.shape[1]
-    pts_dev = pts_cpu.to(dev)                                             # larger than the 126 MB L2
+    pts_dev = pts_cpu.to(dev)                                             # larger than the 50 MB L2
     pts_pin = pts_cpu.pin_memory()
     out_pin = torch.empty(1, 1, N, dtype=torch.float32).pin_memory()
 
@@ -557,11 +568,18 @@ def main():
         im.bind(netG)
         return net.query_func(cfg, netG, [im.feat], pts)
 
-    def step_resident():
-        out = None
+    def step_resident(keep=None):
+        """One step over this rank's images; `keep(out)` (last step of --dump-outputs only) picks what to hold on to,
+        so at most one full output is alive at a time."""
+        out, kept = None, []
         for im in images:
             out = query(im, pts_dev)
-        return out
+            if keep is not None:
+                kept.append(keep(out))
+        return out, kept
+
+    sample = dump_sample(N, n_images) if args.dump_outputs else None
+    sample_dev = torch.from_numpy(sample).to(dev) if args.dump_outputs else None
 
     sampler = ClockSampler(local)
     if rank == 0:
@@ -577,13 +595,17 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record()
-    for _ in range(args.steps):
-        out = step_resident()
+    for s in range(args.steps):
+        last = args.dump_outputs and s == args.steps - 1
+        out, kept = step_resident(keep=(lambda o: o.reshape(-1).index_select(0, sample_dev)) if last else None)
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
     launches = _C.launch_count() - l0
     checksum = float(out.double().sum().item()) if out is not None else 0.0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, kept, mine, sample, rank == 0)
+    del out, kept
 
     # ---- timed region 2: end to end through query_func with HOST buffers.  Every image of every step copies its
     #      points from pinned host memory and its result back; the three stages (H2D, query, D2H) of consecutive
@@ -666,33 +688,25 @@ def main():
         e2e = total_pts / (ms_e2e * 1e-3) / 1e6
         mlp_ms, sdf_ms = stage[3], stage[1]
         achieved = N * wl["flop"] / (mlp_ms * 1e-3) / 1e12 if mlp_ms > 0 else 0.0
-        traffic = _measured_traffic() or {}
-        t_mlp = traffic.get("k_query_mlp_tc", {})
         mlp_roof = {
-            "kernel": f"k_query_mlp_tc<{wl['prior']}> (tcgen05, fp16 hi/lo x3)", "bound": "tensor",
+            "kernel": f"k_query_mlp_tc<{wl['prior']}> (wgmma, fp16 hi/lo x3)", "bound": "tensor",
             "achieved": achieved, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
             "frac": achieved / peaks["bf16_tflops"],
-            "traffic": t_mlp.get("dram_bytes_per_launch") if t_mlp.get("points") == N else None,
-            "traffic_source": (t_mlp.get("source") if t_mlp.get("points") == N else
-                               "no ncu --set full pass of this build at this size under profiles/"),
             "ms": mlp_ms, "executed_tflops": 3.0 * achieved, "executed_frac": 3.0 * achieved / peaks["bf16_tflops"],
             "peak_sustained": peaks["bf16_tflops_sustained"],
             "frac_of_sustained": achieved / peaks["bf16_tflops_sustained"] if peaks["bf16_tflops_sustained"] else None,
-            "peak_source": peaks["src"] + ": cuBLAS bf16 BURST figure (the timed region is well under a second at full "
-                                          "clocks); the 4-s sustained figure is given beside it",
+            "peak_source": peaks["src"],
             "note": "achieved = algorithmic MLP FLOPs (FLOP/pt x points) / kernel time from CUDA events on the launch "
                     "stream; the kernel executes 3 fp16 MMAs per algorithmic one to hold 1e-4 (executed_*)"}
         rooflines = [mlp_roof]
         if wl["prior"] == "icon" and sdf_ms > 0:
             by = N * (16 + 32 + 4)                       # xyz4 in, rec[8] + face-rank out
-            t_sdf = traffic.get("k_sdf_warp", {})
             rooflines.append({
                 "kernel": "k_sdf_warp<32> (exact nearest face + ray parity, issue-bound tree walk)", "bound": "hbm",
                 "ms": sdf_ms, "achieved": by / sdf_ms / 1e6, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                 "frac": by / sdf_ms / 1e6 / peaks["hbm_gbs"], "algorithmic_bytes": by,
-                "traffic": t_sdf.get("dram_bytes_per_launch") if t_sdf.get("points") == N else None,
                 "note": "no clean FLOP count (O(log F)..O(F) triangle tests per point); neither HBM- nor tensor-bound: "
-                        "instruction issue (profiles/); the HBM figure is reported because SURVEY 8d asks for bytes"})
+                        "instruction issue; the HBM figure is reported because SURVEY 8d asks for bytes"})
         rooflines += extras.get("rooflines", [])
         line = {
             "metric": f"M query-points/sec at {grid}^3 grid", "value": value, "unit": "Mpoints/s",

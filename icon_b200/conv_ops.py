@@ -8,14 +8,13 @@ import torch
 
 from . import _C
 from ._C import check, lib
-from .ops import _need_cuda, _p, _stream
+from .ops import _need_cuda, _p, _sm_count, _stream
 
 
-# "auto": encoders run the NHWC / TMA path (icon_b200/nhwc.py); single ops here use the NCHW tcgen05 kernel when
+# "auto": encoders run the NHWC / TMA path (icon_b200/nhwc.py); single ops here use the NCHW wgmma kernel when
 # Cin % 64 == 0 and the FP32 kernel otherwise.  "nchw": the round-1 NCHW path everywhere.  "fp32": always FP32.
 _IMPL = "auto"
 _PACK_CACHE = {}
-NUM_SMS = 148
 
 
 def set_conv_impl(name):
@@ -66,13 +65,14 @@ def _pack_tc(w, transposed, n_tile):
 
 
 def _tc_plan(npix, cout, chunks):
-    """Widest channel tile the layer allows (N=256 MMAs run at 93 % of the tensor rate, N<=128 pay a flat
-    ~93 cycles each: tools/umma_rate.cu); fill the SMs with split-K rather than with narrower tiles."""
+    """Widest channel tile the layer allows (fewest re-reads of the A tile); fill the SMs with split-K rather than with
+    narrower tiles."""
     n_tile = 256 if cout > 128 else (128 if cout > 64 else 64)
     items = ((npix + 127) // 128) * ((cout + n_tile - 1) // n_tile)
     splits = 1
-    if items < NUM_SMS:
-        splits = max(1, min(16, NUM_SMS // items, chunks))
+    sms = _sm_count()
+    if items < sms:
+        splits = max(1, min(16, sms // items, chunks))
     return n_tile, splits
 
 

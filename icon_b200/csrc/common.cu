@@ -147,10 +147,10 @@ namespace icon {
 int device_sm_count() {
     static int counts[ICON_MAX_DEVICES] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= ICON_MAX_DEVICES) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= ICON_MAX_DEVICES) return 132;
     if (!counts[dev]) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         counts[dev] = n;
     }
     return counts[dev];
@@ -162,7 +162,7 @@ bool pdl_enabled() {
     static int v = -1;
     if (v < 0) {
         const char *e = getenv("ICON_B200_PDL");
-        v = (e && e[0] == '1') ? 1 : 0;          // measured on B200: slower than plain graph replay here (profiles/r2_summary.md)
+        v = (e && e[0] == '1') ? 1 : 0;
     }
     return v == 1;
 }

@@ -1,4 +1,4 @@
-// Shared helpers for libicon_b200.so (sm_100a only).
+// Shared helpers for libicon_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -53,7 +53,7 @@ int device_sm_count();    // multiprocessors of the CURRENT device (cached per d
 
 // Programmatic dependent launch (PDL): the encoders are chains of ~600 short kernels; launched with the programmatic-
 // stream-serialization attribute a kernel's CTAs may be scheduled while its predecessor drains, do their local set-up
-// (barrier init, TMEM allocation, descriptor prefetch) and then block in pdl_wait() until the predecessor has completed
+// (barrier init, descriptor prefetch) and then block in pdl_wait() until the predecessor has completed
 // and its writes are visible.  Every kernel launched through launch_pdl() calls pdl_launch_dependents() first thing and
 // pdl_wait() before its first global-memory access; both are no-ops for a normal launch.  OFF by default (it measured
 // slower than plain CUDA-graph replay: dependents park on the SMs the predecessor's tail still needs); ICON_B200_PDL=1 enables it.

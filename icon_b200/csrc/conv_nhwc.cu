@@ -1,4 +1,4 @@
-// Encoder convolutions, Blackwell-first: implicit GEMM on tcgen05 with BOTH operands staged by the TMA engine.
+// Encoder convolutions: implicit GEMM on the Hopper tensor cores (wgmma) with BOTH operands staged by the TMA engine.
 //
 // Replaces cuDNN in the encoders (reference: lib/net/FBNet.py:216-319 GlobalGenerator / ResnetBlock,
 // lib/net/HGFilters.py:49-197 + lib/net/net_util.py:258-280 HGFilter / HourGlass / ConvBlock).
@@ -10,22 +10,23 @@
 // out-of-bounds fill, reflection padding is a halo the producer wrote, stride 2 is a space-to-depth layout the
 // producer wrote (4 parity planes), a transposed convolution is 4 output phases with 1/2/2/4 taps each.  The box
 // lands in shared memory as 128 rows (pixels) x 128 bytes (64 fp16), 16-byte chunks XOR-swizzled by row % 8 --
-// the K-major SWIZZLE_128B operand layout of tcgen05.mma, so the MMA reads it through a descriptor with no thread
+// the K-major SWIZZLE_128B operand layout of wgmma, so the MMA reads it through a descriptor with no thread
 // ever touching the data.  Weights: host-packed tiles in the same layout (1-D bulk copies).
 //
-//   D[128 pixels][NT channels] += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi      (3 kind::f16 MMAs per k-step, fp32 in TMEM)
+//   D[128 pixels][NT channels] += A_hi*B_hi + A_hi*B_lo + A_lo*B_hi      (3 f16 wgmmas per k-step, fp32 in registers)
 //
-//   warp 0      producer: 2 tensor-map loads (A hi, A lo) + 1 bulk copy (B hi|lo) per chunk, STAGES-deep ring
-//   warp 1      TMEM allocation (NT columns only) + MMA issue (one lane)
-//   warps 2-5   epilogue: TMEM -> registers -> (+bias) -> fp32 NHWC store (optionally into a channel slice of a
-//               wider tensor = torch.cat for free) and per-(image, channel) sum / sum-of-squares for the
-//               Instance/GroupNorm that follows (fp64 atomics), so the norm needs no statistics pass.
+//   warps 0-7   two consumer warpgroups (warpgroup g: pixels [64 g, 64 g + 64) of the tile, M = 64, N = NT), then the
+//               epilogue: accumulators -> shared memory -> one column (channel) per thread walking the pixels:
+//               coalesced fp32 NHWC stores (optionally into a channel slice of a wider tensor = torch.cat for free),
+//               +bias, and per-(image, channel) sum / sum-of-squares for the Instance/GroupNorm that follows (fp64
+//               atomics), so the norm needs no statistics pass.
+//   warp 8      producer: 2 tensor-map loads (A hi, A lo) + 1 bulk copy (B hi|lo) per chunk, STAGES-deep ring
 // Small spatial extents (the 32 x 32 ResnetBlocks) fill the machine through split-K (partials + k_splitk_nhwc).
 #include <cuda.h>
 #include <cuda_fp16.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace icon {
 
@@ -47,25 +48,20 @@ struct ConvNhwcParams {
     TapDesc taps[MAX_TAPS];
 };
 
-constexpr int CN_THREADS = 192;
+constexpr int CN_THREADS = 288;
 
 template <int NT, int STAGES>
 __global__ void __launch_bounds__(CN_THREADS, NT == 64 ? 2 : 1)
 k_conv_nhwc(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
             const __grid_constant__ ConvNhwcParams p) {
-    using namespace um;
+    using namespace wg;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t bar_full[STAGES], bar_empty[STAGES], bar_acc;
-    __shared__ uint32_t tmem_slot;
-    // NT <= 128: the hi | lo weight tiles of a chunk are contiguous in shared memory, i.e. ONE K-major operand of 2 NT
-    // rows, so A_hi * [B_hi ; B_lo] is a single N = 2 NT instruction into two accumulators (summed in the epilogue).
-    // Two MMAs per k-step instead of three, and the wide one runs at the full tensor rate (instructions with N <= 128
-    // are bound by fetching the A operand from shared memory, not by the arithmetic).
-    constexpr bool MERGE = NT <= 128;
-    constexpr int TCOLS = MERGE ? 2 * NT : NT;
+    __shared__ uint64_t bar_full[STAGES], bar_empty[STAGES];
     constexpr uint32_t A_BYTES = 128 * 128;                   // one half (hi or lo) of the A tile
     constexpr uint32_t B_BYTES = NT * 256;                    // hi | lo
     constexpr uint32_t STAGE = 2 * A_BYTES + B_BYTES;
+    constexpr int LD = NT + 8;                                // epilogue tile [128][LD] fp32 over the drained stages
+    static_assert(128 * LD * 4 <= STAGES * STAGE, "epilogue tile");
     const uint32_t base = (s32(smem_raw) + 1023u) & ~1023u;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     pdl_launch_dependents();
@@ -82,23 +78,15 @@ k_conv_nhwc(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ 
     const int x0 = tx * p.BW, y0 = ty * p.BH;
 
     if (tid == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(s32(&bar_full[s]), 1); mbar_init(s32(&bar_empty[s]), 1); }
-        mbar_init(s32(&bar_acc), 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(s32(&bar_full[s]), 1); mbar_init(s32(&bar_empty[s]), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         tma_prefetch_desc(&map_hi);
         tma_prefetch_desc(&map_lo);
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s32(&tmem_slot)), "n"(TCOLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = tmem_slot;
     pdl_wait();                       // everything above is local set-up; the predecessor's outputs are read from here on
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             const uint8_t *wsrc = p.wt + (size_t)blockIdx.y * p.wt_chunks * B_BYTES;
             for (int i = 0; i < nchunks; ++i) {
@@ -114,129 +102,77 @@ k_conv_nhwc(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ 
                 bulk_g2s(dst + 2 * A_BYTES, wsrc + (size_t)(td.wtap * p.cpt + cb) * B_BYTES, B_BYTES, full);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t IDESC = idesc_f16(128, NT);
-            for (int i = 0; i < nchunks; ++i) {
-                const uint32_t s = i % STAGES, ph = (i / STAGES) & 1;
-                mbar_wait(s32(&bar_full[s]), ph);
-                fence_after();
-                const uint32_t sb = base + s * STAGE;
-                const uint64_t ah = desc_sw128(sb), al = desc_sw128(sb + A_BYTES);
-                const uint64_t bh = desc_sw128(sb + 2 * A_BYTES), bl = desc_sw128(sb + 2 * A_BYTES + NT * 128);
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {               // 4 x (K = 16): +32 bytes inside the 128-byte row
-                    if constexpr (MERGE) {
-                        constexpr uint32_t IDESC2 = idesc_f16(128, 2 * NT);
-                        mma_ss(tmem, ah + 2 * ks, bh + 2 * ks, IDESC2, (i | ks) != 0);     // [hi*Whi | hi*Wlo]
-                        mma_ss(tmem, al + 2 * ks, bh + 2 * ks, IDESC, 1);                  // lo*Whi -> first accumulator
-                    } else {
-                        mma_ss(tmem, ah + 2 * ks, bh + 2 * ks, IDESC, (i | ks) != 0);
-                        mma_ss(tmem, ah + 2 * ks, bl + 2 * ks, IDESC, 1);
-                        mma_ss(tmem, al + 2 * ks, bh + 2 * ks, IDESC, 1);
-                    }
-                }
-                (void)bl;
-                commit(s32(&bar_empty[s]));
-            }
-            commit(s32(&bar_acc));
-        }
-    } else {
-        // ---------------------------------------------------------------- epilogue
-        // TMEM hands every thread one PIXEL (32 channels at a time); global memory wants a warp on one pixel's
-        // CHANNELS (128 contiguous bytes).  Each warp therefore transposes its 32 x 32 block through shared memory
-        // (conflict-free, stride 33) and then walks its 32 pixels with lane = channel: one coalesced 128-byte store
-        // per pixel, and the per-channel sums for the following norm fall out of the same walk.
-        const int q4 = warp & 3, r = q4 * 32 + lane;                      // TMEM lane = pixel index inside the tile
-        const int et = (warp - 2) * 32 + lane;                            // 0..127 among the epilogue threads
-        const uint32_t tl = tmem + ((uint32_t)(q4 * 32) << 16);
-        mbar_wait(s32(&bar_acc), 0);
-        fence_after();
-        float *red = reinterpret_cast<float *>(smem_raw + (base - s32(smem_raw)));       // [128][33] + [4][32][2]
-        float *part = red + 128 * 33;
-        const int n0 = blockIdx.y * NT;
-        const bool fin = p.splits == 1;
-        const int bw_shift = 31 - __clz(p.BW), bw_mask = p.BW - 1;
-        const size_t split_stride = (size_t)p.N * p.Ht * p.Wt * p.Cout;
+        return;
+    }
 
-        // (a) final tile + statistics: transposed walk (coalesced stores, sums from the same walk)
-        // (b) final tile, no statistics / (c) split-K partial: straight 128-bit stores of the thread's own pixel
-        const int a_me = y0 + (r >> bw_shift), b_me = x0 + (r & bw_mask);
-        const bool pv = a_me < p.Ht && b_me < p.Wt;
-        float *direct = nullptr;
-        if (fin) direct = p.out + (((size_t)n * p.OHf + (size_t)(a_me * p.osy + p.ooy)) * p.OWf + (size_t)(b_me * p.osx + p.oox)) * p.Cs + p.co_off;
-        else direct = p.partial + (size_t)blockIdx.z * split_stride + (((size_t)n * p.Ht + a_me) * p.Wt + b_me) * p.Cout;
-        const bool walk = fin && p.stats != nullptr;
-        const bool vec_ok = ((reinterpret_cast<uintptr_t>(direct) & 15) == 0);
-        for (int cb = 0; cb < NT; cb += 32) {
-            if (n0 + cb >= p.Cout) break;
-            uint32_t acc[32];
-            tmem_ld32(tl + cb, acc);
-            if constexpr (MERGE) {
-                uint32_t acc2[32];
-                tmem_ld32(tl + NT + cb, acc2);
+    // ---------------------------------------------------------------- consumers: mainloop
+    const int g = warp >> 2;
+    float acc[NT / 2];
 #pragma unroll
-                for (int j = 0; j < 32; ++j) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __uint_as_float(acc2[j]));
-            }
-            if (nchunks == 0) {
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < nchunks; ++i) {
+        const uint32_t s = i % STAGES, ph = (i / STAGES) & 1;
+        mbar_wait(s32(&bar_full[s]), ph);
+        const uint32_t sb = base + s * STAGE;
+        const uint64_t ah = desc_sw128(sb + g * 8192), al = desc_sw128(sb + A_BYTES + g * 8192);
+        const uint64_t bh = desc_sw128(sb + 2 * A_BYTES), bl = desc_sw128(sb + 2 * A_BYTES + NT * 128);
+        fence();
 #pragma unroll
-                for (int j = 0; j < 32; ++j) acc[j] = 0u;
-            }
-            if (!walk) {
-                if (fin && p.bias) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (n0 + cb + j < p.Cout) acc[j] = __float_as_uint(__uint_as_float(acc[j]) + __ldg(p.bias + n0 + cb + j));
-                }
-                if (pv) {
-                    if (vec_ok && n0 + cb + 32 <= p.Cout) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4)
-                            *reinterpret_cast<uint4 *>(direct + n0 + cb + j) = make_uint4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (n0 + cb + j < p.Cout) direct[n0 + cb + j] = __uint_as_float(acc[j]);
-                    }
-                }
-                continue;
-            }
-            const int co = n0 + cb + lane;
-            const bool cv = co < p.Cout;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) red[r * 33 + j] = __uint_as_float(acc[j]);
+        for (int ks = 0; ks < 4; ++ks) {               // 4 x (K = 16): +32 bytes inside the 128-byte row
+            mma_ss<NT>(acc, ah + 2 * ks, bh + 2 * ks, 1);
+            mma_ss<NT>(acc, ah + 2 * ks, bl + 2 * ks, 1);
+            mma_ss<NT>(acc, al + 2 * ks, bh + 2 * ks, 1);
+        }
+        commit();
+        wait<1>();                                       // chunk i - 1 is complete: hand its stage back
+        fence_regs(acc);
+        if (i) {
             __syncwarp();
-            const float bias = (p.bias && cv) ? __ldg(p.bias + co) : 0.f;
-            float s1 = 0.f, s2 = 0.f;
-#pragma unroll 4
-            for (int i = 0; i < 32; ++i) {
-                const int row = q4 * 32 + i;
-                const int a = y0 + (row >> bw_shift), b = x0 + (row & bw_mask);
-                if (cv && a < p.Ht && b < p.Wt) {
-                    const float val = red[row * 33 + lane] + bias;
-                    p.out[(((size_t)n * p.OHf + (size_t)(a * p.osy + p.ooy)) * p.OWf + (size_t)(b * p.osx + p.oox)) * p.Cs + p.co_off + co] = val;
-                    s1 += val; s2 = fmaf(val, val, s2);
-                }
-            }
-            __syncwarp();
-            part[(q4 * 32 + lane) * 2] = s1; part[(q4 * 32 + lane) * 2 + 1] = s2;
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (et < 64) {
-                const int j = et >> 1, w = et & 1, c2 = n0 + cb + j;
-                if (c2 < p.Cout) {
-                    const double tot = (double)part[(0 * 32 + j) * 2 + w] + (double)part[(1 * 32 + j) * 2 + w] +
-                                       (double)part[(2 * 32 + j) * 2 + w] + (double)part[(3 * 32 + j) * 2 + w];
-                    atomicAdd(p.stats + ((size_t)n * p.Cout + c2) * 2 + w, tot);
-                }
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            if (lane == 0) mbar_arrive(s32(&bar_empty[(i - 1) % STAGES]));
         }
     }
-    fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TCOLS) : "memory");
+    wait<0>();
+    fence_regs(acc);
+
+    // ---------------------------------------------------------------- epilogue
+    // The accumulator fragment gives a thread 2 pixels x NT / 4 channels; global memory wants a warp on one pixel's
+    // CHANNELS.  Both warpgroups park their fragments in shared memory (the drained stages), then every thread walks the
+    // pixels of one channel: lane = channel, one coalesced 128-byte store per pixel and warp, and the per-channel sums
+    // for the following norm fall out of the same walk.
+    float *tile = reinterpret_cast<float *>(smem_raw + (base - s32(smem_raw)));
+    bar_sync(1, 256);                                    // both warpgroups' wgmmas have drained every stage
+    {
+        const int rf = 64 * g + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+        for (int i = 0; i < NT / 8; ++i) {
+            *reinterpret_cast<float2 *>(tile + rf * LD + 8 * i + cq) = make_float2(acc[4 * i], acc[4 * i + 1]);
+            *reinterpret_cast<float2 *>(tile + (rf + 8) * LD + 8 * i + cq) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+        }
+    }
+    bar_sync(1, 256);
+    const int col = tid % NT, row0 = tid / NT;
+    constexpr int RSTEP = 256 / NT;
+    const int co = blockIdx.y * NT + col;
+    if (co >= p.Cout) return;
+    const bool fin = p.splits == 1;
+    const int bw_shift = 31 - __clz(p.BW), bw_mask = p.BW - 1;
+    const size_t split_stride = (size_t)p.N * p.Ht * p.Wt * p.Cout;
+    const float bias = (fin && p.bias) ? __ldg(p.bias + co) : 0.f;
+    float s1 = 0.f, s2 = 0.f;
+    for (int row = row0; row < 128; row += RSTEP) {
+        const int a = y0 + (row >> bw_shift), b = x0 + (row & bw_mask);
+        if (a >= p.Ht || b >= p.Wt) continue;
+        const float val = tile[row * LD + col] + bias;
+        if (fin) {
+            p.out[(((size_t)n * p.OHf + (size_t)(a * p.osy + p.ooy)) * p.OWf + (size_t)(b * p.osx + p.oox)) * p.Cs + p.co_off + co] = val;
+            s1 += val; s2 = fmaf(val, val, s2);
+        } else {
+            p.partial[(size_t)blockIdx.z * split_stride + (((size_t)n * p.Ht + a) * p.Wt + b) * p.Cout + co] = val;
+        }
+    }
+    if (fin && p.stats) {
+        atomicAdd(p.stats + ((size_t)n * p.Cout + co) * 2, (double)s1);
+        atomicAdd(p.stats + ((size_t)n * p.Cout + co) * 2 + 1, (double)s2);
     }
 }
 

@@ -1,4 +1,4 @@
-// Implicit-GEMM conv2d / conv-transpose2d on tcgen05 (NCHW fp32 in/out, fp32-class accuracy).
+// Implicit-GEMM conv2d / conv-transpose2d on the Hopper tensor cores (wgmma; NCHW fp32 in/out, fp32-class accuracy).
 //
 // Replaces cuDNN in the encoders' heavy layers (reference: lib/net/FBNet.py:216-319 GlobalGenerator /
 // ResnetBlock, lib/net/HGFilters.py + lib/net/net_util.py:258-280 ConvBlock) whenever Cin % 64 == 0.
@@ -7,17 +7,19 @@
 //   k = tap * Cin + ci, so a chunk is one filter tap x 64 consecutive input channels.
 //
 // Same numerics as the occupancy MLP (mlp_tc.cu): activations and weights are split x = hi + lo in fp16
-// and every k-step issues hi*Whi + hi*Wlo + lo*Whi with fp32 accumulation in tensor memory.
-//   warp 0      weight producer: bulk copies of host-packed K-major SWIZZLE_128B tiles (hi | lo), 2-stage ring
-//   warp 1      MMA issuer (tcgen05.mma.cta_group::1.kind::f16, M = 128, N = NT, A operand in TMEM)
-//   warps 2-5   one output pixel (= TMEM lane) per thread: im2col gather of the chunk's 64 input values
-//               (zero / reflection padding, stride, transposed-conv index maps), hi/lo split, tcgen05.st into
-//               a double-buffered A region; afterwards the epilogue (TMEM -> +bias/residual/activation -> NCHW).
+// and every k-step issues hi*Whi + hi*Wlo + lo*Whi with fp32 accumulation in registers.
+//   warps 0-7   two consumer warpgroups, warpgroup g owns pixels [64 g, 64 g + 64) of the tile: im2col gather of the
+//               chunk's input values (two threads per pixel, 32 channels each; zero / reflection padding, stride,
+//               transposed-conv index maps), hi/lo split, SWIZZLE_128B store into the warpgroup's rows of the A tile,
+//               wgmma (M = 64, N = NT) from shared memory; afterwards the epilogue (+bias/residual/activation -> NCHW)
+//               straight from the accumulator fragment.
+//   warps 8-11  weight producer (one lane): bulk copies of host-packed K-major SWIZZLE_128B tiles (hi | lo), 2-stage ring.
 // Small spatial extents (the 32 x 32 ResnetBlocks) are filled across SMs with split-K: partial sums go to a
 // workspace and k_splitk_finish reduces them deterministically.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace icon {
 
@@ -31,81 +33,20 @@ struct ConvTcParams {
     int chunks_total, splits;
 };
 
-constexpr int CT_THREADS = 192;
+constexpr int CT_THREADS = 384;
 
-namespace tc {
-__device__ __forceinline__ uint32_t s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.shared::cta.b64 st, [%0];\n}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n}" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0, spins = 0;
-    while (true) {
-        asm volatile("{\n.reg .pred q;\nmbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\nselp.b32 %0, 1, 0, q;\n}"
-                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (done) break;
-        if (++spins > (1u << 24)) __trap();
-    }
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void mma_ts(uint32_t d, uint32_t a_tmem, uint64_t bd, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n.reg .pred q;\nsetp.ne.b32 q, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, q;\n}" ::"r"(d),
-                 "r"(a_tmem), "l"(bd), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ void ld32(uint32_t addr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,"
-        "%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(addr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void st16(uint32_t addr, const uint32_t (&r)[16]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(addr),
-                 "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-                 "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-__device__ __forceinline__ void split2(float a, float b, uint32_t &hi, uint32_t &lo) {
-    __half2 h = __floats2half2_rn(a, b);
-    float2 hf = __half22float2(h);
-    __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-    hi = *reinterpret_cast<uint32_t *>(&h);
-    lo = *reinterpret_cast<uint32_t *>(&l);
-}
-}  // namespace tc
-
-// grid: (pixel tiles, channel tiles, splits).  TMEM: [0,NT) accumulator, [256,384) two A buffers (hi 32 | lo 32).
+// grid: (pixel tiles, channel tiles, splits).  Shared memory: 2 weight stages (hi NT*128 | lo NT*128), then the A tile
+// (hi 16 KB | lo 16 KB, 128 rows x 128 bytes, SWIZZLE_128B).
 template <int NT>
 __global__ void __launch_bounds__(CT_THREADS, 1) k_conv_tc(ConvTcParams p) {
-    using namespace tc;
+    using namespace wg;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ uint64_t bars[8];
-    __shared__ uint32_t tmem_slot;
-    const uint32_t raw = s32(smem_raw), base = (raw + 1023u) & ~1023u;     // 2 stages x (hi NT*128 | lo NT*128)
+    __shared__ uint64_t bars[4];
+    const uint32_t raw = s32(smem_raw), base = (raw + 1023u) & ~1023u;
+    uint8_t *sm = smem_raw + (base - raw);
     constexpr uint32_t STAGE = NT * 256;
-    enum { B_BFULL0 = 0, B_BFULL1, B_BEMPTY0, B_BEMPTY1, B_AFULL0, B_AFULL1, B_AEMPTY0, B_AEMPTY1 };
-    __shared__ uint64_t bar_acc;
+    constexpr uint32_t A_OFF = 2 * STAGE;
+    enum { B_FULL0 = 0, B_FULL1, B_EMPTY0, B_EMPTY1 };
     auto BAR = [&](int i) { return s32(&bars[i]); };
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
@@ -115,145 +56,136 @@ __global__ void __launch_bounds__(CT_THREADS, 1) k_conv_tc(ConvTcParams p) {
     const int n0 = blockIdx.y * NT;
 
     if (tid == 0) {
-        mbar_init(BAR(B_BFULL0), 1); mbar_init(BAR(B_BFULL1), 1);
-        mbar_init(BAR(B_BEMPTY0), 1); mbar_init(BAR(B_BEMPTY1), 1);
-        mbar_init(BAR(B_AFULL0), 128); mbar_init(BAR(B_AFULL1), 128);
-        mbar_init(BAR(B_AEMPTY0), 1); mbar_init(BAR(B_AEMPTY1), 1);
-        mbar_init(s32(&bar_acc), 1);
+        mbar_init(BAR(B_FULL0), 1); mbar_init(BAR(B_FULL1), 1);
+        mbar_init(BAR(B_EMPTY0), 8); mbar_init(BAR(B_EMPTY1), 8);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(s32(&tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem = tmem_slot;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= 8) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 8 && lane == 0) {
             const uint8_t *src = p.wt + ((size_t)blockIdx.y * p.chunks_total + c_begin) * STAGE;
             for (int c = 0; c < nchunks; ++c) {
                 const uint32_t s = c & 1, ph = (c >> 1) & 1;
-                mbar_wait(BAR(B_BEMPTY0 + s), ph ^ 1);
-                mbar_expect_tx(BAR(B_BFULL0 + s), STAGE);
-                bulk_g2s(base + s * STAGE, src + (size_t)c * STAGE, STAGE, BAR(B_BFULL0 + s));
+                mbar_wait(BAR(B_EMPTY0 + s), ph ^ 1);
+                mbar_expect_tx(BAR(B_FULL0 + s), STAGE);
+                bulk_g2s(base + s * STAGE, src + (size_t)c * STAGE, STAGE, BAR(B_FULL0 + s));
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(NT >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            for (int c = 0; c < nchunks; ++c) {
-                const uint32_t s = c & 1, ph = (c >> 1) & 1;
-                mbar_wait(BAR(B_AFULL0 + s), ph);
-                mbar_wait(BAR(B_BFULL0 + s), ph);
-                fence_after();
-                const uint32_t a_hi = tmem + 256 + 64u * s, a_lo = a_hi + 32;
-                const uint64_t bh = desc_sw128(base + s * STAGE), bl = desc_sw128(base + s * STAGE + NT * 128);
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {
-                    mma_ts(tmem, a_hi + 8 * ks, bh + 2 * ks, IDESC, (c | ks) != 0);
-                    mma_ts(tmem, a_hi + 8 * ks, bl + 2 * ks, IDESC, 1);
-                    mma_ts(tmem, a_lo + 8 * ks, bh + 2 * ks, IDESC, 1);
-                }
-                commit(BAR(B_BEMPTY0 + s));
-                commit(BAR(B_AEMPTY0 + s));
-            }
-            commit(s32(&bar_acc));
-        }
-    } else {
-        // ---------------------------------------------------- gather + epilogue: one output pixel per thread
-        const int q4 = warp & 3;
-        const int r = q4 * 32 + lane;
-        const uint32_t tl = tmem + ((uint32_t)(q4 * 32) << 16);
-        const int64_t npix = (int64_t)p.N * p.OH * p.OW;
-        const int64_t gp = (int64_t)blockIdx.x * 128 + r;
-        const bool pv = gp < npix;
-        int pn = 0, oy = 0, ox = 0;
-        if (pv) {
-            pn = (int)(gp / ((int64_t)p.OH * p.OW));
-            const int rem = (int)(gp % ((int64_t)p.OH * p.OW));
-            oy = rem / p.OW; ox = rem % p.OW;
-        }
-        const size_t plane = (size_t)p.H * p.W;
-        const float *xn = p.x + (size_t)pn * p.Cin * plane;
-        const int cpt = p.Cin / 64;                          // chunks per tap
-        for (int c = 0; c < nchunks; ++c) {
-            const uint32_t s = c & 1, ph = (c >> 1) & 1;
-            const int ck = c_begin + c, tap = ck / cpt, ci0 = (ck % cpt) * 64;
-            const int kh = tap / p.KW, kw = tap % p.KW;
-            int iy, ix;
-            bool ok = pv;
-            if (!p.transposed) {
-                iy = oy * p.stride - p.pad + kh;
-                ix = ox * p.stride - p.pad + kw;
-                if (p.reflect) {
-                    iy = iy < 0 ? -iy : (iy >= p.H ? 2 * p.H - 2 - iy : iy);
-                    ix = ix < 0 ? -ix : (ix >= p.W ? 2 * p.W - 2 - ix : ix);
-                } else ok = ok && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-            } else {
-                const int ty2 = oy + p.pad - kh, tx2 = ox + p.pad - kw;
-                ok = ok && ty2 >= 0 && tx2 >= 0 && (ty2 % p.stride) == 0 && (tx2 % p.stride) == 0;
-                iy = ty2 / p.stride; ix = tx2 / p.stride;
-                ok = ok && iy < p.H && ix < p.W;
-            }
-            uint32_t hi[32], lo[32];
-            if (ok) {
-                const float *src = xn + (size_t)ci0 * plane + (size_t)iy * p.W + ix;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float a = __ldg(src + (size_t)(2 * j) * plane), b = __ldg(src + (size_t)(2 * j + 1) * plane);
-                    split2(a, b, hi[j], lo[j]);
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) { hi[j] = 0u; lo[j] = 0u; }
-            }
-            mbar_wait(BAR(B_AEMPTY0 + s), ph ^ 1);
-            fence_after();
-            const uint32_t a0 = tl + 256 + 64u * s;
-            st16(a0, reinterpret_cast<const uint32_t(&)[16]>(hi[0]));
-            st16(a0 + 16, reinterpret_cast<const uint32_t(&)[16]>(hi[16]));
-            st16(a0 + 32, reinterpret_cast<const uint32_t(&)[16]>(lo[0]));
-            st16(a0 + 48, reinterpret_cast<const uint32_t(&)[16]>(lo[16]));
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            fence_before();
-            mbar_arrive(BAR(B_AFULL0 + s));
-        }
-        // ---- epilogue
-        mbar_wait(s32(&bar_acc), 0);
-        fence_after();
-        const size_t ohw = (size_t)p.OH * p.OW;
-        float *yb = p.y + (p.splits > 1 ? (size_t)blockIdx.z * p.N * p.Cout * ohw : 0);
-        const bool fin = p.splits == 1;
-        for (int cb = 0; cb < NT; cb += 32) {
-            uint32_t acc[32];
-            ld32(tl + cb, acc);
-            if (pv) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int co = n0 + cb + j;
-                    if (co < p.Cout) {
-                        const size_t o = ((size_t)pn * p.Cout + co) * ohw + (size_t)oy * p.OW + ox;
-                        float v = nchunks > 0 ? __uint_as_float(acc[j]) : 0.f;
-                        if (fin) {
-                            if (p.bias) v += __ldg(p.bias + co);
-                            if (p.res) v += p.res[o];
-                            if (p.act == 1) v = fmaxf(v, 0.f);
-                            else if (p.act == 2) v = tanhf(v);
-                        }
-                        yb[o] = v;
-                    }
-                }
-            }
-        }
+        return;
     }
-    fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+
+    // ---------------------------------------------------- consumers
+    const int g = warp >> 2, tw = tid & 127;
+    const int r = 64 * g + (tw & 63), half = tw >> 6;            // gather: pixel r of the tile, channels [32 half, +32)
+    const int64_t npix = (int64_t)p.N * p.OH * p.OW;
+    const int64_t ohw = (int64_t)p.OH * p.OW;
+    int pn = 0, oy = 0, ox = 0;
+    const int64_t gp = (int64_t)blockIdx.x * 128 + r;
+    const bool pv = gp < npix;
+    if (pv) {
+        pn = (int)(gp / ohw);
+        const int rem = (int)(gp % ohw);
+        oy = rem / p.OW; ox = rem % p.OW;
+    }
+    const size_t plane = (size_t)p.H * p.W;
+    const float *xn = p.x + (size_t)pn * p.Cin * plane;
+    const int cpt = p.Cin / 64;                          // chunks per tap
+    const uint32_t a_hi = base + A_OFF, a_lo = a_hi + 16384;
+    const uint64_t dah = desc_sw128(a_hi + g * 8192), dal = desc_sw128(a_lo + g * 8192);
+    float acc[NT / 2];
+#pragma unroll
+    for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
+    for (int c = 0; c < nchunks; ++c) {
+        const uint32_t s = c & 1, ph = (c >> 1) & 1;
+        const int ck = c_begin + c, tap = ck / cpt, ci0 = (ck % cpt) * 64 + 32 * half;
+        const int kh = tap / p.KW, kw = tap % p.KW;
+        int iy, ix;
+        bool ok = pv;
+        if (!p.transposed) {
+            iy = oy * p.stride - p.pad + kh;
+            ix = ox * p.stride - p.pad + kw;
+            if (p.reflect) {
+                iy = iy < 0 ? -iy : (iy >= p.H ? 2 * p.H - 2 - iy : iy);
+                ix = ix < 0 ? -ix : (ix >= p.W ? 2 * p.W - 2 - ix : ix);
+            } else ok = ok && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
+        } else {
+            const int ty2 = oy + p.pad - kh, tx2 = ox + p.pad - kw;
+            ok = ok && ty2 >= 0 && tx2 >= 0 && (ty2 % p.stride) == 0 && (tx2 % p.stride) == 0;
+            iy = ty2 / p.stride; ix = tx2 / p.stride;
+            ok = ok && iy < p.H && ix < p.W;
+        }
+        uint32_t hi[16], lo[16];
+        if (ok) {
+            const float *src = xn + (size_t)ci0 * plane + (size_t)iy * p.W + ix;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const float a = __ldg(src + (size_t)(2 * j) * plane), b = __ldg(src + (size_t)(2 * j + 1) * plane);
+                split2(a, b, hi[j], lo[j]);
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) { hi[j] = 0u; lo[j] = 0u; }
+        }
+        if (c) {                                          // chunk c - 1 has finished reading the A tile and its stage
+            wait<0>();
+            fence_regs(acc);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(BAR(B_EMPTY0 + (s ^ 1)));
+        }
+        bar_sync(1 + g, 128);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {                     // 16-byte chunks 4 half + q of row r, XOR-swizzled by r % 8
+            const uint32_t o = (uint32_t)r * 128 + (uint32_t)(((4 * half + q) ^ (r & 7)) * 16);
+            *reinterpret_cast<uint4 *>(sm + A_OFF + o) = make_uint4(hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]);
+            *reinterpret_cast<uint4 *>(sm + A_OFF + 16384 + o) = make_uint4(lo[4 * q], lo[4 * q + 1], lo[4 * q + 2], lo[4 * q + 3]);
+        }
+        fence_proxy_async();
+        bar_sync(1 + g, 128);
+        mbar_wait(BAR(B_FULL0 + s), ph);
+        const uint64_t bh = desc_sw128(base + s * STAGE), bl = desc_sw128(base + s * STAGE + NT * 128);
+        fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {               // 4 x (K = 16): +32 bytes inside the 128-byte row
+            mma_ss<NT>(acc, dah + 2 * ks, bh + 2 * ks, 1);
+            mma_ss<NT>(acc, dah + 2 * ks, bl + 2 * ks, 1);
+            mma_ss<NT>(acc, dal + 2 * ks, bh + 2 * ks, 1);
+        }
+        commit();
+    }
+    wait<0>();
+    fence_regs(acc);
+
+    // ---- epilogue from the accumulator fragment: rows rf, rf + 8, columns 8 i + cq + (0, 1)
+    const int rf = 64 * g + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+    float *yb = p.y + (p.splits > 1 ? (size_t)blockIdx.z * p.N * p.Cout * ohw : 0);
+    const bool fin = p.splits == 1;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+        const int64_t gq = (int64_t)blockIdx.x * 128 + rf + 8 * hr;
+        if (gq >= npix) continue;
+        const int qn = (int)(gq / ohw);
+        const int64_t pix = gq % ohw;
+#pragma unroll
+        for (int i = 0; i < NT / 8; ++i) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int co = n0 + 8 * i + cq + e;
+                if (co < p.Cout) {
+                    const size_t o = ((size_t)qn * p.Cout + co) * ohw + pix;
+                    float v = acc[4 * i + 2 * hr + e];
+                    if (fin) {
+                        if (p.bias) v += __ldg(p.bias + co);
+                        if (p.res) v += p.res[o];
+                        if (p.act == 1) v = fmaxf(v, 0.f);
+                        else if (p.act == 2) v = tanhf(v);
+                    }
+                    yb[o] = v;
+                }
+            }
+        }
     }
 }
 
@@ -275,7 +207,7 @@ __global__ void k_splitk_finish(const float *__restrict__ part, int splits, cons
 template <int NT>
 static int launch_conv_tc(const ConvTcParams &p, dim3 grid, cudaStream_t stream) {
     static bool attr_set[ICON_MAX_DEVICES] = {};
-    const int smem = 2 * NT * 256 + 1024;
+    const int smem = 2 * NT * 256 + 32768 + 1024;
     if (device_needs_setup(attr_set))
         ICON_CUDA(cudaFuncSetAttribute(k_conv_tc<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     k_conv_tc<NT><<<grid, CT_THREADS, smem, stream>>>(p);

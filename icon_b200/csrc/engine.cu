@@ -300,7 +300,7 @@ extern "C" int icon_grid_count_above(const float *occ, int64_t n, float balance,
     ICON_CHECK_ARG(occ && d_count && n >= 0, "icon_grid_count_above: bad argument");
     ICON_CUDA(cudaMemsetAsync(d_count, 0, sizeof(int64_t), stream));
     if (n == 0) return ICON_OK;
-    unsigned nb = (unsigned)min((int64_t)148 * 8, (n + 255) / 256);
+    unsigned nb = (unsigned)min((int64_t)device_sm_count() * 8, (n + 255) / 256);
     k_count_above<<<nb, 256, 0, stream>>>(occ, n, balance, (unsigned long long *)d_count);
     ICON_LAUNCHED();
     return ICON_OK;

@@ -309,13 +309,13 @@ static int g_mlp_impl = 1;
 template <int MODE>
 static int launch_any(const QueryParams &q, const void *tc, cudaStream_t stream) {
     if (g_mlp_impl == 1) {
-        if (!tc) {          // never degrade silently to the 10x slower FP32 kernel: the caller asked for tcgen05
-            set_error("icon_query / icon_mlp_only: the tcgen05 MLP needs the packed tensor-core weight blob (mlp_tc == NULL); "
+        if (!tc) {          // never degrade silently to the 10x slower FP32 kernel: the caller asked for the tensor cores
+            set_error("icon_query / icon_mlp_only: the tensor-core MLP needs the packed tensor-core weight blob (mlp_tc == NULL); "
                       "pass it or select the FP32 kernel with icon_set_mlp_impl(0)");
             return ICON_EINVAL;
         }
         if (q.c0 > 15) {    // x0 column 15 is the constant 1 that carries the folded biases
-            set_error("icon_query / icon_mlp_only: the tcgen05 MLP takes c0 <= 15 input channels (got %d)", q.c0);
+            set_error("icon_query / icon_mlp_only: the tensor-core MLP takes c0 <= 15 input channels (got %d)", q.c0);
             return ICON_EINVAL;
         }
         return launch_mlp_tc(MODE, q, tc, stream);
@@ -433,7 +433,7 @@ extern "C" int icon_query(int prior, const float *points, int64_t stride_c, int6
 }
 
 extern "C" int icon_set_mlp_impl(int impl) {
-    ICON_CHECK_ARG(impl == 0 || impl == 1, "icon_set_mlp_impl: 0 (fp32) or 1 (tcgen05)");
+    ICON_CHECK_ARG(impl == 0 || impl == 1, "icon_set_mlp_impl: 0 (fp32) or 1 (tensor cores)");
     g_mlp_impl = impl;
     return ICON_OK;
 }

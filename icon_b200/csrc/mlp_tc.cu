@@ -1,51 +1,39 @@
-// Fused feature gather + occupancy MLP on the 5th-generation tensor cores (tcgen05 / TMEM).
+// Fused feature gather + occupancy MLP on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Same contract as mlp.cu (reference: lib/net/MLP.py:49-72, lib/net/geometry.py:21-43,
 // lib/dataset/mesh_util.py:266-277, lib/net/HGPIFuNet.py:298-311, 335-363).
 //
 // Precision: every layer input x is split x = hi + lo with hi = fp16(x), lo = fp16(x - hi) (22
 // significant bits), the BN-folded weights likewise on the host, and each layer is evaluated as
-// hi*Whi + hi*Wlo + lo*Whi with fp32 accumulation in tensor memory -- three kind::f16 MMAs per
-// k-step, fp32-class accuracy (parity bar 1e-4 on the logit; measured error in DESIGN.md).
+// hi*Whi + hi*Wlo + lo*Whi with fp32 accumulation -- three f16 wgmmas per k-step, fp32-class accuracy
+// (parity bar 1e-4 on the logit).
 //
-// One persistent CTA per SM, 128 query points (= 128 TMEM lanes) per tile, 576 threads (18 warps):
-//   warp 0      weight producer: 1-D bulk copies (cp.async.bulk, TMA engine) of host-pre-swizzled
-//               K-major SWIZZLE_128B tiles from L2 into a 2 x 64 KB ring, mbarrier complete_tx
-//               (per tile: 8 layer-1 K-chunks and 2 pairs of layer-2 K-chunks; layer 0 and the x0 tail of
-//               layer 2 stay resident in shared memory)
-//   warp 1      MMA issuer, all 32 lanes converged, tcgen05.mma.cta_group::1.kind::f16 M=128 under elect.sync
-//               (operands in uniform registers); the barriers of chunk j+1 are checked while chunk j still has
-//               MMAs to issue, so the tensor pipe never drains between chunks
-//   warps 2-9   workers, one TMEM lane (= query point) per thread, two threads per lane:
-//               per 64-column chunk of layer 0: tcgen05.ld -> LeakyReLU -> hi/lo fp16 -> tcgen05.st as the A
-//               operand (in TMEM) of layer 1 (b0 is already in the accumulator: x0 column 15 is the constant 1 and
-//               row 15 of W0 holds b0); same with + b1 for layer 1 -> layer 2 (in 4 K-chunks so layer 2 starts
-//               early).  They go straight on to the next tile.
-//   warps 10-13 gather + epilogue, one query point per thread: the 16 input features of tile i+1 (bilinear /
-//               trilinear samples, SMPL record, outlier rule) are produced and published as the double-buffered
-//               x0 operand while tile i is in the tensor pipe; then layer 3 (141 -> 1) of tile i as an fp32 dot
-//               over columns 0..63 of the layer-2 accumulator (b2 included, through the same constant-1 column
-//               in the x0 tail), off the critical path of the next tile (which only waits until the accumulator
-//               has been read); they sleep EPI_YIELD_NS after that read: the MMA warp and the next tile's first
-//               conversion need the issue slots more.
-//   warps 14-17 layer 3 over columns 64..127, partial sums handed to warps 10-13 through shared memory.
-// Layer-0 chunks are issued two ahead of the layer-1 chunk that consumes them, so the tensor pipe
-// always has queued work while the workers convert.  TMEM map (512 columns):
-//   [0,256) layer-1 accumulator (later [0,128) layer-2 accumulator)
-//   [256,384) 2 x (hi 32 | lo 32) A-operand chunks of layer 1   } later: layer-1 activations
-//   [384,512) 2 x 64 layer-0 accumulator chunks                 } hi [256,384), lo [384,512)
-// Where the cycles of a tile go was measured with tools/mlp_timeline.py (profiles/r2_summary.md).
-// Operand layouts were verified on hardware with tools/umma_probe.cu.
+// One persistent CTA per SM, 128 query points per tile, 384 threads (3 warpgroups):
+//   warps 0-7   two consumer warpgroups, warpgroup g owns rows [64 g, 64 g + 64) of the tile.  Per tile:
+//               gather (threads 0..63 of the warpgroup, one point each: bilinear / trilinear samples, SMPL
+//               record, outlier rule) -> x0 operand (fp16 hi / lo, shared memory; column 15 is the constant 1
+//               that carries b0 and b2) -> for each half h of layer 1's 256 outputs: 8 x (layer-0 chunk of 64
+//               outputs, wgmma from shared memory -> LeakyReLU -> hi / lo register fragments -> layer-1 K-chunk
+//               with A from registers, N = 128) -> LeakyReLU(+ b1) of the half -> its two layer-2 K-chunks (A
+//               from registers, N = 128) -> x0 tail of layer 2 -> layer 3 (144 -> 1) as an fp32 dot over the
+//               accumulator fragment, reduced across the 4 lanes that share a row.  Layer 0 is recomputed for
+//               the second half: 16 of 174 k MACs per point, and it keeps the live accumulators at 160 registers.
+//   warps 8-11  weight producer (warp 8, one lane; the warpgroup hands its registers to the consumers with setmaxnreg): 1-D bulk copies (cp.async.bulk, TMA engine) of host-pre-swizzled K-major SWIZZLE_128B
+//               tiles from L2 into a 4 x 32 KB ring, mbarrier complete_tx (per tile 16 half-chunks of layer 1 and 4
+//               chunks of layer 2; layer 0, the x0 tail of layer 2 and the fp32 tail stay resident).
 #include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "query_common.cuh"
+#include "wgmma.cuh"
 
 namespace icon {
 
-constexpr int TC_THREADS = 576;      // 1 producer + 1 MMA + 8 worker + 4 gather/epilogue + 4 epilogue warps
+constexpr int TC_THREADS = 384;      // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int TC_M = 128;
-constexpr unsigned EPI_YIELD_NS = 1200;  // epilogue warps sleep this long after reading the layer-2 accumulator (measured: tools/mlp_timeline.py)
+constexpr int NSTAGE = 4;            // weight ring depth
+constexpr int STAGE_BYTES = 32768;   // one SW128 operand of 128 rows x 64 k, hi | lo
+constexpr int STAGES_PER_TILE = 20;
 
 // byte offsets inside the packed tensor-core weight blob (host: icon_b200/ops.py pack_mlp)
 constexpr int TCB_W0 = 0;                         // hi 16384 | lo 16384, no swizzle, LBO 8192, SBO 128
@@ -58,153 +46,45 @@ constexpr int TCB_BYTES = TCB_F32 + TCB_F32_FLOATS * 4;
 static_assert(TCB_BYTES == ICON_MLP_TC_BYTES, "blob layout");
 
 // shared memory map (bytes from a 1024-aligned base)
-constexpr int SM_STAGE = 0;                       // 2 x 65536
-constexpr int SM_W0 = 131072;                     // 32768
-constexpr int SM_X0H = SM_W0 + 32768;             // 2 x 4096  A tile of x0 (hi), no swizzle, LBO 2048, SBO 128
-constexpr int SM_X0L = SM_X0H + 8192;             // 2 x 4096
-constexpr int SM_X0F = SM_X0L + 8192;             // 2 x [16][128] fp32
-constexpr int SM_F32 = SM_X0F + 2 * 8192;         // biases etc.
-constexpr int SM_W2T = (SM_F32 + TCB_F32_FLOATS * 4 + 127) / 128 * 128;   // 8192: x0 tail of layer 2 (hi 4096 | lo 4096), resident
-constexpr int SM_PART = SM_W2T + 8192;            // 2 x [128] fp32 layer-3 partials (columns 64..127)
-constexpr int SM_BAR = SM_PART + 1024;            // 24 mbarriers
-constexpr int SM_MISC = SM_BAR + 24 * 8;
-constexpr int SM_TOTAL = SM_MISC + 64;
+constexpr int SM_STAGE = 0;                       // NSTAGE x 32768
+constexpr int SM_W0 = NSTAGE * STAGE_BYTES;       // 32768
+constexpr int SM_X0H = SM_W0 + 32768;             // 4096  A tile of x0 (hi), no swizzle, LBO 2048, SBO 128
+constexpr int SM_X0L = SM_X0H + 4096;             // 4096
+constexpr int SM_X0F = SM_X0L + 4096;             // [16][128] fp32 (layer 3 skip connection, row 15 = in_cube)
+constexpr int SM_F32 = SM_X0F + 8192;             // biases etc.
+constexpr int SM_W2T = (SM_F32 + TCB_F32_FLOATS * 4 + 127) / 128 * 128;   // x0 tail of layer 2 (hi 4096 | lo 4096)
+constexpr int SM_BAR = SM_W2T + 8192;
+constexpr int SM_TOTAL = SM_BAR + (2 * NSTAGE + 1) * 8;
 constexpr int TC_SMEM_BYTES = SM_TOTAL + 1024;    // slack for manual 1024-B alignment
+static_assert(TC_SMEM_BYTES <= 227 * 1024, "shared memory");
 
-enum { B_WFULL0 = 0, B_WFULL1, B_WEMPTY0, B_WEMPTY1, B_X0R0, B_X0R1, B_ACC2E, B_SPARE, B_ACC0F0, B_ACC0F1, B_A0F0, B_A0F1,
-       B_A0E0, B_A0E1, B_ACC1, B_ACT1_0, B_ACT1_1, B_ACT1_2, B_ACT1_3, B_ACC2, B_W0RDY };
+enum { B_FULL0 = 0, B_EMPTY0 = NSTAGE, B_W0RDY = 2 * NSTAGE };
 
-// TMEM columns
-constexpr uint32_t T_ACC1 = 0, T_A0 = 256, T_ACC0 = 384, T_ACT1H = 256, T_ACT1L = 384, T_ACC2 = 0;
-
-// ---------------------------------------------------------------- PTX helpers
-__device__ __forceinline__ uint32_t s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.shared::cta.b64 st, [%0];\n}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n}" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    uint32_t spins = 0;
-    while (true) {
-        asm volatile("{\n.reg .pred q;\nmbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\nselp.b32 %0, 1, 0, q;\n}"
-                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (done) break;
-        if (++spins > (1u << 24)) __trap();     // a protocol bug must fail, not hang the GPU (a deadlocked kernel sat 400 s at 1 << 27)
-    }
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                 "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// One lane of a CONVERGED warp.  The MMA warp runs its whole loop on all 32 lanes and predicates only the tcgen05
-// instructions with this: their operands then stay in uniform registers.  (Issuing from inside `if (lane == 0)` made ptxas
-// build every descriptor in vector registers and wrap each UTCHMMA in an ELECT / R2UR.BROADCAST / BRA.U.ANY waterfall:
-// ~90 clocks per issue against 32-128 clocks of execution, measured with tools/mlp_timeline.py.)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t p;
-    asm volatile("{\n.reg .pred q;\nelect.sync _|q, 0xffffffff;\nselp.b32 %0, 1, 0, q;\n}" : "=r"(p));
-    return p != 0;
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void mma_ss(uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n.reg .pred q;\nsetp.ne.b32 q, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, q;\n}" ::"r"(d),
-                 "l"(ad), "l"(bd), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void mma_ts(uint32_t d, uint32_t a_tmem, uint64_t bd, uint32_t idesc, uint32_t acc) {
-    asm volatile("{\n.reg .pred q;\nsetp.ne.b32 q, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, q;\n}" ::"r"(d),
-                 "r"(a_tmem), "l"(bd), "r"(idesc), "r"(acc) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t addr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,"
-        "%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(addr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t addr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,"
-        "%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(addr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st16(uint32_t addr, const uint32_t (&r)[16]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(addr),
-                 "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-                 "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// descriptors (tools/umma_probe.cu)
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {      // K-major, SWIZZLE_128B, SBO = 1024 B
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)2 << 61);
-}
-__device__ __forceinline__ uint64_t desc_nosw(uint32_t saddr, uint32_t lbo, uint32_t sbo) {   // K-major, no swizzle
-    return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) |
-           ((uint64_t)1 << 46);
-}
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N) {     // A = B = F16, D = F32, both K-major
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// x -> (hi, lo) fp16 pairs for two values
-__device__ __forceinline__ void split2(float a, float b, uint32_t &hi, uint32_t &lo) {
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
-    float2 hf = __half22float2(h);
-    __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-    hi = *reinterpret_cast<uint32_t *>(&h);
-    lo = *reinterpret_cast<uint32_t *>(&l);
+    return *reinterpret_cast<uint32_t *>(&h);
 }
 
-// [bias +] LeakyReLU + split of 32 accumulator values -> 16 hi words + 16 lo words (bias == nullptr: already in the
-// accumulator, folded into the MMA through the constant-1 input column)
-__device__ __forceinline__ void act_split32(const uint32_t (&acc)[32], const float *__restrict__ bias, uint32_t (&hi)[16],
-                                            uint32_t (&lo)[16]) {
+// LeakyReLU(d + bias) of 4 k-steps (64 columns) of an accumulator fragment -> hi / lo register A fragments.
+// d points at the fragment of the chunk's first 8-column block; bias (or null) at the chunk's column 2 (lane % 4).
+__device__ __forceinline__ void act_frag64(const float *d, const float *bias, uint32_t (&ah)[4][4], uint32_t (&al)[4][4]) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 4) {
-        float4 b = bias ? *reinterpret_cast<const float4 *>(bias + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-        float v0 = __uint_as_float(acc[i]) + b.x, v1 = __uint_as_float(acc[i + 1]) + b.y;
-        float v2 = __uint_as_float(acc[i + 2]) + b.z, v3 = __uint_as_float(acc[i + 3]) + b.w;
-        v0 = fmaxf(v0, 0.01f * v0); v1 = fmaxf(v1, 0.01f * v1);
-        v2 = fmaxf(v2, 0.01f * v2); v3 = fmaxf(v3, 0.01f * v3);
-        split2(v0, v1, hi[i / 2], lo[i / 2]);
-        split2(v2, v3, hi[i / 2 + 1], lo[i / 2 + 1]);
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {            // q: (row, row + 8) x (cols 0..7, 8..15) in fragment order
+            const int nb = 2 * kk + (q >> 1), e = 4 * nb + 2 * (q & 1);
+            float v0 = d[e], v1 = d[e + 1];
+            if (bias) { v0 += bias[8 * nb]; v1 += bias[8 * nb + 1]; }
+            v0 = fmaxf(v0, 0.01f * v0); v1 = fmaxf(v1, 0.01f * v1);
+            wg::split2(v0, v1, ah[kk][q], al[kk][q]);
+        }
     }
 }
-
-#ifdef ICON_MLP_TIMELINE
-// diagnostics build only (tools/mlp_timeline.py): SM-clock stamps of one tile of one CTA
-__device__ long long g_tl[256];
-#define TL(slot) do { if (blockIdx.x == 3 && tcount == 6) g_tl[slot] = clock64(); } while (0)
-#else
-#define TL(slot) do { } while (0)
-#endif
 
 // MODE: 0 icon, 1 pifu, 2 pamir, 3 raw feature matrix
 template <int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, const uint8_t *__restrict__ blob) {
+    using namespace wg;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = s32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -212,239 +92,73 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
     float *x0f = reinterpret_cast<float *>(sm + SM_X0F);
     const float *sf32 = reinterpret_cast<const float *>(sm + SM_F32);
     const float *sb1 = sf32 + 512, *sw3 = sf32 + 896, *sb3 = sf32 + 1040;     // b0 [0,512) and b2 [768,896) ride in the weight tiles
-    float *spart = reinterpret_cast<float *>(sm + SM_PART);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(sm + SM_MISC);
     const uint32_t bar0 = base + SM_BAR;
     auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int64_t ntiles = (q.N + TC_M - 1) / TC_M;
 
-    // ------------------------------------------------------------ one-time setup
     if (tid == 0) {
-        mbar_init(BAR(B_WFULL0), 1); mbar_init(BAR(B_WFULL1), 1);
-        mbar_init(BAR(B_WEMPTY0), 1); mbar_init(BAR(B_WEMPTY1), 1);
-        mbar_init(BAR(B_X0R0), 128); mbar_init(BAR(B_X0R1), 128);      // gather warps -> MMA
-        mbar_init(BAR(B_ACC2E), 256); mbar_init(BAR(B_SPARE), 1);     // epilogue: layer-2 accumulator has been read
-        mbar_init(BAR(B_ACC0F0), 1); mbar_init(BAR(B_ACC0F1), 1);
-        mbar_init(BAR(B_A0F0), 256); mbar_init(BAR(B_A0F1), 256);
-        mbar_init(BAR(B_A0E0), 1); mbar_init(BAR(B_A0E1), 1);
-        mbar_init(BAR(B_ACC1), 1); mbar_init(BAR(B_ACC2), 1);
-        for (int c = 0; c < 4; ++c) mbar_init(BAR(B_ACT1_0 + c), 256);
+        for (int s = 0; s < NSTAGE; ++s) { mbar_init(BAR(B_FULL0 + s), 1); mbar_init(BAR(B_EMPTY0 + s), 8); }
         mbar_init(BAR(B_W0RDY), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(s32(tmem_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp >= 8) {
         // ======================================================== weight producer
-        if (lane == 0) {
-            // resident: W0 (hi | lo) and the fp32 tail (biases, last layer)
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 8 && lane == 0) {
             mbar_expect_tx(BAR(B_W0RDY), 32768 + TCB_F32_FLOATS * 4 + 8192);
             bulk_g2s(base + SM_W0, blob + TCB_W0, 32768, BAR(B_W0RDY));
             bulk_g2s(base + SM_F32, blob + TCB_F32, TCB_F32_FLOATS * 4, BAR(B_W0RDY));
             bulk_g2s(base + SM_W2T, blob + TCB_W2T, 8192, BAR(B_W0RDY));
             uint32_t cnt = 0;
             for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                for (int i = 0; i < 10; ++i) {           // 8 K-chunks of layer 1, then layer 2 two K-chunks at a time
-                    const uint32_t s = cnt & 1, ph = (cnt >> 1) & 1;
-                    mbar_wait(BAR(B_WEMPTY0 + s), ph ^ 1);
-                    const uint8_t *src = i < 8 ? blob + TCB_W1 + (size_t)i * 65536 : blob + TCB_W2 + (size_t)(i - 8) * 65536;
-                    mbar_expect_tx(BAR(B_WFULL0 + s), 65536);
-                    bulk_g2s(base + SM_STAGE + s * 65536, src, 65536, BAR(B_WFULL0 + s));
-                    ++cnt;
+                // consumption order: layer-1 rows [0,128) chunks 0..7, layer-2 chunks 0, 1, rows [128,256), chunks 2, 3
+                for (int i = 0; i < STAGES_PER_TILE; ++i, ++cnt) {
+                    const uint32_t s = cnt % NSTAGE, ph = (cnt / NSTAGE) & 1;
+                    mbar_wait(BAR(B_EMPTY0 + s), ph ^ 1);
+                    const uint32_t dst = base + SM_STAGE + s * STAGE_BYTES, full = BAR(B_FULL0 + s);
+                    mbar_expect_tx(full, STAGE_BYTES);
+                    const int h = i < 10 ? 0 : 1, k = i - 10 * h;
+                    if (k < 8) {
+                        const uint8_t *src = blob + TCB_W1 + (size_t)k * 65536 + h * 16384;
+                        bulk_g2s(dst, src, 16384, full);
+                        bulk_g2s(dst + 16384, src + 32768, 16384, full);
+                    } else {
+                        bulk_g2s(dst, blob + TCB_W2 + (size_t)(2 * h + k - 8) * 32768, 32768, full);
+                    }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ======================================================== MMA issuer (all 32 lanes converged; see elect_one)
-        {
-            constexpr uint32_t ID64 = idesc_f16(128, 64), ID256 = idesc_f16(128, 256), ID128 = idesc_f16(128, 128);
-            const uint32_t tm = __shfl_sync(0xffffffffu, tmem, 0);      // provably warp-uniform
-            const uint64_t dx0h0 = desc_nosw(base + SM_X0H, 2048, 128), dx0l0 = desc_nosw(base + SM_X0L, 2048, 128);
-            const uint64_t dw0h = desc_nosw(base + SM_W0, 8192, 128), dw0l = desc_nosw(base + SM_W0 + 16384, 8192, 128);
-            uint32_t ph_x0 = 0, ph_a0f = 0, ph_act1 = 0, cnt = 0, tcount = 0;     // per-buffer phase bits
-            mbar_wait(BAR(B_W0RDY), 0);
-            auto L0 = [&](int j, uint32_t xb, uint32_t dcol) {          // layer-0 chunk j of the tile whose x0 is in buffer xb
-                const uint32_t d = tm + dcol;
-                const uint64_t ah = dx0h0 + (uint64_t)(xb * 256), al = dx0l0 + (uint64_t)(xb * 256);     // 4096 B = 256 units
-                const uint64_t o = (uint64_t)(j * 64);              // 64 rows = 8 groups x 128 B = 1024 B -> 64 units
-                if (elect_one()) {
-                    mma_ss(d, ah, dw0h + o, ID64, 0);
-                    mma_ss(d, ah, dw0l + o, ID64, 1);
-                    mma_ss(d, al, dw0h + o, ID64, 1);
-                    tc_commit(BAR(B_ACC0F0 + (j & 1)));
-                }
-                __syncwarp();
-            };
-            for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tcount) {
-                const uint32_t xb = tcount & 1;
-                if (lane == 0) TL(0);
-                mbar_wait(BAR(B_X0R0 + xb), (ph_x0 >> xb) & 1); ph_x0 ^= 1u << xb;
-                tc_fence_after();
-                L0(0, xb, T_ACC0);                  // [384,512) was ACT1L of the previous tile: its layer-2 MMAs are ahead in the pipe
-                L0(1, xb, T_ACC0 + 64);
-                uint32_t s_cur = 0, s_nxt = 0;
-                auto wait_a0 = [&](int j) {
-                    const int b = j & 1;
-                    mbar_wait(BAR(B_A0F0 + b), (ph_a0f >> b) & 1); ph_a0f ^= 1u << b;
-                    if (lane == 0) TL(32 + j);
-                };
-                auto wait_w = [&](int slot) {
-                    s_nxt = cnt & 1;
-                    mbar_wait(BAR(B_WFULL0 + s_nxt), (cnt >> 1) & 1); ++cnt;
-                    tc_fence_after();
-                    if (lane == 0) TL(slot);
-                };
-                auto l1_ks = [&](int j, int ks0, int ks1) {
-                    const int b = j & 1;
-                    const uint32_t a_hi = tm + T_A0 + 64u * b, a_lo = a_hi + 32;
-                    const uint64_t bh = desc_sw128(base + SM_STAGE + s_cur * 65536), bl = desc_sw128(base + SM_STAGE + s_cur * 65536 + 32768);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int ks = ks0; ks < ks1; ++ks) {
-                            mma_ts(tm + T_ACC1, a_hi + 8 * ks, bh + 2 * ks, ID256, (j | ks) != 0);
-                            mma_ts(tm + T_ACC1, a_hi + 8 * ks, bl + 2 * ks, ID256, 1);
-                            mma_ts(tm + T_ACC1, a_lo + 8 * ks, bh + 2 * ks, ID256, 1);
-                        }
-                        if (ks1 == 4) {
-                            tc_commit(BAR(B_WEMPTY0 + s_cur));
-                            tc_commit(BAR(B_A0E0 + b));
-                        }
-                    }
-                    __syncwarp();
-                };
-                auto l2_ks = [&](int c, int ks0, int ks1) {              // a weight stage holds K-chunks (c & ~1, c | 1)
-                    const uint32_t wb = base + SM_STAGE + s_cur * 65536 + (uint32_t)(c & 1) * 32768;
-                    const uint64_t bh = desc_sw128(wb), bl = desc_sw128(wb + 16384);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int ks = ks0; ks < ks1; ++ks) {
-                            const uint32_t ah = tm + T_ACT1H + 32 * c + 8 * ks, al = tm + T_ACT1L + 32 * c + 8 * ks;
-                            mma_ts(tm + T_ACC2, ah, bh + 2 * ks, ID128, (c | ks) != 0);
-                            mma_ts(tm + T_ACC2, ah, bl + 2 * ks, ID128, 1);
-                            mma_ts(tm + T_ACC2, al, bh + 2 * ks, ID128, 1);
-                        }
-                        if (ks1 == 4 && (c & 1)) tc_commit(BAR(B_WEMPTY0 + s_cur));
-                    }
-                    __syncwarp();
-                };
-                // Layer 1 overwrites [0,256): the epilogue warps must have read the previous tile's layer-2 accumulator.
-                // The three waits are taken in the order the barriers complete (weights long ago, accumulator read ~0.9 k
-                // clocks into the tile, first converted chunk ~1.3 k): each costs a few hundred clocks of this warp's thin
-                // share of the scheduler even when already complete, and only the last one should be exposed.
-                wait_w(3); s_cur = s_nxt;
-                if (tcount) mbar_wait(BAR(B_ACC2E), (tcount - 1) & 1);
-                wait_a0(0);
-                tc_fence_after();
-                if (lane == 0) TL(1);
-#pragma unroll 1
-                for (int j = 0; j < 8; ++j) {
-                    l1_ks(j, 0, 3);
-                    if (j < 7) {                                    // chunk j+1, while chunk j still has MMAs to issue
-                        wait_a0(j + 1);
-                        wait_w(3 + 2 * (j + 1));
-                    }
-                    l1_ks(j, 3, 4);
-                    if (j + 2 < 8) L0(j + 2, xb, T_ACC0 + 64u * (uint32_t)(j & 1));
-                    s_cur = s_nxt;
-                    if (lane == 0) TL(4 + 2 * j);
-                }
-                if (elect_one()) tc_commit(BAR(B_ACC1));
-                __syncwarp();
-                if (lane == 0) TL(19);
-                // ---- layer 2, K-chunk c as soon as the workers have converted it
-                auto wait_act1 = [&](int c) {
-                    mbar_wait(BAR(B_ACT1_0 + c), ph_act1);
-                    tc_fence_after();
-                    if (lane == 0) TL(40 + c);
-                };
-                wait_w(20); s_cur = s_nxt;
-                wait_act1(0);
-                l2_ks(0, 0, 3); wait_act1(1); l2_ks(0, 3, 4);
-                l2_ks(1, 0, 3); wait_act1(2); wait_w(22); l2_ks(1, 3, 4);
-                s_cur = s_nxt;
-                l2_ks(2, 0, 3); wait_act1(3); l2_ks(2, 3, 4);
-                l2_ks(3, 0, 4);
-                ph_act1 ^= 1;
-                {
-                    const uint64_t ah = dx0h0 + (uint64_t)(xb * 256), al = dx0l0 + (uint64_t)(xb * 256);
-                    const uint64_t th = desc_nosw(base + SM_W2T, 2048, 128), tl = desc_nosw(base + SM_W2T + 4096, 2048, 128);
-                    if (elect_one()) {
-                        mma_ss(tm + T_ACC2, ah, th, ID128, 1);
-                        mma_ss(tm + T_ACC2, ah, tl, ID128, 1);
-                        mma_ss(tm + T_ACC2, al, th, ID128, 1);
-                        tc_commit(BAR(B_ACC2));
-                    }
-                    __syncwarp();
-                }
-                if (lane == 0) TL(25);
-            }
-        }
-    } else if (warp < 10) {
-        // ======================================================== workers (8 warps, 256 threads)
-        const int q4 = warp & 3;                  // TMEM lane quarter this warp may touch
-        const int h = (warp - 2) >> 2;            // which half of the columns
-        const uint32_t tl = tmem + ((uint32_t)(q4 * 32) << 16);
-        uint32_t ph_acc0 = 0, ph_a0e = 0, ph_acc1 = 0;      // per-buffer phase bits
-        uint32_t tcount = 0;
-        mbar_wait(BAR(B_W0RDY), 0);               // biases are in shared memory
-        for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tcount) {
-            // ---------------- layer 0 chunks -> A operand of layer 1
-#pragma unroll 1
-            for (int j = 0; j < 8; ++j) {
-                const int b = j & 1;
-                mbar_wait(BAR(B_ACC0F0 + b), (ph_acc0 >> b) & 1); ph_acc0 ^= 1u << b;
-                tc_fence_after();
-                if (tid == 64) TL(64 + 4 * j);
-                uint32_t acc[32], hi[16], lo[16];
-                tmem_ld32(tl + T_ACC0 + 64u * b + 32u * h, acc);
-                if (tid == 64) TL(65 + 4 * j);
-                act_split32(acc, nullptr, hi, lo);               // b0 rides on x0 column 15 = 1
-                if (tid == 64) TL(66 + 4 * j);
-                mbar_wait(BAR(B_A0E0 + b), ((ph_a0e >> b) & 1) ^ 1); ph_a0e ^= 1u << b;
-                tc_fence_after();
-                tmem_st16(tl + T_A0 + 64u * b + 16u * h, hi);
-                tmem_st16(tl + T_A0 + 64u * b + 32u + 16u * h, lo);
-                tmem_st_wait();
-                tc_fence_before();
-                mbar_arrive(BAR(B_A0F0 + b));
-                if (tid == 64) TL(67 + 4 * j);
-            }
-            // ---------------- layer 1 accumulator -> A operand of layer 2, one 64-wide K-chunk at a time
-            mbar_wait(BAR(B_ACC1), ph_acc1); ph_acc1 ^= 1;
-            tc_fence_after();
-            if (tid == 64) TL(100);
-#pragma unroll 1
-            for (int t = 0; t < 4; ++t) {
-                uint32_t acc[32], hi[16], lo[16];
-                tmem_ld32(tl + T_ACC1 + 64u * t + 32u * h, acc);
-                act_split32(acc, sb1 + 64 * t + 32 * h, hi, lo);
-                tmem_st16(tl + T_ACT1H + 32u * t + 16u * h, hi);
-                tmem_st16(tl + T_ACT1L + 32u * t + 16u * h, lo);
-                tmem_st_wait();
-                tc_fence_before();
-                mbar_arrive(BAR(B_ACT1_0 + t));
-                if (tid == 64) TL(101 + t);
-            }
-        }
-    } else if (warp < 14) {
-        // ======================================================== gather + epilogue warps (4 warps, one row per thread)
-        const int q4 = warp & 3;
-        const int r = q4 * 32 + lane;             // row of the tile = TMEM lane this warp may touch
-        const uint32_t tl = tmem + ((uint32_t)(q4 * 32) << 16);
-        const int c0 = q.c0;
-        uint32_t ph_acc2 = 0, tcount = 0;
+        return;
+    }
 
-        // features of one tile -> x0 operand buffer xb (fp16 hi / lo tiles for the tensor pipe, fp32 copy for layer 3)
-        auto gather_tile = [&](int64_t tile, uint32_t xb) {
+    // ============================================================ consumer warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int g = warp >> 2, tw = tid & 127;
+    const int rf = 64 * g + 16 * (warp & 3) + (lane >> 2);       // fragment rows rf, rf + 8 of the tile
+    const int cq = 2 * (lane & 3);                               // fragment column offset inside an 8-column block
+    const int c0 = q.c0;
+    uint32_t cnt = 0;
+    auto stage_wait = [&]() {
+        const uint32_t s = cnt % NSTAGE;
+        mbar_wait(BAR(B_FULL0 + s), (cnt / NSTAGE) & 1);
+        return s;
+    };
+    auto stage_release = [&](uint32_t s) {     // after wait<0>(): the wgmmas that read stage s are complete
+        __syncwarp();
+        if (lane == 0) mbar_arrive(BAR(B_EMPTY0 + s));
+    };
+    const uint64_t dx0h = desc_nosw(base + SM_X0H + g * 1024, 2048, 128), dx0l = desc_nosw(base + SM_X0L + g * 1024, 2048, 128);
+    const uint64_t dw2th = desc_nosw(base + SM_W2T, 2048, 128), dw2tl = desc_nosw(base + SM_W2T + 4096, 2048, 128);
+    mbar_wait(BAR(B_W0RDY), 0);
+
+    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        bar_sync(1 + g, 128);                    // the previous tile's layer 3 has read x0f
+        if (tw < 64) {
+            const int r = 64 * g + tw;
             const int64_t pi = tile * TC_M + r;
             const bool live = pi < q.N;
             float f[16], in_cube = 1.f;
@@ -496,113 +210,113 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
                     }
                 }
             }
-            // Buffer xb is free: its last reader was tile-2's x0 tail MMA and this thread's own epilogue of that tile.
-            float *xf = x0f + xb * (16 * TC_M);
             uint32_t hi[8], lo[8];
 #pragma unroll
-            for (int j = 0; j < 15; ++j) xf[j * TC_M + r] = f[j];
-            xf[15 * TC_M + r] = in_cube;                      // c0 <= 13: row 15 is spare
+            for (int j = 0; j < 15; ++j) x0f[j * TC_M + r] = f[j];
+            x0f[15 * TC_M + r] = in_cube;                     // c0 <= 15: row 15 is spare
 #pragma unroll
             for (int i = 0; i < 7; ++i) split2(f[2 * i], f[2 * i + 1], hi[i], lo[i]);
             split2(f[14], 1.f, hi[7], lo[7]);                 // column 15 = 1: carries b0 (layer 0) and b2 (x0 tail of layer 2)
-            const int off = (int)xb * 4096 + (r >> 3) * 128 + (r & 7) * 16;
+            const int off = (r >> 3) * 128 + (r & 7) * 16;
             *reinterpret_cast<uint4 *>(sm + SM_X0H + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
             *reinterpret_cast<uint4 *>(sm + SM_X0H + off + 2048) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
             *reinterpret_cast<uint4 *>(sm + SM_X0L + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
             *reinterpret_cast<uint4 *>(sm + SM_X0L + off + 2048) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            mbar_arrive(BAR(B_X0R0 + xb));
-        };
-        // 32 columns of layer 3: LeakyReLU(acc) . w3 (b2 is already in the accumulator)
-        auto dot32 = [&](const uint32_t (&acc)[32], int col, float s) {
-            const float *ww = sw3 + col;
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                float v = __uint_as_float(acc[i]);
-                v = fmaxf(v, 0.01f * v);
-                s = fmaf(ww[i], v, s);
-            }
-            return s;
-        };
+            fence_proxy_async();
+        }
+        bar_sync(1 + g, 128);
 
-        if ((int64_t)blockIdx.x < ntiles) gather_tile(blockIdx.x, 0);
-        mbar_wait(BAR(B_W0RDY), 0);               // b2 / w3 / b3 are in shared memory
-        for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tcount) {
-            const uint32_t xb = tcount & 1;
-            if (tid == 320) TL(128);
-            if (tile + gridDim.x < ntiles) gather_tile(tile + gridDim.x, xb ^ 1);     // while this tile is in the tensor pipe
-            if (tid == 320) TL(131);
-            // ---------------- layer 3 of this tile
+        float acc2[64];
+#pragma unroll 1
+        for (int h = 0; h < 2; ++h) {
+            float acc1[64];
+            uint32_t s_prev = 0;
+#pragma unroll 1
+            for (int j = 0; j < 8; ++j) {
+                // layer 0, outputs [64 j, 64 j + 64): K = 16, one k-step
+                float acc0[32];
+                const uint64_t w0h = desc_nosw(base + SM_W0 + j * 1024, 8192, 128), w0l = w0h + (16384 >> 4);
+                fence();
+                mma_ss<64>(acc0, dx0h, w0h, 0);
+                mma_ss<64>(acc0, dx0h, w0l, 1);
+                mma_ss<64>(acc0, dx0l, w0h, 1);
+                commit();
+                wait<0>();                       // also retires layer-1 chunk j - 1
+                fence_regs(acc0);
+                if (j) stage_release(s_prev);
+                uint32_t ah[4][4], al[4][4];
+                act_frag64(acc0, nullptr, ah, al);              // b0 rides on x0 column 15 = 1
+                // layer 1, K-chunk j, outputs [128 h, 128 h + 128)
+                const uint32_t s = stage_wait();
+                const uint64_t bh = desc_sw128(base + SM_STAGE + s * STAGE_BYTES), bl = bh + (16384 >> 4);
+                fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    mma_rs<128>(acc1, ah[kk], bh + 2 * kk, (j | kk) != 0);
+                    mma_rs<128>(acc1, ah[kk], bl + 2 * kk, 1);
+                    mma_rs<128>(acc1, al[kk], bh + 2 * kk, 1);
+                }
+                commit();
+                s_prev = s;
+                ++cnt;
+            }
+            wait<0>();
+            fence_regs(acc1);
+            stage_release(s_prev);
+            // layer 2, K-chunks 2 h, 2 h + 1 (= this half of layer 1's outputs)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                uint32_t ah[4][4], al[4][4];
+                act_frag64(acc1 + 32 * c, sb1 + 128 * h + 64 * c + cq, ah, al);
+                const uint32_t s = stage_wait();
+                const uint64_t bh = desc_sw128(base + SM_STAGE + s * STAGE_BYTES), bl = bh + (16384 >> 4);
+                fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    mma_rs<128>(acc2, ah[kk], bh + 2 * kk, (h | c | kk) != 0);
+                    mma_rs<128>(acc2, ah[kk], bl + 2 * kk, 1);
+                    mma_rs<128>(acc2, al[kk], bh + 2 * kk, 1);
+                }
+                commit();
+                wait<0>();
+                fence_regs(acc2);
+                stage_release(s);
+                ++cnt;
+            }
+        }
+        // x0 tail of layer 2 (b2 through the constant-1 column)
+        fence();
+        mma_ss<128>(acc2, dx0h, dw2th, 1);
+        mma_ss<128>(acc2, dx0h, dw2tl, 1);
+        mma_ss<128>(acc2, dx0l, dw2th, 1);
+        commit();
+        wait<0>();
+        fence_regs(acc2);
+
+        // layer 3: LeakyReLU(acc2) . w3 over this thread's 32 columns of rows rf and rf + 8, then across the quad
+        float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const float w0 = sw3[8 * i + cq], w1 = sw3[8 * i + cq + 1];
+            float v0 = acc2[4 * i], v1 = acc2[4 * i + 1], v2 = acc2[4 * i + 2], v3 = acc2[4 * i + 3];
+            v0 = fmaxf(v0, 0.01f * v0); v1 = fmaxf(v1, 0.01f * v1);
+            v2 = fmaxf(v2, 0.01f * v2); v3 = fmaxf(v3, 0.01f * v3);
+            s0 = fmaf(w0, v0, s0); s0 = fmaf(w1, v1, s0);
+            s1 = fmaf(w0, v2, s1); s1 = fmaf(w1, v3, s1);
+        }
+        s0 += __shfl_xor_sync(0xffffffffu, s0, 1); s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+        if ((lane & 3) < 2) {
+            const int r = rf + 8 * (lane & 1);
+            float s = (lane & 1) ? s1 : s0;
             const int64_t pi = tile * TC_M + r;
-            const float *xf = x0f + xb * (16 * TC_M);
-            mbar_wait(BAR(B_ACC2), ph_acc2); ph_acc2 ^= 1;
-            tc_fence_after();
-            if (tid == 320) TL(132);
-            if (tid == 416) TL(140);
-            uint32_t a0[32], a1[32];
-            tmem_ld32_issue(tl + T_ACC2, a0);                 // columns 0..63 here, 64..127 in warps 14-17
-            tmem_ld32_issue(tl + T_ACC2 + 32, a1);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(BAR(B_ACC2E));            // the next tile's layer 1 may overwrite the accumulator
-            if (tid == 320) TL(133);
-            if (tid == 416) TL(141);
-            __nanosleep(EPI_YIELD_NS);            // the workers are converting the next tile's first chunk (critical path): stay out of their issue slots
-            float s = dot32(a0, 0, 0.f);
-            s = dot32(a1, 32, s);
-            asm volatile("bar.sync 1, 256;" ::: "memory");
             if (pi < q.N) {
-                s += spart[xb * TC_M + r];
 #pragma unroll
-                for (int j = 0; j < 15; ++j) s = fmaf(sw3[128 + j], xf[j * TC_M + r], s);    // skip connection; rows >= c0 are zero
+                for (int j = 0; j < 15; ++j) s = fmaf(sw3[128 + j], x0f[j * TC_M + r], s);    // skip connection; rows >= c0 are zero
                 s += sb3[0];
-                q.out[pi] = xf[15 * TC_M + r] * s;            // in_cube flag
+                q.out[pi] = x0f[15 * TC_M + r] * s;          // in_cube flag
             }
-            if (tid == 320) TL(134);
         }
-    } else {
-        // ======================================================== epilogue warps 14-17: layer-3 partial over columns 64..127
-        const int q4 = warp & 3;
-        const int r = q4 * 32 + lane;
-        const uint32_t tl = tmem + ((uint32_t)(q4 * 32) << 16);
-        uint32_t ph_acc2 = 0, tcount = 0;
-        mbar_wait(BAR(B_W0RDY), 0);
-        for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++tcount) {
-            mbar_wait(BAR(B_ACC2), ph_acc2); ph_acc2 ^= 1;
-            tc_fence_after();
-            if (tid == 544) TL(142);
-            uint32_t a0[32], a1[32];
-            tmem_ld32_issue(tl + T_ACC2 + 64, a0);
-            tmem_ld32_issue(tl + T_ACC2 + 96, a1);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(BAR(B_ACC2E));
-            if (tid == 544) TL(143);
-            __nanosleep(EPI_YIELD_NS);
-            float s = 0.f;
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                float v = __uint_as_float(a0[i]);
-                v = fmaxf(v, 0.01f * v);
-                s = fmaf(sw3[64 + i], v, s);
-            }
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                float v = __uint_as_float(a1[i]);
-                v = fmaxf(v, 0.01f * v);
-                s = fmaf(sw3[96 + i], v, s);
-            }
-            spart[(tcount & 1) * TC_M + r] = s;
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-        }
-    }
-
-    // ------------------------------------------------------------ teardown
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
     }
 }
 
@@ -620,14 +334,6 @@ int launch_mlp_tc_t(const QueryParams &q, const void *blob, cudaStream_t stream)
     ICON_LAUNCHED();
     return ICON_OK;
 }
-
-#ifdef ICON_MLP_TIMELINE
-}  // namespace icon
-extern "C" int icon_debug_mlp_timeline(long long *h_out) {
-    return cudaMemcpyFromSymbol(h_out, icon::g_tl, sizeof(long long) * 256) == cudaSuccess ? 0 : 1;
-}
-namespace icon {
-#endif
 
 int launch_mlp_tc(int mode, const QueryParams &q, const void *blob, cudaStream_t stream) {
     switch (mode) {

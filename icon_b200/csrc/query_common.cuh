@@ -1,5 +1,5 @@
 // Shared by the two implementations of the fused gather + MLP kernel (mlp.cu: FP32 FMA,
-// mlp_tc.cu: tcgen05 fp16x3): kernel parameters and the grid_sample restatements.
+// mlp_tc.cu: wgmma fp16x3): kernel parameters and the grid_sample restatements.
 #pragma once
 #include "common.cuh"
 

@@ -455,8 +455,7 @@ __global__ void __launch_bounds__(256) k_sdf_brute(const float *__restrict__ pts
 
 // points-per-warp policy of k_sdf_warp (see its header comment); icon_set_sdf_policy() overrides it for tuning
 static int64_t g_sdf_ppw32_from = 6000000, g_sdf_ppw8_from = 300000;
-static int g_sdf_order = -1;          // near-first leaf order: measured neutral-to-slower on the dense lattice (8.43 vs 8.33 ms,
-                                      // profiles/r2_summary.md), so OFF unless ICON_B200_SDF_ORDER=1
+static int g_sdf_order = -1;          // near-first leaf order: experimental, OFF unless ICON_B200_SDF_ORDER=1
 static int g_sdf_ppw_force = 0;
 
 // ---------------------------------------------------------------- host-side pipeline pieces

@@ -187,7 +187,7 @@ class HGFilter(nn.Module):
         return outputs
 
     def _forward_nhwc(self, x):
-        """HGFilters.py:161-197 on the NHWC / TMA / tcgen05 path (icon_b200/nhwc.py), 7x7 stride-2 stem included."""
+        """HGFilters.py:161-197 on the NHWC / TMA / wgmma path (icon_b200/nhwc.py), 7x7 stride-2 stem included."""
         from . import nhwc as T
         with torch.no_grad(), T.stats_arena(x.device):
             r = T.stem_conv7(x, self.conv1, reflect=False)                       # 7x7 s2 on the tensor cores, [N,H/2,W/2,64]
@@ -290,7 +290,7 @@ class GlobalGenerator(nn.Module):
         return y
 
     def _forward_nhwc(self, x):
-        """FBNet.py:216-264 on the NHWC / TMA / tcgen05 path: every InstanceNorm reads the sums its producing conv
+        """FBNet.py:216-264 on the NHWC / TMA / wgmma path: every InstanceNorm reads the sums its producing conv
         accumulated; ReflectionPad2d = halo written by the normalising pass; stride-2 convs read space-to-depth
         planes; ConvTranspose2d = 4 output phases; the 7x7 stem (Cin = 6) runs its K axis over filter rows; the 64 -> 3
         head is FP32 (k_conv7_head)."""

@@ -2,7 +2,7 @@
 
 Same class names, constructor arguments, method signatures and state_dict keys as the
 reference (SURVEY.md 8b) so that apps/ICON.py / apps/infer.py and `load_checkpoint`
-(lib/dataset/mesh_util.py:187-237) work unchanged; the bodies call the sm_100a kernels in
+(lib/dataset/mesh_util.py:187-237) work unchanged; the bodies call the sm_90a kernels in
 libicon_b200.so through icon_b200.ops.  Re-exported under the reference's import paths by
 lib/net/*.py and lib/common/train_util.py.
 

@@ -19,9 +19,8 @@ import torch
 
 from . import _C
 from ._C import check, lib
-from .ops import _need_cuda, _p, _stream
+from .ops import _need_cuda, _p, _sm_count, _stream
 
-NUM_SMS = 148
 
 
 class Raw:
@@ -239,9 +238,10 @@ def invalidate_packed(module):
 # ------------------------------------------------------------------------------------------------ convolution
 def _splits(n_pix_tiles, n_ch_tiles, chunks):
     items = n_pix_tiles * n_ch_tiles
-    if items >= NUM_SMS:
+    sms = _sm_count()
+    if items >= sms:
         return 1
-    return max(1, min(16, NUM_SMS // items, chunks))
+    return max(1, min(16, sms // items, chunks))
 
 
 def _launch(op, blob, wt_chunks, bias, out, co_off, Cout, Ht, Wt, osy, osx, ooy, oox, taps, cpt, n_tile, stats):

@@ -1,7 +1,7 @@
 """Tensor-level wrappers over the C ABI (include/icon_b200.h).
 
 PyTorch is plumbing here: device memory (caching allocator), the current CUDA stream and
-dtype/shape checks.  Every function enqueues hand-written sm_100a kernels from
+dtype/shape checks.  Every function enqueues hand-written sm_90a kernels from
 libicon_b200.so on torch's current stream and fails loudly otherwise.
 """
 import ctypes
@@ -27,6 +27,17 @@ def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
             raise _C.IconError("icon_b200 ops need CUDA tensors: there is no CPU path")
+
+
+_SM_COUNT = {}
+
+
+def _sm_count():
+    """Multiprocessors of the current CUDA device (split-K planners fill the SMs of the GPU they run on)."""
+    dev = torch.cuda.current_device()
+    if dev not in _SM_COUNT:
+        _SM_COUNT[dev] = torch.cuda.get_device_properties(dev).multi_processor_count
+    return _SM_COUNT[dev]
 
 
 def _hf(vals):
@@ -71,7 +82,7 @@ MLP_TC_BYTES = 32768 + 8 * 65536 + 4 * 32768 + 8192 + (512 + 256 + 128 + 144 + 4
 
 class PackedMLP:
     """BN-folded occupancy-MLP weights in the two device layouts of include/icon_b200.h:
-    `f32` (k-major fp32, FP32-FMA kernel) and `tc` (fp16 hi/lo UMMA tiles, tcgen05 kernel)."""
+    `f32` (k-major fp32, FP32-FMA kernel) and `tc` (fp16 hi/lo tensor-core tiles, wgmma kernel)."""
 
     def __init__(self, f32, tc, c0):
         self.f32, self.tc, self.c0 = f32, tc, c0
@@ -172,7 +183,7 @@ def pack_mlp(sd, c0, prefix="", device=None):
 
 
 def set_mlp_impl(name):
-    """'tcgen05' (default) or 'fp32' -- which fused gather+MLP kernel icon_query launches."""
+    """'tcgen05' (the tensor-core kernel, default; the name is historical) or 'fp32' -- which fused gather+MLP kernel icon_query launches."""
     check(lib.icon_set_mlp_impl({"fp32": 0, "tcgen05": 1}[name]), "icon_set_mlp_impl")
 
 

@@ -1,5 +1,5 @@
 /*
- * icon_b200.h -- C ABI of libicon_b200.so (sm_100a kernels for ICON's occupancy-query +
+ * icon_b200.h -- C ABI of libicon_b200.so (sm_90a kernels for ICON's occupancy-query +
  * mesh-extraction hot path).
  *
  * The reference (YuliangXiu/ICON) has no FFI: its "plugin API" for this path is Python
@@ -72,7 +72,7 @@ int icon_smpl_prepare(const float *verts, const int64_t *faces, const float *cma
  * columns ordered [y | x0]. */
 #define ICON_MLP_PACKED_FLOATS (16 * 512 + 512 + 512 * 256 + 256 + 272 * 128 + 128 + 144 + 1)
 /* Tensor-core form of the same folded weights (host: icon_b200/ops.py pack_mlp): every matrix
- * split W = hi + lo in fp16 and stored as ready-to-use K-major UMMA tiles (bytes):
+ * split W = hi + lo in fp16 and stored as ready-to-use K-major wgmma tiles (bytes):
  *   W0  hi 16384 | lo 16384    512 rows x 16 k, no swizzle (LBO 8192, SBO 128); k = 15 holds b0: the kernel feeds
  *                              x0 column 15 = 1, so the tensor-core path takes c0 <= 15
  *   W1  8 x (hi 32768 | lo 32768)   256 rows x 64 k per chunk, SWIZZLE_128B
@@ -80,7 +80,7 @@ int icon_smpl_prepare(const float *verts, const int64_t *faces, const float *cma
  *   W2t hi 4096 | lo 4096      128 rows x 16 k (the skip-concat x0 columns), no swizzle; k = 15 holds b2
  *   f32 b0[512] b1[256] b2[128] w3[144] b3[1] pad[3] */
 #define ICON_MLP_TC_BYTES (32768 + 8 * 65536 + 4 * 32768 + 8192 + (512 + 256 + 128 + 144 + 4) * 4)
-/* 0 = FP32 FMA kernel (mlp.cu), 1 = tcgen05 fp16x3 kernel (mlp_tc.cu, default when mlp_tc != NULL) */
+/* 0 = FP32 FMA kernel (mlp.cu), 1 = wgmma fp16x3 kernel (mlp_tc.cu, default when mlp_tc != NULL) */
 int icon_set_mlp_impl(int impl);
 int icon_get_mlp_impl(void);
 
@@ -210,7 +210,7 @@ int icon_visibility(const float *xyz, int V, const int64_t *faces, int F, int im
 int icon_conv2d(const float *x, const float *w, const float *bias, const float *res, float *y, int N, int Cin,
                 int H, int W, int Cout, int KH, int KW, int stride, int pad, int out_pad, int reflect,
                 int transposed, int act, icon_stream_t stream);
-/* Tensor-core (tcgen05, fp16 hi/lo x3, fp32-class accuracy) variant for Cin % 64 == 0; same semantics.
+/* Tensor-core (wgmma, fp16 hi/lo x3, fp32-class accuracy) variant for Cin % 64 == 0; same semantics.
  * wt_packed: per output-channel tile (n_tile rows, zero padded) and per 64-wide K-chunk (k = tap*Cin + ci) a
  * K-major SWIZZLE_128B tile of the fp16 hi parts followed by one of the lo parts (icon_b200/conv_ops.py packs
  * it).  splits > 1 = split-K over the chunks, partial sums in `ws` (icon_conv2d_tc_workspace_bytes). */
@@ -221,7 +221,7 @@ int icon_conv2d_tc(const float *x, const void *wt_packed, const float *bias, con
 /* ---- NHWC encoder path (csrc/conv_nhwc.cu, csrc/act_nhwc.cu): activations between layers are NHWC, pre-split
  * x = hi + lo into two fp16 tensors [N * nplanes][Hp][Wp][Cp] (Cp % 64 == 0) by icon_act_nhwc.
  *
- * icon_conv_nhwc: implicit-GEMM convolution on tcgen05, A operand staged by 4-D tiled TMA loads straight from the
+ * icon_conv_nhwc: implicit-GEMM convolution on wgmma, A operand staged by 4-D tiled TMA loads straight from the
  *   hi / lo tensors (`dims` = tensor-map extents innermost first, `strides` = element strides of dims 1..3), weights
  *   from `wt_packed` (per n_tile output channels and per chunk a K-major SWIZZLE_128B fp16 hi tile followed by the lo
  *   tile; `wt_chunks` chunks per tile, chunk index = wtap * cpt + channel block).  The launch covers a logical

@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz|json by running the REFERENCE's own modules, imported live
-from /root/reference (read-only).  Runs only in the build container (the GPU box has no
-/root/reference); the produced fixtures are committed and pin the oracle.
+from an ICON checkout (read-only; path in ICON_REFERENCE_DIR).  Needs only the CPU; the produced fixtures are
+committed and pin the oracle.
 
 Recipe (SURVEY.md 8c): the reference's optional dependencies that are not installed here
 (pytorch_lightning, matplotlib, mcubes, kaolin) are stubbed, and `lib`, `lib.net`,
@@ -18,7 +18,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-REF = "/root/reference"
+REF = os.environ["ICON_REFERENCE_DIR"]
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 

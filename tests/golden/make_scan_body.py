@@ -1,11 +1,11 @@
 """Build tests/golden/scan_body.npz: a body-shaped, deliberately NASTY triangle mesh decimated from the one real
-human scan the reference ships (/root/reference/sample_data/thuman2/scans/0525/0525.obj, 289 106 v / 500 000 f).
+human scan the reference ships (sample_data/thuman2/scans/0525/0525.obj of an ICON checkout, 289 106 v / 500 000 f).
 
 The synthetic capsule of icon_b200.synthetic.body_mesh is smooth, watertight and in general position; what a
 first-minimum nearest-face rule and a parity ray cast actually disagree on is the opposite: sliver and zero-area
 faces, non-manifold edges, holes, duplicated vertices, rays through shared edges / vertices.  Vertex clustering
 (uniform grid, cluster mean) of a raw scan produces all of these by itself; a handful of exactly degenerate faces
-are added on top.  Runs only in the build container (the GPU box has no /root/reference); the fixture is committed.
+are added on top.  Needs the ICON checkout (ICON_REFERENCE_DIR); the fixture is committed.
 
     python tests/golden/make_scan_body.py
 """
@@ -13,7 +13,7 @@ import os
 
 import numpy as np
 
-SRC = "/root/reference/sample_data/thuman2/scans/0525/0525.obj"
+SRC = os.path.join(os.environ["ICON_REFERENCE_DIR"], "sample_data/thuman2/scans/0525/0525.obj")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

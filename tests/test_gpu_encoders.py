@@ -35,7 +35,7 @@ def test_conv2d_matches_torch(cin, cout, k, s, p, reflect, hw):
         ref = conv(F.pad(x, (reflect,) * 4, mode="reflect") if reflect else x)
         res = torch.randn(ref.shape, generator=_g(7))
         ref_r = torch.tanh(ref + res)
-    for impl in ("auto", "fp32"):                 # auto = tcgen05 kernel when Cin % 64 == 0
+    for impl in ("auto", "fp32"):                 # auto = tensor-core kernel when Cin % 64 == 0
         C.set_conv_impl(impl)
         try:
             y = C.conv2d(x.to(dev), conv.to(dev), reflect=reflect)
@@ -69,7 +69,7 @@ def test_conv2d_tensor_core_shapes(cin, cout, k, s, p, reflect, hw, relu):
 def test_conv_transpose2d_matches_torch():
     dev = _cuda()
     from icon_b200 import conv_ops as C
-    for cin, cout in ((48, 24), (128, 64)):          # FP32 kernel / tcgen05 kernel
+    for cin, cout in ((48, 24), (128, 64)):          # FP32 kernel / tensor-core kernel
         ct = nn.ConvTranspose2d(cin, cout, 3, stride=2, padding=1, output_padding=1)
         x = torch.randn(2, cin, 17, 19, generator=_g(1))
         with torch.no_grad():

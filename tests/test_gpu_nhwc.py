@@ -1,4 +1,4 @@
-"""The NHWC / TMA / tcgen05 encoder path (csrc/conv_nhwc.cu, csrc/act_nhwc.cu, icon_b200/nhwc.py) op by op against
+"""The NHWC / TMA / wgmma encoder path (csrc/conv_nhwc.cu, csrc/act_nhwc.cu, icon_b200/nhwc.py) op by op against
 torch's own operators (the layers the reference composes in lib/net/FBNet.py, HGFilters.py, net_util.py)."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Parity of the CUDA occupancy-query path against the CPU oracle (run on the B200 box).
+"""Parity of the CUDA occupancy-query path against the CPU oracle (run on an H100).
 
 Bars: nearest face / sign / visibility / sdf bit-exact; occupancy within 1e-4 (north_star);
 engine query sets identical; marching-cubes indexing identical.

@@ -99,7 +99,7 @@ def _unpack_nosw(buf, rows):
 
 @pytest.mark.parametrize("c0", [13, 10])
 def test_tensor_core_blob_evaluated_like_the_kernel_matches_oracle(built_lib, c0):
-    """Decode the UMMA tiles of the tcgen05 blob (hi + lo) and run the network the way k_query_mlp_tc does: x0 column
+    """Decode the tensor-core tiles of the packed blob (hi + lo) and run the network the way k_query_mlp_tc does: x0 column
     15 is the constant 1, b0 and b2 are NOT added (they sit in row 15 of W0 and of the x0 tail of W2), b1 / b3 are."""
     import numpy as np
     from icon_b200 import ops

@@ -5,7 +5,7 @@ containers of icon_b200.encoders (which hold the reference's exact state_dict). 
 
 * checker: same weights, same input, torch ops instead of libicon_b200.so (tests/test_oracle_golden.py pins it
   to outputs of the reference's own modules);
-* baseline: bench.py times these on the same B200 as "the reference's own GPU path" for filter() / NormalNet
+* baseline: bench.py times these on the same GPU as "the reference's own GPU path" for filter() / NormalNet
   (the reference runs exactly these torch ops -- with TF32 allowed, its default on Ampere and later).
 
   conv_block       lib/net/net_util.py:258-280   ConvBlock.forward

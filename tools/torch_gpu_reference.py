@@ -1,4 +1,4 @@
-"""Reference-equivalent single-GPU path on the B200 (SURVEY.md 8d (b): the ">= 10x" denominator of north_star).
+"""Reference-equivalent single-GPU path (SURVEY.md 8d (b): the ">= 10x" denominator of north_star).
 
 The reference's GPU path = kaolin's two brute-force O(N*F) CUDA kernels (point_to_mesh_distance, check_sign) for
 the SMPL block + stock PyTorch ops (grid_sample, gather, cat, Conv1d, BatchNorm1d, LeakyReLU) for everything else.
