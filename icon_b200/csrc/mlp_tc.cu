@@ -81,7 +81,23 @@ __device__ __forceinline__ void act_frag64(const float *d, const float *bias, ui
     }
 }
 
-// MODE: 0 icon, 1 pifu, 2 pamir, 3 raw feature matrix
+// f[off + t] = v[t] for a runtime offset off, where off + NV <= 15.  Every index into f is a compile-time constant,
+// so f stays in registers (a runtime index would move it to local memory); columns outside [off, off + NV) keep their
+// value.
+template <int NV>
+__device__ __forceinline__ void place_at(float (&f)[16], int off, const float (&v)[NV]) {
+#pragma unroll
+    for (int j = 0; j < 15; ++j) {
+        float x = f[j];
+#pragma unroll
+        for (int t = 0; t < NV; ++t) x = j - t == off ? v[t] : x;
+        f[j] = x;
+    }
+}
+
+// MODE: 0 icon, 1 pifu, 2 pamir, 3 raw feature matrix.  The gather places the c0 input columns as mlp.cu and the
+// reference do (image channels first, then the prior's own columns); columns c0..14 stay zero, since layer 0, the x0
+// tail of layer 2 and layer 3's skip connection read all of rows 0..14.
 template <int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, const uint8_t *__restrict__ blob) {
     using namespace wg;
@@ -166,7 +182,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
             for (int j = 0; j < 16; ++j) f[j] = 0.f;
             if (live) {
                 if (MODE == 3) {
-                    for (int j = 0; j < c0; ++j) f[j] = q.raw[(size_t)j * q.N + pi];
+#pragma unroll
+                    for (int j = 0; j < 15; ++j)
+                        if (j < c0) f[j] = q.raw[(size_t)j * q.N + pi];
                 } else {
                     const float4 xyz = q.xyz4[pi];
                     in_cube = xyz.w;
@@ -188,25 +206,49 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
                             for (int ch = 0; ch < 6; ++ch)
                                 f[ch] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
                             f[6] = sdf; f[7] = cx; f[8] = cy; f[9] = cz; f[10] = r1.x; f[11] = r1.y; f[12] = r1.z;
-                        } else {
+                        } else if (d == 3) {
 #pragma unroll
                             for (int ch = 0; ch < 3; ++ch)
                                 f[ch] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
                             f[3] = sdf; f[4] = cx; f[5] = cy; f[6] = cz; f[7] = r1.x; f[8] = r1.y; f[9] = r1.z;
+                        } else {                                     // any d in 1..8 (c0 = d + 7 <= 15)
+#pragma unroll
+                            for (int ch = 0; ch < 8; ++ch)
+                                if (ch < d) f[ch] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                            const float smpl[7] = {sdf, cx, cy, cz, r1.x, r1.y, r1.z};
+                            place_at(f, d, smpl);
                         }
                     } else if (MODE == 1) {
+                        if (q.C == 12) {
 #pragma unroll
-                        for (int ch = 0; ch < 12; ++ch)
-                            f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                        f[12] = xyz.z;
+                            for (int ch = 0; ch < 12; ++ch)
+                                f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                            f[12] = xyz.z;
+                        } else {                                     // any C in 1..14 (c0 = C + 1 <= 15)
+#pragma unroll
+                            for (int ch = 0; ch < 14; ++ch)
+                                if (ch < q.C) f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                            const float z[1] = {xyz.z};
+                            place_at(f, q.C, z);
+                        }
                     } else {
                         const size_t vs = (size_t)q.VD * q.VD * q.VD;
+                        if (q.C == 6) {
 #pragma unroll
-                        for (int ch = 0; ch < 6; ++ch)
-                            f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                            for (int ch = 0; ch < 6; ++ch)
+                                f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
 #pragma unroll
-                        for (int ch = 0; ch < 7; ++ch)
-                            f[6 + ch] = trilinear(q.vol + ch * vs, q.VD, xyz.x, xyz.y, xyz.z);
+                            for (int ch = 0; ch < 7; ++ch)
+                                f[6 + ch] = trilinear(q.vol + ch * vs, q.VD, xyz.x, xyz.y, xyz.z);
+                        } else {                                     // any C in 1..8 (c0 = C + 7 <= 15)
+#pragma unroll
+                            for (int ch = 0; ch < 8; ++ch)
+                                if (ch < q.C) f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                            float v[7];
+#pragma unroll
+                            for (int ch = 0; ch < 7; ++ch) v[ch] = trilinear(q.vol + ch * vs, q.VD, xyz.x, xyz.y, xyz.z);
+                            place_at(f, q.C, v);
+                        }
                     }
                 }
             }
@@ -314,7 +356,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
 #pragma unroll
                 for (int j = 0; j < 15; ++j) s = fmaf(sw3[128 + j], x0f[j * TC_M + r], s);    // skip connection; rows >= c0 are zero
                 s += sb3[0];
-                q.out[pi] = x0f[15 * TC_M + r] * s;          // in_cube flag
+                // in_cube * s as the reference computes it, signed zero included; but outside the cube the features
+                // are unbounded (pifu's z, icon's normals far from the body) and can overflow the fp16 operands,
+                // so a non-finite s must not turn the product into NaN there
+                q.out[pi] = x0f[15 * TC_M + r] != 0.f ? s : copysignf(0.f, s);
             }
         }
     }

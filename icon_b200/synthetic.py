@@ -86,8 +86,15 @@ def lattice_points(res, device="cpu"):
     return torch.stack([x, y, z], -1).reshape(1, -1, 3).to(device)
 
 
-def mlp_state_dict(c0=13, dims=(512, 256, 128, 1), res_layers=(2, 3, 4), seed=0):
-    """Random weights with the reference MLP's state_dict keys (lib/net/MLP.py:26-47)."""
+def mlp_state_dict(c0=13, dims=(512, 256, 128, 1), res_layers=(2, 3, 4), seed=0, trained_bn=False):
+    """Random weights with the reference MLP's state_dict keys (lib/net/MLP.py:26-47).
+
+    By default the BatchNorm statistics are mild (running_var in [0.5, 1.5], gamma near 1).  trained_bn=True gives
+    BatchNorm layers like a trained network's instead: running_var log-uniform in [1e-4, 10], |gamma| log-uniform in
+    [0.1, 10] with random signs, running_mean up to about +-30.  As in training, the statistics agree with the conv
+    they follow: a channel's weight row is scaled by sqrt(running_var) and its bias sits near running_mean, so the
+    normalised pre-activations stay O(1) while the folded weights and biases (gamma / sqrt(var + eps) up to ~1e3)
+    exercise the fold."""
     g = torch.Generator().manual_seed(seed)
     chans = [c0] + list(dims)
     sd = {}
@@ -102,7 +109,35 @@ def mlp_state_dict(c0=13, dims=(512, 256, 128, 1), res_layers=(2, 3, 4), seed=0)
             sd[f"norms.{l}.running_mean"] = 0.1 * torch.randn(cout, generator=g)
             sd[f"norms.{l}.running_var"] = 0.5 + torch.rand(cout, generator=g)
             sd[f"norms.{l}.num_batches_tracked"] = torch.tensor(100)
+    if trained_bn:
+        t = torch.Generator().manual_seed(seed + 1000)
+        for l in range(len(chans) - 2):
+            cout = chans[l + 1]
+            var = 10.0 ** (torch.rand(cout, generator=t) * 5 - 4)
+            mean = 10.0 * torch.randn(cout, generator=t)
+            sign = torch.where(torch.rand(cout, generator=t) < 0.5, -1.0, 1.0)
+            sd[f"norms.{l}.running_var"] = var
+            sd[f"norms.{l}.running_mean"] = mean
+            sd[f"norms.{l}.weight"] = sign * 10.0 ** (torch.rand(cout, generator=t) * 2 - 1)
+            sd[f"filters.{l}.weight"] = sd[f"filters.{l}.weight"] * var.sqrt()[:, None, None]
+            sd[f"filters.{l}.bias"] = mean + var.sqrt() * sd[f"filters.{l}.bias"]
     return sd
+
+
+def wide_range_features(c0, n, seed=0):
+    """[1, c0, n] MLP inputs over a wide dynamic range: magnitudes log-uniform in [1e-6, 1e4] with random signs and
+    about 10 % exact zeros.  In the last quarter of the points column 0 is in [-1e4, -1e3] and the other columns are
+    N(0, 1): with a layer-0 weight column of one sign (positive after the BatchNorm fold) those points drive nearly
+    every layer-0 unit onto the LeakyReLU negative branch."""
+    g = torch.Generator().manual_seed(seed)
+    mag = 10.0 ** (torch.rand(1, c0, n, generator=g, dtype=torch.float64) * 10 - 6)
+    sign = torch.where(torch.rand(1, c0, n, generator=g) < 0.5, -1.0, 1.0).double()
+    x = (mag * sign).float()
+    x[torch.rand(1, c0, n, generator=g) < 0.1] = 0.0
+    q = n - n // 4
+    x[:, :, q:] = torch.randn(1, c0, n - q, generator=g)
+    x[:, 0, q:] = -(10.0 ** (3 + torch.rand(n - q, generator=g)))
+    return x
 
 
 def feature_map(channels=12, size=128, seed=0):

@@ -219,9 +219,10 @@ def cal_sdf_batch_torch(verts, faces, cmaps, vis, points):
 
 
 # ----------------------------------------------------------------------------- MLP
-def mlp_forward(sd, feature, res_layers=(2, 3, 4), last_op=None, dtype=torch.float32):
+def mlp_forward(sd, feature, res_layers=(2, 3, 4), last_op=None, dtype=torch.float32, activations=None):
     """MLP.forward (MLP.py:49-72) from a state_dict with keys filters.{l}.*, norms.{l}.*
-    (norm='batch', eval mode)."""
+    (norm='batch', eval mode).  activations: a list that receives each layer's output (after the
+    LeakyReLU, before last_op)."""
     n_layers = len([k for k in sd if k.startswith("filters.") and k.endswith(".weight")])
     y = feature.to(dtype)
     tmpy = y
@@ -233,6 +234,8 @@ def mlp_forward(sd, feature, res_layers=(2, 3, 4), last_op=None, dtype=torch.flo
                              sd[f"norms.{i}.running_var"].to(dtype), sd[f"norms.{i}.weight"].to(dtype),
                              sd[f"norms.{i}.bias"].to(dtype), False, 0.1, 1e-5)
             y = F.leaky_relu(y, 0.01)
+        if activations is not None:
+            activations.append(y)
     if last_op is not None:
         y = last_op(y)
     return y

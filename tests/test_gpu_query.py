@@ -267,11 +267,15 @@ def test_query_pifu_and_pamir_vs_oracle():
 def test_query_empty_and_tiny_inputs():
     dev = _cuda()
     from icon_b200 import ops
+    from oracle import query as OQ
     pts, feat, sd, packed, body, smpl = _icon_case(dev, n=128)
     for n in (0, 1, 63, 65):
-        out = ops.query("icon", pts[:, :n].permute(0, 2, 1).to(dev), EYE, feat.to(dev), packed, body=body)
+        samples = pts[:, :n].permute(0, 2, 1)
+        out = ops.query("icon", samples.to(dev), EYE, feat.to(dev), packed, body=body).cpu()
         assert out.shape == (1, 1, n)
-        assert torch.isfinite(out).all()
+        if n:
+            ref = OQ.query(sd, [feat], samples, EYE, prior="icon", smpl=smpl, mlp_dtype=torch.float64)[0]
+            assert ((out - ref).abs() <= 1e-4 * ref.abs().clamp(min=1.0)).all(), (out - ref).abs().max().item()
 
 
 def test_hgpifunet_query_func_matches_oracle():

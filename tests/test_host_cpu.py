@@ -97,14 +97,42 @@ def _unpack_nosw(buf, rows):
     return np.ascontiguousarray(t.transpose(1, 2, 0, 3)).reshape(rows, 16).astype(np.float64)
 
 
-@pytest.mark.parametrize("c0", [13, 10])
+def _split_hi_lo(v):
+    """wgmma.cuh split2 on an fp32 layer input: hi = fp16(v), lo = fp16(v - hi)."""
+    import numpy as np
+    v = v.astype(np.float32)
+    hi = v.astype(np.float16)
+    lo = (v - hi.astype(np.float32)).astype(np.float16)
+    return hi.astype(np.float64), lo.astype(np.float64)
+
+
+@pytest.mark.parametrize("c0", range(1, 16))
 def test_tensor_core_blob_evaluated_like_the_kernel_matches_oracle(built_lib, c0):
-    """Decode the tensor-core tiles of the packed blob (hi + lo) and run the network the way k_query_mlp_tc does: x0 column
-    15 is the constant 1, b0 and b2 are NOT added (they sit in row 15 of W0 and of the x0 tail of W2), b1 / b3 are."""
+    """Decode the tensor-core tiles of the packed blob and run the network the way k_query_mlp_tc does: x0 column 15 is
+    the constant 1, b0 and b2 are NOT added (they sit in row 15 of W0 and of the x0 tail of W2), b1 / b3 are.  Every
+    wgmma layer input (x0, h0, h1) is split into fp16 hi + lo and each product is hi*Whi + hi*Wlo + lo*Whi; layer 3 is
+    an fp32-operand dot.  N(0, 1.5^2) inputs and the default weights, for every c0 the kernel takes."""
+    _check_tc_blob_emulation(c0, "normal")
+
+
+@pytest.mark.parametrize("c0", range(1, 16))
+@pytest.mark.parametrize("inputs", ["wide_range", "trained_bn"])
+def test_tensor_core_blob_emulation_over_wide_range_and_trained_bn(built_lib, c0, inputs):
+    """The same emulation on the two harder input kinds of tests/test_gpu_mlp.py::test_mlp_only_dynamic_range
+    (magnitudes 1e-6 .. 1e4, trained-like BatchNorm folds): the bar that test uses holds for the kernel's numerics."""
+    _check_tc_blob_emulation(c0, inputs)
+
+
+def _check_tc_blob_emulation(c0, inputs):
     import numpy as np
     from icon_b200 import ops
     from oracle import query as OQ
-    sd = S.mlp_state_dict(c0, seed=9)
+    sd = S.mlp_state_dict(c0, seed=9, trained_bn=inputs == "trained_bn")
+    if inputs == "wide_range":
+        sd["filters.0.weight"][:, 0].abs_()
+        x = S.wide_range_features(c0, 2000, seed=c0)
+    else:
+        x = 1.5 * torch.randn(1, c0, 2000, generator=torch.Generator().manual_seed(1))
     blob = ops.pack_mlp(sd, c0).tc.numpy().tobytes()
     o = 0
 
@@ -114,23 +142,41 @@ def test_tensor_core_blob_evaluated_like_the_kernel_matches_oracle(built_lib, c0
         o += n
         return r
 
-    W0 = _unpack_nosw(take(16384), 512) + _unpack_nosw(take(16384), 512)                       # [512, 16]
-    W1 = np.concatenate([_unswizzle128(take(32768), 256) + _unswizzle128(take(32768), 256) for _ in range(8)], 1)   # [256, 512]
-    W2 = np.concatenate([_unswizzle128(take(16384), 128) + _unswizzle128(take(16384), 128) for _ in range(4)], 1)   # [128, 256]
-    W2t = _unpack_nosw(take(4096), 128) + _unpack_nosw(take(4096), 128)                        # [128, 16]
+    def pair(unpack, nbytes, rows):
+        return unpack(take(nbytes), rows), unpack(take(nbytes), rows)
+
+    W0 = pair(_unpack_nosw, 16384, 512)                                                       # [512, 16] hi, lo
+    W1 = [pair(_unswizzle128, 32768, 256) for _ in range(8)]
+    W1 = tuple(np.concatenate([w[i] for w in W1], 1) for i in range(2))                        # [256, 512]
+    W2 = [pair(_unswizzle128, 16384, 128) for _ in range(4)]
+    W2 = tuple(np.concatenate([w[i] for w in W2], 1) for i in range(2))                        # [128, 256]
+    W2t = pair(_unpack_nosw, 4096, 128)                                                        # [128, 16]
     f32 = np.frombuffer(take((512 + 256 + 128 + 144 + 4) * 4), dtype=np.float32).astype(np.float64)
     assert o == ops.MLP_TC_BYTES
     b1, w3, b3 = f32[512:768], f32[896:1040], f32[1040]
-    x = torch.randn(1, c0, 300, generator=torch.Generator().manual_seed(1)).double()
-    x16 = np.zeros((16, 300)); x16[:c0] = x[0].numpy(); x16[15] = 1.0
+
+    def mma(W, v):
+        hi, lo = _split_hi_lo(v)
+        return W[0] @ hi + W[1] @ hi + W[0] @ lo
+
+    n = x.shape[2]
+    x16 = np.zeros((16, n), np.float32); x16[:c0] = x[0].numpy(); x16[15] = 1.0
     lre = lambda v: np.maximum(v, 0.01 * v)
-    h0 = lre(W0 @ x16)
-    h1 = lre(W1 @ h0 + b1[:, None])
-    h2 = lre(W2 @ h1 + W2t @ x16)
-    xs = x16.copy(); xs[15] = 0.0                                # layer 3 reads the fp32 feature copy: no constant row
+    h0 = lre(mma(W0, x16))
+    h1 = lre(mma(W1, h0) + b1[:, None])
+    h2 = lre(mma(W2, h1) + mma(W2t, x16))
+    xs = x16.astype(np.float64); xs[15] = 0.0                    # layer 3 reads the fp32 feature copy: no constant row
     y = w3[:128] @ h2 + w3[128:] @ xs + b3
-    ref = OQ.mlp_forward(sd, x, dtype=torch.float64)[0, 0].numpy()
-    assert np.abs(y - ref).max() < 2e-5                          # fp16 hi + lo weights: 22 significant bits
+    acts = []
+    ref = OQ.mlp_forward(sd, x, dtype=torch.float64, activations=acts)[0, 0].numpy()
+    scale = torch.cat([x[0].double().abs()] + [a[0].abs() for a in acts]).amax(0).numpy()
+    assert scale.max() < 65504                                  # every layer input fits the fp16 hi part
+    err = np.abs(y - ref)
+    assert (err <= 1e-4 * np.maximum(1.0, np.abs(ref)) + 2e-6 * scale).all(), (err.max(), scale.max())
+    if inputs == "normal":
+        assert err.max() < 2e-5                                  # fp16 hi + lo operands: 22 significant bits
+    if inputs == "wide_range":
+        assert (acts[0][0, :, -n // 4:] < 0).double().mean() > 0.9      # the negative LeakyReLU branch is exercised
 
 
 def test_pack_mlp_refuses_16_input_channels(built_lib):
