@@ -44,10 +44,6 @@ _SIGS = {
     "icon_grid_scatter": (_i, [_vp, _vp, _vp, _i64, _vp]),
     "icon_grid_init_points": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
     "icon_grid_count_above": (_i, [_vp, _i64, _f, _vp, _vp]),
-    "icon_conv2d": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    "icon_conv2d_tc_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
-    "icon_conv2d_tc": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz,
-                           _vp]),
     "icon_conv_nhwc_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "icon_conv_nhwc": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i,
                            _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
@@ -59,16 +55,10 @@ _SIGS = {
     "icon_nchw_to_nhwc": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp]),
     "icon_nhwc_to_nchw": (_i, [_vp, _vp, _i, _i, _i, _i, _i64, _vp]),
     "icon_stem_pack": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    "icon_conv7_head": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "icon_clean_mesh_workspace_bytes": (_sz, [_i64, _i64]),
     "icon_clean_mesh_count": (_i, [_vp, _i64, _i64, _vp, _sz, _vp, _vp]),
     "icon_clean_mesh_emit": (_i, [_vp, _i, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
-    "icon_group_norm": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _vp]),
     "icon_conv3d": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    "icon_avg_pool2": (_i, [_vp, _vp, _i64, _i, _i, _vp]),
-    "icon_bicubic_up2_add": (_i, [_vp, _vp, _vp, _i64, _i, _i, _vp]),
-    "icon_cat3_add": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i64, _vp]),
-    "icon_add3": (_i, [_vp, _vp, _vp, _vp, _i64, _vp]),
     "icon_normalize_mask": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp]),
     "icon_voxelize_workspace_bytes": (_sz, [_i]),
     "icon_voxelize": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _f, _vp, _vp, _sz, _vp]),

@@ -8,8 +8,6 @@
 //   k_ew_nhwc         add2 / add3 / 2x2 average pool / bicubic x2 upsample + add (HGFilters.py:49-79), each also
 //                     accumulating the statistics of its result for the GroupNorm that reads it next
 //   k_nchw_to_nhwc / k_nhwc_to_nchw   layout adaptors at the ends of an encoder (+ statistics)
-//   k_conv7_head      the 64 -> 3 channel 7 x 7 reflect-padded output convolution + tanh of the pix2pixHD generator
-//                     (FBNet.py:258-261): N = 3 cannot use a 128 x N tensor-core tile, FP32 FMA from NHWC
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -468,56 +466,6 @@ __global__ void k_stem_pack(const float *__restrict__ x, __half *__restrict__ hi
     }
 }
 
-// ---------------------------------------------------------------------------------------- 7 x 7 output head (Cout <= 3)
-// x fp32 NHWC [N][H][W][64], w torch layout [Cout][64][7][7], reflection pad 3, y NCHW [N][Cout][H][W], tanh optional
-__global__ void __launch_bounds__(128) k_conv7_head(const float *__restrict__ x, const float *__restrict__ w,
-                                                    const float *__restrict__ bias, float *__restrict__ y, int N, int H,
-                                                    int W, int Cout, int act) {
-    __shared__ float4 sw[49 * 16 * 3];                         // [tap][c4][co] -> float4 over 4 consecutive input channels
-    for (int i = threadIdx.x; i < 49 * 16 * 3; i += blockDim.x) {
-        const int co = i % 3, c4 = (i / 3) & 15, tap = i / 48;
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (co < Cout) {
-            const float *s = w + ((size_t)co * 64 + c4 * 4) * 49 + tap;
-            v = make_float4(s[0], s[49], s[98], s[147]);
-        }
-        sw[i] = v;
-    }
-    __syncthreads();
-    // 16 x 8 pixel tile per block so that the 7 x 7 windows of neighbouring threads overlap in L1
-    const int tx = blockIdx.x % ((W + 15) / 16), ty = blockIdx.x / ((W + 15) / 16);
-    const int n = blockIdx.y;
-    const int ox = tx * 16 + (threadIdx.x & 15), oy = ty * 8 + (threadIdx.x >> 4);
-    if (ox >= W || oy >= H) return;
-    float acc[3] = {0.f, 0.f, 0.f};
-    for (int kh = 0; kh < 7; ++kh) {
-        int iy = oy - 3 + kh;
-        iy = iy < 0 ? -iy : (iy >= H ? 2 * H - 2 - iy : iy);
-        for (int kw = 0; kw < 7; ++kw) {
-            int ix = ox - 3 + kw;
-            ix = ix < 0 ? -ix : (ix >= W ? 2 * W - 2 - ix : ix);
-            const float4 *src = reinterpret_cast<const float4 *>(x + (((size_t)n * H + iy) * W + ix) * 64);
-            const float4 *wt = sw + (kh * 7 + kw) * 48;
-#pragma unroll
-            for (int c4 = 0; c4 < 16; ++c4) {
-                const float4 v = __ldg(src + c4);
-#pragma unroll
-                for (int co = 0; co < 3; ++co) {
-                    const float4 ww = wt[c4 * 3 + co];
-                    acc[co] = fmaf(v.x, ww.x, acc[co]); acc[co] = fmaf(v.y, ww.y, acc[co]);
-                    acc[co] = fmaf(v.z, ww.z, acc[co]); acc[co] = fmaf(v.w, ww.w, acc[co]);
-                }
-            }
-        }
-    }
-    for (int co = 0; co < Cout; ++co) {
-        float v = acc[co] + (bias ? bias[co] : 0.f);
-        if (act == 2) v = tanhf(v);
-        else if (act == 1) v = fmaxf(v, 0.f);
-        y[(((size_t)n * Cout + co) * H + oy) * W + ox] = v;
-    }
-}
-
 // out[n][co][y][x] = act(bias[co] + sum_{ky,kx} P[n][refl(y + ky - 3)][refl(x + kx - 3)][(ky * 7 + kx) * Cout + co])
 // P = the 1 x 1 tensor-core GEMM of the 64-channel activation with the head's weights regrouped per tap
 // (49 * Cout columns): the 7 x 7 head (FBNet.py:258-261) as GEMM + col2im instead of an N = 3 implicit GEMM.
@@ -669,17 +617,6 @@ extern "C" int icon_stem_pack(const float *x, void *hi, void *lo, int N, int Cin
     const int64_t total = (int64_t)N * sy * Hrows * Wp;
     ICON_CUDA(launch_pdl(k_stem_pack, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, stream, x, (__half *)hi, (__half *)lo, N, Cin,
                          H, W, Cp8, Wp, Hrows, sy, reflect));
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
-
-extern "C" int icon_conv7_head(const float *x, const float *w, const float *bias, float *y, int N, int H, int W, int Cin,
-                               int Cout, int act, icon_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(x && w && y && N > 0 && H > 3 && W > 3, "icon_conv7_head: bad argument");
-    ICON_CHECK_ARG(Cin == 64 && Cout >= 1 && Cout <= 3, "icon_conv7_head: 64 -> (1..3) channels (FBNet.py:258)");
-    dim3 grid((unsigned)(((W + 15) / 16) * ((H + 7) / 8)), (unsigned)N);
-    k_conv7_head<<<grid, 128, 0, stream>>>(x, w, bias, y, N, H, W, Cout, act);
     ICON_LAUNCHED();
     return ICON_OK;
 }

@@ -1,362 +1,9 @@
-// Encoder kernels (NCHW fp32): implicit-GEMM conv2d / conv-transpose2d, GroupNorm / InstanceNorm,
-// 2x2 average pool, bicubic x2 upsample, and the few elementwise joins the two encoders need.
-//
-// Replace the cuDNN / torch calls of (reference)
-//   HGFilter / HourGlass / ConvBlock     lib/net/HGFilters.py:49-197, lib/net/net_util.py:258-280
-//   GlobalGenerator / ResnetBlock        lib/net/FBNet.py:216-319
-//   NormalNet.forward                    lib/net/NormalNet.py:84-97
-// k_conv2d is the FP32-FMA implicit GEMM used for the layers the tensor-core kernel does not take
-// (conv_tc.cu needs Cin % 64 == 0: the 7x7 stem / head and the 32-channel ConvBlock convs land here).
+// The encoder kernels that live outside the NHWC path (conv_nhwc.cu, act_nhwc.cu), NCHW fp32:
+//   k_normalize_mask   NormalNet.forward's L2 normalisation + background mask   lib/net/NormalNet.py:84-97
+//   k_conv3d           PaMIR VolumeEncoder's Conv3d + BatchNorm3d layers        lib/net/VE.py:96-183
 #include "common.cuh"
 
 namespace icon {
-
-struct ConvParams {
-    const float *x;      // [N][Cin][H][W]
-    const float *w;      // conv: [Cout][Cin][KH][KW]; transposed: [Cin][Cout][KH][KW]
-    const float *bias;   // [Cout] or null
-    const float *res;    // residual [N][Cout][OH][OW] or null
-    float *y;            // [N][Cout][OH][OW]
-    int N, Cin, H, W, Cout, OH, OW, KH, KW, stride, pad;
-    int reflect;         // 1: reflection padding (pad < H, W), 0: zero padding
-    int transposed;      // 1: ConvTranspose2d semantics (stride = upsampling factor)
-    int act;             // 0 none, 1 relu, 2 tanh
-};
-
-constexpr int CB_M = 64, CB_N = 128, CB_K = 16, CT = 256;
-
-// C[Cout][pixels] = W[Cout][K] * im2col[K][pixels], K = Cin*KH*KW in torch's (ci, kh, kw) order
-__global__ void __launch_bounds__(CT) k_conv2d(ConvParams p) {
-    __shared__ float As[CB_K][CB_M + 4];
-    __shared__ float Bs[CB_K][CB_N + 4];
-    const int tid = threadIdx.x;
-    const int K = p.Cin * p.KH * p.KW;
-    const int64_t npix = (int64_t)p.N * p.OH * p.OW;
-    const int64_t pix0 = (int64_t)blockIdx.x * CB_N;
-    const int m0 = blockIdx.y * CB_M;
-
-    // B loader: this thread always gathers the same output pixel, for 8 k-rows per tile
-    const int bp = tid % CB_N, bk0 = tid / CB_N;         // bk0 in {0,1}
-    const int64_t gp = pix0 + bp;
-    const bool pvalid = gp < npix;
-    int pn = 0, poy = 0, pox = 0;
-    if (pvalid) {
-        pn = (int)(gp / ((int64_t)p.OH * p.OW));
-        const int r = (int)(gp % ((int64_t)p.OH * p.OW));
-        poy = r / p.OW; pox = r % p.OW;
-    }
-    const float *xn = p.x + (size_t)pn * p.Cin * p.H * p.W;
-    // A loader: 64 x 16 weights per tile, 4 per thread
-    const int am = tid % CB_M, ak0 = tid / CB_M;          // ak0 in 0..3
-
-    // thread tile: 4 channels x 8 pixels
-    const int ty = tid / 16, tx = tid % 16;               // ty 0..15 -> channels ty*4.., tx -> pixels tx*8..
-    float acc[4][8];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-
-    const int khw = p.KH * p.KW;
-    for (int k0 = 0; k0 < K; k0 += CB_K) {
-        // ---- weights
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int kk = ak0 + 4 * j, k = k0 + kk, m = m0 + am;
-            float v = 0.f;
-            if (k < K && m < p.Cout) {
-                if (!p.transposed) v = __ldg(p.w + (size_t)m * K + k);
-                else {
-                    const int ci = k / khw, t = k % khw;
-                    v = __ldg(p.w + ((size_t)ci * p.Cout + m) * khw + t);
-                }
-            }
-            As[kk][am] = v;
-        }
-        // ---- im2col gather
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int kk = bk0 + 2 * j, k = k0 + kk;
-            float v = 0.f;
-            if (pvalid && k < K) {
-                const int ci = k / khw, t = k % khw, kh = t / p.KW, kw = t % p.KW;
-                int iy, ix;
-                bool ok = true;
-                if (!p.transposed) {
-                    iy = poy * p.stride - p.pad + kh;
-                    ix = pox * p.stride - p.pad + kw;
-                    if (p.reflect) {
-                        iy = iy < 0 ? -iy : (iy >= p.H ? 2 * p.H - 2 - iy : iy);
-                        ix = ix < 0 ? -ix : (ix >= p.W ? 2 * p.W - 2 - ix : ix);
-                    } else ok = iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-                } else {
-                    const int ty2 = poy + p.pad - kh, tx2 = pox + p.pad - kw;
-                    ok = ty2 >= 0 && tx2 >= 0 && (ty2 % p.stride) == 0 && (tx2 % p.stride) == 0;
-                    iy = ty2 / p.stride; ix = tx2 / p.stride;
-                    ok = ok && iy < p.H && ix < p.W;
-                }
-                if (ok) v = __ldg(xn + ((size_t)ci * p.H + iy) * p.W + ix);
-            }
-            Bs[kk][bp] = v;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < CB_K; ++kk) {
-            const float4 a = *reinterpret_cast<const float4 *>(&As[kk][ty * 4]);
-            const float4 b0 = *reinterpret_cast<const float4 *>(&Bs[kk][tx * 8]);
-            const float4 b1 = *reinterpret_cast<const float4 *>(&Bs[kk][tx * 8 + 4]);
-            const float av[4] = {a.x, a.y, a.z, a.w};
-            const float bv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-        }
-        __syncthreads();
-    }
-    // ---- epilogue: bias, residual, activation, NCHW store
-    const int64_t ohw = (int64_t)p.OH * p.OW;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int m = m0 + ty * 4 + i;
-        if (m >= p.Cout) continue;
-        const float b = p.bias ? __ldg(p.bias + m) : 0.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int64_t g = pix0 + tx * 8 + j;
-            if (g >= npix) continue;
-            const int n = (int)(g / ohw);
-            const int64_t r = g % ohw;
-            const size_t o = ((size_t)n * p.Cout + m) * ohw + r;
-            float v = acc[i][j] + b;
-            if (p.res) v += p.res[o];
-            if (p.act == 1) v = fmaxf(v, 0.f);
-            else if (p.act == 2) v = tanhf(v);
-            p.y[o] = v;
-        }
-    }
-}
-
-// ---------------------------------------------------------------- GroupNorm / InstanceNorm
-// one CTA per (sample, group); y = (x - mean) * rstd * gamma + beta, optional ReLU / residual add.
-// groups == C with gamma == null is InstanceNorm2d(affine=False).  Biased variance, two passes.
-__global__ void __launch_bounds__(512) k_group_norm(const float *__restrict__ x, const float *__restrict__ gamma,
-                                                    const float *__restrict__ beta, const float *__restrict__ res,
-                                                    float *__restrict__ y, int C, int HW, int groups, float eps,
-                                                    int relu) {
-    __shared__ float red[32];
-    __shared__ float s_mean, s_rstd;
-    const int n = blockIdx.x / groups, g = blockIdx.x % groups;
-    const int cpg = C / groups;
-    const size_t base = ((size_t)n * C + (size_t)g * cpg) * HW;
-    const int64_t cnt = (int64_t)cpg * HW;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    auto block_sum = [&](float v) {
-        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        __syncthreads();
-        if (lane == 0) red[wid] = v;
-        __syncthreads();
-        float t = (tid < (int)(blockDim.x >> 5)) ? red[tid] : 0.f;
-        if (wid == 0) {
-            for (int o = 16; o; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-            if (lane == 0) red[0] = t;
-        }
-        __syncthreads();
-        return red[0];
-    };
-    float s = 0.f;
-    for (int64_t i = tid; i < cnt; i += blockDim.x) s += x[base + i];
-    const float mean = block_sum(s) / (float)cnt;
-    float q = 0.f;
-    for (int64_t i = tid; i < cnt; i += blockDim.x) { const float d = x[base + i] - mean; q = fmaf(d, d, q); }
-    const float var = block_sum(q) / (float)cnt;
-    if (tid == 0) { s_mean = mean; s_rstd = rsqrtf(var + eps); }
-    __syncthreads();
-    const float rstd = s_rstd;
-    for (int64_t i = tid; i < cnt; i += blockDim.x) {
-        const int c = g * cpg + (int)(i / HW);
-        float v = (x[base + i] - s_mean) * rstd;
-        if (gamma) v = fmaf(v, __ldg(gamma + c), __ldg(beta + c));
-        if (res) v += res[base + i];
-        if (relu) v = fmaxf(v, 0.f);
-        y[base + i] = v;
-    }
-}
-
-// small groups (InstanceNorm at 32x32 .. 64x64): one WARP per (sample, group), values kept in registers,
-// shuffle reductions only.  cnt <= 32 * NV.
-template <int NV>
-__global__ void __launch_bounds__(256) k_group_norm_warp(const float *__restrict__ x, const float *__restrict__ gamma,
-                                                         const float *__restrict__ beta, const float *__restrict__ res,
-                                                         float *__restrict__ y, int C, int HW, int groups, float eps,
-                                                         int relu, int ngroups_total) {
-    const int gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (gw >= ngroups_total) return;
-    const int n = gw / groups, g = gw % groups, cpg = C / groups;
-    const size_t base = ((size_t)n * C + (size_t)g * cpg) * HW;
-    const int cnt = cpg * HW;
-    float v[NV];
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const int idx = lane + 32 * i;
-        v[i] = idx < cnt ? x[base + idx] : 0.f;
-        s += v[i];
-    }
-    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    const float mean = s / (float)cnt;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const float d = (lane + 32 * i < cnt) ? v[i] - mean : 0.f;
-        q = fmaf(d, d, q);
-    }
-    for (int o = 16; o; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-    const float rstd = rsqrtf(q / (float)cnt + eps);
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-        const int idx = lane + 32 * i;
-        if (idx >= cnt) continue;
-        float o = (v[i] - mean) * rstd;
-        if (gamma) { const int c = g * cpg + idx / HW; o = fmaf(o, __ldg(gamma + c), __ldg(beta + c)); }
-        if (res) o += res[base + idx];
-        if (relu) o = fmaxf(o, 0.f);
-        y[base + idx] = o;
-    }
-}
-
-// large groups: statistics by many CTAs per group (fp32 block partials, fp64 atomics), then a flat apply pass
-__global__ void __launch_bounds__(256) k_norm_stats(const float *__restrict__ x, int C, int HW, int groups, int slices,
-                                                    double *__restrict__ stats) {
-    __shared__ float rs[8], rq[8];
-    const int gi = blockIdx.x / slices, sl = blockIdx.x % slices;
-    const int n = gi / groups, g = gi % groups, cpg = C / groups;
-    const size_t base = ((size_t)n * C + (size_t)g * cpg) * HW;
-    const int64_t cnt = (int64_t)cpg * HW;
-    const int64_t per = (cnt + slices - 1) / slices, lo = sl * per, hi = min(cnt, lo + per);
-    float s = 0.f, q = 0.f;
-    for (int64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) { const float t = x[base + i]; s += t; q = fmaf(t, t, q); }
-    for (int o = 16; o; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); q += __shfl_xor_sync(0xffffffffu, q, o); }
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (lane == 0) { rs[wid] = s; rq[wid] = q; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double ds = 0.0, dq = 0.0;
-        for (int w = 0; w < 8; ++w) { ds += (double)rs[w]; dq += (double)rq[w]; }
-        atomicAdd(&stats[2 * gi], ds);
-        atomicAdd(&stats[2 * gi + 1], dq);
-    }
-}
-// sums -> (mean, rstd) per group, in place and in double as before; done once per group instead of once per element
-__global__ void k_norm_finalize(double *__restrict__ stats, int ng, double cnt, float eps) {
-    const int gi = blockIdx.x * blockDim.x + threadIdx.x;
-    if (gi >= ng) return;
-    const double mean = stats[2 * gi] / cnt;
-    const double var = fmax(stats[2 * gi + 1] / cnt - mean * mean, 0.0);
-    stats[2 * gi] = (double)(float)mean;
-    stats[2 * gi + 1] = (double)(float)(1.0 / sqrt(var + (double)eps));
-}
-
-// one (n, c) plane per blockIdx.x, 1024-element segments along blockIdx.y: the group statistics and the affine
-// pair are block-uniform, the element loop is a float4 stream
-__global__ void __launch_bounds__(256) k_norm_apply(const float *__restrict__ x, const double *__restrict__ stats,
-                                                    const float *__restrict__ gamma, const float *__restrict__ beta,
-                                                    const float *__restrict__ res, float *__restrict__ y, int C, int HW,
-                                                    int groups, int relu) {
-    const int plane = blockIdx.x, c = plane % C, n = plane / C;
-    const int gi = n * groups + c / (C / groups);
-    const float mean = (float)stats[2 * gi], rstd = (float)stats[2 * gi + 1];
-    const bool affine = gamma != nullptr;
-    const float g = affine ? __ldg(gamma + c) : 1.f, bt = affine ? __ldg(beta + c) : 0.f;
-    const size_t base = (size_t)plane * HW;
-    auto f = [&](float v, float r) {
-        float o = (v - mean) * rstd;
-        if (affine) o = fmaf(o, g, bt);
-        o += r;
-        return relu ? fmaxf(o, 0.f) : o;
-    };
-    const int i0 = (blockIdx.y * 256 + threadIdx.x) * 4;
-    if (i0 >= HW) return;
-    if ((HW & 3) == 0) {
-        const float4 v = *reinterpret_cast<const float4 *>(x + base + i0);
-        float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (res) r = *reinterpret_cast<const float4 *>(res + base + i0);
-        *reinterpret_cast<float4 *>(y + base + i0) = make_float4(f(v.x, r.x), f(v.y, r.y), f(v.z, r.z), f(v.w, r.w));
-    } else {
-        for (int i = i0; i < min(i0 + 4, HW); ++i) y[base + i] = f(x[base + i], res ? res[base + i] : 0.f);
-    }
-}
-
-// ---------------------------------------------------------------- pooling / resampling / joins
-__global__ void k_avg_pool2(const float *__restrict__ x, float *__restrict__ y, int64_t planes, int H, int W) {
-    const int OH = H / 2, OW = W / 2;
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= planes * OH * OW) return;
-    const int ox = (int)(i % OW), oy = (int)((i / OW) % OH);
-    const int64_t pl = i / ((int64_t)OW * OH);
-    const float *s = x + (size_t)pl * H * W + (size_t)(2 * oy) * W + 2 * ox;
-    y[i] = (s[0] + s[1] + s[W] + s[W + 1]) * 0.25f;
-}
-
-__device__ __forceinline__ void cubic_w(float t, float (&w)[4]) {     // torch upsample_bicubic2d, A = -0.75
-    const float A = -0.75f;
-    float x;
-    x = t + 1.f; w[0] = ((A * x - 5.f * A) * x + 8.f * A) * x - 4.f * A;
-    x = t;       w[1] = ((A + 2.f) * x - (A + 3.f)) * x * x + 1.f;
-    x = 1.f - t; w[2] = ((A + 2.f) * x - (A + 3.f)) * x * x + 1.f;
-    x = 2.f - t; w[3] = ((A * x - 5.f * A) * x + 8.f * A) * x - 4.f * A;
-}
-
-// y = add + interpolate(x, scale 2, bicubic, align_corners=True)   (HGFilters.py:70-76)
-__global__ void k_bicubic_up2_add(const float *__restrict__ x, const float *__restrict__ add, float *__restrict__ y,
-                                  int64_t planes, int H, int W) {
-    const int OH = 2 * H, OW = 2 * W;
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= planes * OH * OW) return;
-    const int ox = (int)(i % OW), oy = (int)((i / OW) % OH);
-    const int64_t pl = i / ((int64_t)OW * OH);
-    const float sy = OH > 1 ? (float)(H - 1) / (float)(OH - 1) : 0.f, sx = OW > 1 ? (float)(W - 1) / (float)(OW - 1) : 0.f;
-    const float fy = sy * oy, fx = sx * ox;
-    const int iy = (int)floorf(fy), ix = (int)floorf(fx);
-    float wy[4], wx[4];
-    cubic_w(fy - iy, wy);
-    cubic_w(fx - ix, wx);
-    const float *s = x + (size_t)pl * H * W;
-    float out = 0.f;
-#pragma unroll
-    for (int a = 0; a < 4; ++a) {
-        const int yy = min(max(iy - 1 + a, 0), H - 1);
-        float row = 0.f;
-#pragma unroll
-        for (int b = 0; b < 4; ++b) {
-            const int xx = min(max(ix - 1 + b, 0), W - 1);
-            row = fmaf(s[(size_t)yy * W + xx], wx[b], row);
-        }
-        out = fmaf(row, wy[a], out);
-    }
-    y[i] = out + (add ? add[i] : 0.f);
-}
-
-// y[n][c] = (c < C1 ? a : c < C1+C2 ? b : c3)[...] + res   (ConvBlock: cat(out1,out2,out3) + residual)
-__global__ void k_cat3_add(const float *__restrict__ a, const float *__restrict__ b, const float *__restrict__ c3,
-                           const float *__restrict__ res, float *__restrict__ y, int N, int C1, int C2, int C3, int64_t HW) {
-    const int C = C1 + C2 + C3;
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (int64_t)N * C * HW) return;
-    const int64_t r = i % HW;
-    const int c = (int)((i / HW) % C), n = (int)(i / (HW * C));
-    float v;
-    if (c < C1) v = a[((size_t)n * C1 + c) * HW + r];
-    else if (c < C1 + C2) v = b[((size_t)n * C2 + (c - C1)) * HW + r];
-    else v = c3[((size_t)n * C3 + (c - C1 - C2)) * HW + r];
-    y[i] = v + res[i];
-}
-
-__global__ void k_add3(const float *__restrict__ a, const float *__restrict__ b, const float *__restrict__ c,
-                       float *__restrict__ y, int64_t n) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) y[i] = a[i] + b[i] + c[i];
-}
 
 // NormalNet.py:88-97: y = x / ||x||_2 over the 3 channels (no eps) * (sum_c |image| != 0)
 __global__ void k_normalize_mask(const float *__restrict__ x, const float *__restrict__ image, float *__restrict__ y,
@@ -378,98 +25,6 @@ __global__ void k_normalize_mask(const float *__restrict__ x, const float *__res
 }  // namespace icon
 
 using namespace icon;
-
-extern "C" int icon_conv2d(const float *x, const float *w, const float *bias, const float *res, float *y, int N,
-                           int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int out_pad,
-                           int reflect, int transposed, int act, icon_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(x && w && y && N > 0 && Cin > 0 && Cout > 0 && H > 0 && W > 0 && KH > 0 && KW > 0 && stride > 0,
-                   "icon_conv2d: bad argument");
-    ICON_CHECK_ARG(!reflect || (pad < H && pad < W && !transposed), "icon_conv2d: reflection pad %d needs pad < H, W", pad);
-    ConvParams p{};
-    p.x = x; p.w = w; p.bias = bias; p.res = res; p.y = y;
-    p.N = N; p.Cin = Cin; p.H = H; p.W = W; p.Cout = Cout; p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad;
-    p.reflect = reflect; p.transposed = transposed; p.act = act;
-    if (!transposed) {
-        p.OH = (H + 2 * pad - KH) / stride + 1;
-        p.OW = (W + 2 * pad - KW) / stride + 1;
-    } else {
-        p.OH = (H - 1) * stride - 2 * pad + KH + out_pad;
-        p.OW = (W - 1) * stride - 2 * pad + KW + out_pad;
-    }
-    ICON_CHECK_ARG(p.OH > 0 && p.OW > 0, "icon_conv2d: empty output");
-    const int64_t npix = (int64_t)N * p.OH * p.OW;
-    dim3 grid((unsigned)((npix + CB_N - 1) / CB_N), (unsigned)((Cout + CB_M - 1) / CB_M));
-    k_conv2d<<<grid, CT, 0, stream>>>(p);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
-
-extern "C" int icon_group_norm(const float *x, const float *gamma, const float *beta, const float *res, float *y,
-                               int N, int C, int HW, int groups, float eps, int relu, void *stats_ws,
-                               icon_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(x && y && N > 0 && C > 0 && HW > 0 && groups > 0 && C % groups == 0, "icon_group_norm: bad argument");
-    ICON_CHECK_ARG((gamma == nullptr) == (beta == nullptr), "icon_group_norm: gamma and beta go together");
-    const int64_t cnt = (int64_t)(C / groups) * HW;
-    const int ng = N * groups;
-    if (cnt <= 32 * 32) {
-        k_group_norm_warp<32><<<(ng + 7) / 8, 256, 0, stream>>>(x, gamma, beta, res, y, C, HW, groups, eps, relu, ng);
-    } else if (cnt <= 32 * 128 && ng >= 296) {
-        k_group_norm_warp<128><<<(ng + 7) / 8, 256, 0, stream>>>(x, gamma, beta, res, y, C, HW, groups, eps, relu, ng);
-    } else if (stats_ws && (int64_t)ng * 4 < 592) {
-        // few large groups: spread each over several CTAs
-        int slices = (int)min((int64_t)64, max((int64_t)1, (int64_t)1184 / ng));
-        ICON_CUDA(cudaMemsetAsync(stats_ws, 0, sizeof(double) * 2 * ng, stream));
-        k_norm_stats<<<ng * slices, 256, 0, stream>>>(x, C, HW, groups, slices, (double *)stats_ws);
-        ICON_LAUNCHED();
-        k_norm_finalize<<<(ng + 127) / 128, 128, 0, stream>>>((double *)stats_ws, ng, (double)cnt, eps);
-        ICON_LAUNCHED();
-        k_norm_apply<<<dim3((unsigned)(N * C), (unsigned)((HW + 1023) / 1024)), 256, 0, stream>>>(
-            x, (const double *)stats_ws, gamma, beta, res, y, C, HW, groups, relu);
-    } else {
-        k_group_norm<<<ng, 512, 0, stream>>>(x, gamma, beta, res, y, C, HW, groups, eps, relu);
-    }
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
-
-extern "C" int icon_avg_pool2(const float *x, float *y, int64_t planes, int H, int W, icon_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(x && y && planes > 0 && H >= 2 && W >= 2, "icon_avg_pool2: bad argument");
-    const int64_t n = planes * (H / 2) * (W / 2);
-    k_avg_pool2<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(x, y, planes, H, W);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
-
-extern "C" int icon_bicubic_up2_add(const float *x, const float *add, float *y, int64_t planes, int H, int W,
-                                    icon_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(x && y && planes > 0 && H > 0 && W > 0, "icon_bicubic_up2_add: bad argument");
-    const int64_t n = planes * 4 * H * W;
-    k_bicubic_up2_add<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(x, add, y, planes, H, W);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
-
-extern "C" int icon_cat3_add(const float *a, const float *b, const float *c, const float *res, float *y, int N, int C1,
-                             int C2, int C3, int64_t HW, icon_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(a && b && c && res && y, "icon_cat3_add: null pointer");
-    const int64_t n = (int64_t)N * (C1 + C2 + C3) * HW;
-    k_cat3_add<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(a, b, c, res, y, N, C1, C2, C3, HW);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
-
-extern "C" int icon_add3(const float *a, const float *b, const float *c, float *y, int64_t n, icon_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(a && b && c && y && n > 0, "icon_add3: bad argument");
-    k_add3<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(a, b, c, y, n);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
 
 extern "C" int icon_normalize_mask(const float *x, const float *image, float *y, int N, int Cimg, int64_t HW,
                                    icon_stream_t stream_) {

@@ -1,5 +1,5 @@
 // Hopper (sm_90a) tensor-core and TMA / mbarrier PTX wrappers shared by the tensor-core kernels
-// (mlp_tc.cu, conv_tc.cu, conv_nhwc.cu).
+// (mlp_tc.cu, conv_nhwc.cu).
 //
 // wgmma: one warpgroup (4 consecutive warps, 128 threads) computes D[64][N] (+)= A[64][16] * B[N][16]^T per instruction,
 // fp16 inputs, fp32 accumulator in registers.  Accumulator fragment of thread t (warp w = (t >> 5) & 3, lane l):

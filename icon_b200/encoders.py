@@ -1,11 +1,15 @@
 """Image / volume encoders of the hot path: parameter containers with the reference's exact
-state_dict keys and shapes, and forwards that run the hand-written conv kernels
-(icon_b200.conv_ops -> libicon_b200.so).
+state_dict keys and shapes, and forwards that run hand-written kernels of libicon_b200.so: the
+2-D encoders on the NHWC path (icon_b200.nhwc), NormalNet's normalisation and the volume encoder
+through icon_b200.conv_ops.
 
   ConvBlock, HourGlass, HGFilter   lib/net/net_util.py:224-280, lib/net/HGFilters.py:23-197
   ResnetBlock, GlobalGenerator     lib/net/FBNet.py:202-319
   NormalNet                        lib/net/NormalNet.py:39-99
   Residual3D, VolumeEncoder        lib/net/VE.py:56-183
+
+HGFilter and GlobalGenerator take the input sizes ICON produces (512 x 512 crops) and raise
+NotImplementedError for the others (see their forward).
 """
 import torch
 import torch.nn as nn
@@ -43,18 +47,8 @@ class ConvBlock(nn.Module):
             self.downsample = None
 
     def forward(self, x):
-        C = _conv_ops()
-        out1 = C.conv2d(C.group_norm(x, self.bn1, relu=True), self.conv1)
-        out2 = C.conv2d(C.group_norm(out1, self.bn2, relu=True), self.conv2)
-        out3 = C.conv2d(C.group_norm(out2, self.bn3, relu=True), self.conv3)
-        residual = x
-        if self.downsample is not None:
-            residual = C.conv2d(C.group_norm(x, self.bn4, relu=True), self.downsample[2])
-        return C.cat_add((out1, out2, out3), residual)
-
-    def forward_nhwc(self, x):
-        """Same block on the NHWC path: x = nhwc.Raw with statistics; the three convs write their channel slices
-        of ONE output tensor (torch.cat for free), every GroupNorm reads the sums its producer accumulated."""
+        """x = nhwc.Raw with statistics -> nhwc.Raw; the three convs write their channel slices of ONE output tensor
+        (torch.cat for free), every GroupNorm reads the sums its producer accumulated."""
         from . import nhwc as T
         c1, c2, c3 = self.conv1.out_channels, self.conv2.out_channels, self.conv3.out_channels
         y = torch.empty(x.N, x.H, x.W, c1 + c2 + c3, dtype=torch.float32, device=x.t.device)
@@ -100,35 +94,28 @@ class HourGlass(nn.Module):
             self.add_module("b2_plus_" + str(level), ConvBlock(self.features, self.features, self.opt))
         self.add_module("b3_" + str(level), ConvBlock(self.features, self.features, self.opt))
 
-    def _forward(self, level, inp):
-        C = _conv_ops()
-        up1 = self._modules["b1_" + str(level)](inp)
-        low1 = self._modules["b2_" + str(level)](C.avg_pool2(inp))
-        if level > 1:
-            low2 = self._forward(level - 1, low1)
-        else:
-            low2 = self._modules["b2_plus_" + str(level)](low1)
-        low3 = self._modules["b3_" + str(level)](low2)
-        return C.bicubic_up2_add(low3, up1)          # up1 + interpolate(low3, x2, bicubic, align_corners)
-
     def forward(self, x):
-        return self._forward(self.depth, x)
+        """NCHW fp32 in and out, like the reference's HourGlass.forward; the block itself runs on the NHWC path."""
+        from . import nhwc as T
+        with torch.no_grad(), T.stats_arena(x.device):
+            return T.to_nchw(self._forward(self.depth, T.raw_from_nchw(x)))
 
-    def forward_nhwc(self, level, inp):
+    def _forward(self, level, inp):
+        """nhwc.Raw with statistics -> nhwc.Raw."""
         from . import nhwc as T
         from .graphs import run_pair
 
         def low_path():
-            low1 = self._modules["b2_" + str(level)].forward_nhwc(T.avg_pool2(inp.dense()))
+            low1 = self._modules["b2_" + str(level)](T.avg_pool2(inp.dense()))
             if level > 1:
-                low2 = self.forward_nhwc(level - 1, low1)
+                low2 = self._forward(level - 1, low1)
             else:
-                low2 = self._modules["b2_plus_" + str(level)].forward_nhwc(low1)
-            return self._modules["b3_" + str(level)].forward_nhwc(low2)
+                low2 = self._modules["b2_plus_" + str(level)](low1)
+            return self._modules["b3_" + str(level)](low2)
 
         # the skip branch (one ConvBlock at full resolution) and the whole low-resolution path are independent until
         # the final add: two streams (inside the captured graph: two parallel branches)
-        low3, up1 = run_pair(low_path, lambda: self._modules["b1_" + str(level)].forward_nhwc(inp))
+        low3, up1 = run_pair(low_path, lambda: self._modules["b1_" + str(level)](inp))
         return T.bicubic_up2_add(low3.dense(), up1.dense())
 
 
@@ -158,49 +145,32 @@ class HGFilter(nn.Module):
                 self.add_module("al" + str(hg_module), nn.Conv2d(opt.hourglass_dim, 256, kernel_size=1, stride=1, padding=0))
 
     def forward(self, x):
+        # the stem and the pool halve the image, then every hourglass level halves it again
+        step = 1 << (self.opt.num_hourglass + 2)
+        H, W = x.shape[-2:]
+        if H % step or W % step:
+            raise NotImplementedError(f"HGFilter: H and W must be multiples of {step} = 2^(num_hourglass + 2), "
+                                      f"got {H} x {W}")
+        # checked before the graph wrapper: an exception while capturing would turn CUDA graphs off for this module
         if not hasattr(self, "_graphed"):
             object.__setattr__(self, "_graphed", GraphedForward(self, "_forward_eager"))
-        return self._graphed(x, extra=_conv_ops()._IMPL)
+        return self._graphed(x)
 
     def _forward_eager(self, x):
-        C = _conv_ops()
-        if C._IMPL == "auto" and x.shape[2] % 16 == 0 and x.shape[3] % 16 == 0:
-            return self._forward_nhwc(x)
-        with torch.no_grad():
-            x = C.group_norm(C.conv2d(x, self.conv1), self.bn1, relu=True)
-            x = C.avg_pool2(self.conv2(x))
-            x = self.conv3(x)
-            x = self.conv4(x)
-            previous = x
-            outputs = []
-            for i in range(self.num_modules):
-                hg = self._modules["m" + str(i)](previous)
-                ll = self._modules["top_m_" + str(i)](hg)
-                ll = C.group_norm(C.conv2d(ll, self._modules["conv_last" + str(i)]),
-                                  self._modules["bn_end" + str(i)], relu=True)
-                tmp_out = C.conv2d(ll, self._modules["l" + str(i)])
-                outputs.append(tmp_out)
-                if i < self.num_modules - 1:
-                    ll = C.conv2d(ll, self._modules["bl" + str(i)])
-                    tmp_out_ = C.conv2d(tmp_out, self._modules["al" + str(i)])
-                    previous = C.add3(previous, ll, tmp_out_)
-        return outputs
-
-    def _forward_nhwc(self, x):
         """HGFilters.py:161-197 on the NHWC / TMA / wgmma path (icon_b200/nhwc.py), 7x7 stride-2 stem included."""
         from . import nhwc as T
         with torch.no_grad(), T.stats_arena(x.device):
             r = T.stem_conv7(x, self.conv1, reflect=False)                       # 7x7 s2 on the tensor cores, [N,H/2,W/2,64]
             x = T.norm_relu(r, T.finalize(r, self.bn1))                          # + statistics for conv2.bn1
-            x = T.avg_pool2(self.conv2.forward_nhwc(x).dense())
-            x = self.conv3.forward_nhwc(x)
-            x = self.conv4.forward_nhwc(x)
+            x = T.avg_pool2(self.conv2(x).dense())
+            x = self.conv3(x)
+            x = self.conv4(x)
             previous = x
             outputs = []
             for i in range(self.num_modules):
                 m = self._modules["m" + str(i)]
-                hg = m.forward_nhwc(m.depth, previous)
-                ll = self._modules["top_m_" + str(i)].forward_nhwc(hg)
+                hg = m._forward(m.depth, previous)
+                ll = self._modules["top_m_" + str(i)](hg)
                 op, _ = T.act(ll)                                                # conv_last reads ll itself (no norm)
                 r = T.conv(op, self._modules["conv_last" + str(i)])
                 op_ll, _ = T.act(r, T.finalize(r, self._modules["bn_end" + str(i)]), relu=True)
@@ -219,7 +189,8 @@ class HGFilter(nn.Module):
 
 # ------------------------------------------------------------------------ pix2pixHD generator
 class ResnetBlock(nn.Module):
-    """FBNet.py:268-319 (padding 'reflect', InstanceNorm2d affine=False, no dropout)."""
+    """FBNet.py:268-319 (padding 'reflect', InstanceNorm2d affine=False, no dropout).  Parameter container only:
+    GlobalGenerator runs its two convolutions on the NHWC path."""
 
     def __init__(self, dim):
         super().__init__()
@@ -229,18 +200,13 @@ class ResnetBlock(nn.Module):
             nn.ReflectionPad2d(1), nn.Conv2d(dim, dim, kernel_size=3, padding=0),
             nn.InstanceNorm2d(dim, affine=False))
 
-    def forward(self, x):
-        C = _conv_ops()
-        y = C.instance_norm(C.conv2d(x, self.conv_block[1], reflect=1), relu=True)
-        y = C.instance_norm(C.conv2d(y, self.conv_block[5], reflect=1), relu=False, residual=x)
-        return y
-
 
 class GlobalGenerator(nn.Module):
     """FBNet.py:202-264 with define_G(…, 'instance') as NormalNet builds it (NormalNet.py:67-70)."""
 
     def __init__(self, input_nc, output_nc, ngf=64, n_downsampling=3, n_blocks=9, last_op=nn.Tanh()):
         super().__init__()
+        self.ngf, self.output_nc = ngf, output_nc
         self.n_downsampling, self.n_blocks = n_downsampling, n_blocks
         act = nn.ReLU(True)
         model = [nn.ReflectionPad2d(3), nn.Conv2d(input_nc, ngf, kernel_size=7, padding=0),
@@ -263,37 +229,25 @@ class GlobalGenerator(nn.Module):
         self.model = nn.Sequential(*model)
 
     def forward(self, x):
+        # every downsampling halves the image, and the innermost one must keep a reflection halo of 1 inside the image
+        step = 1 << self.n_downsampling
+        H, W = x.shape[-2:]
+        if H % step or W % step or H < 2 * step or W < 2 * step:
+            raise NotImplementedError(f"GlobalGenerator: H and W must be multiples of {step} = 2^n_downsampling and at "
+                                      f"least {2 * step}, got {H} x {W}")
+        if self.ngf != 64 or self.output_nc > 3:
+            raise NotImplementedError(f"GlobalGenerator: ngf == 64 and output_nc <= 3 (NormalNet's generators), got "
+                                      f"ngf = {self.ngf}, output_nc = {self.output_nc}")
+        # checked before the graph wrapper: an exception while capturing would turn CUDA graphs off for this module
         if not hasattr(self, "_graphed"):
             object.__setattr__(self, "_graphed", GraphedForward(self, "_forward_eager"))
-        return self._graphed(x, extra=_conv_ops()._IMPL)
+        return self._graphed(x)
 
     def _forward_eager(self, x):
-        C = _conv_ops()
-        m = self.model
-        if (C._IMPL == "auto" and x.shape[2] % (1 << self.n_downsampling) == 0 and x.shape[3] % (1 << self.n_downsampling) == 0
-                and m[1].out_channels == 64 and m[-2 if isinstance(m[-1], nn.Tanh) else -1].out_channels <= 3
-                and (x.shape[2] >> self.n_downsampling) >= 2 and (x.shape[3] >> self.n_downsampling) >= 2):
-            return self._forward_nhwc(x)
-        with torch.no_grad():
-            y = C.instance_norm(C.conv2d(x, m[1], reflect=3), relu=True)
-            idx = 4
-            for _ in range(self.n_downsampling):
-                y = C.instance_norm(C.conv2d(y, m[idx]), relu=True)
-                idx += 3
-            for _ in range(self.n_blocks):
-                y = m[idx](y)
-                idx += 1
-            for _ in range(self.n_downsampling):
-                y = C.instance_norm(C.conv_transpose2d(y, m[idx]), relu=True)
-                idx += 3
-            y = C.conv2d(y, m[idx + 1], reflect=3, tanh=(len(m) > idx + 2))
-        return y
-
-    def _forward_nhwc(self, x):
         """FBNet.py:216-264 on the NHWC / TMA / wgmma path: every InstanceNorm reads the sums its producing conv
         accumulated; ReflectionPad2d = halo written by the normalising pass; stride-2 convs read space-to-depth
         planes; ConvTranspose2d = 4 output phases; the 7x7 stem (Cin = 6) runs its K axis over filter rows; the 64 -> 3
-        head is FP32 (k_conv7_head)."""
+        head is a 1x1 tensor-core GEMM followed by col2im (k_col2im7)."""
         from . import nhwc as T
         m = self.model
         nd, nb = self.n_downsampling, self.n_blocks

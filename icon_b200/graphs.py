@@ -97,17 +97,17 @@ class GraphedForward:
         import copy
         return GraphedForward(copy.deepcopy(self.module, memo), self.method)
 
-    def _key(self, x, extra):
+    def _key(self, x):
         m = self.module
         weights = tuple((t.data_ptr(), t._version) for t in list(m.parameters()) + list(m.buffers()))
-        return (tuple(x.shape), x.dtype, str(x.device), extra, _SLOT[0], weights)
+        return (tuple(x.shape), x.dtype, str(x.device), _SLOT[0], weights)
 
-    def __call__(self, x, extra=None):
+    def __call__(self, x):
         usable = (_ENABLED and not self.disabled and x.is_cuda and not self.module.training
                   and not torch.cuda.is_current_stream_capturing())
         if not usable:
             return self.fn(x)
-        key = self._key(x, extra)
+        key = self._key(x)
         if key not in self.entries:
             if len(self.entries) >= MAX_GRAPHS_PER_MODULE:
                 self.entries.clear()

@@ -177,29 +177,35 @@ def _n_tile(cout):
     return 256 if cout > 128 else (128 if cout > 64 else 64)
 
 
-def packed_weight(conv, transposed, cin_pad, n_tile):
-    """torch conv weight -> device blob of K-major SWIZZLE_128B fp16 hi / lo tiles, chunk = (tap, 64-channel block).
-    Cached ON the module (the blob must live as long as any CUDA graph that captured its address: ADVICE r1)."""
-    w = conv.weight
-    key = (w.data_ptr(), w._version, str(w.device), bool(transposed), cin_pad, n_tile)
-    cache = conv.__dict__.setdefault("_icon_pack", {})
-    hit = cache.get(key)
-    if hit is not None:
-        return hit
-    wd = w.detach().float()
-    if transposed:                                   # [Cin, Cout, KH, KW] -> [Cout, taps, Cin]
-        w3 = wd.permute(1, 2, 3, 0).reshape(wd.shape[1], -1, wd.shape[0])
-    else:                                            # [Cout, Cin, KH, KW] -> [Cout, taps, Cin]
-        w3 = wd.permute(0, 2, 3, 1).reshape(wd.shape[0], -1, wd.shape[1])
-    cout, taps, cin = w3.shape
-    if cin_pad != cin:
-        w3 = torch.cat([w3, torch.zeros(cout, taps, cin_pad - cin, device=w3.device)], 2)
-    w2 = w3.reshape(cout, taps * cin_pad)
-    blob = pack_tiles(w2, n_tile)
-    for k in [k for k in cache if k[:3] != key[:3]]:          # weights changed: drop the stale blobs of this module
-        del cache[k]
-    cache[key] = blob
+def _cached_blob(m, variant, build):
+    """Packed-weight blob of module `m` for `variant` (a tuple), made by `build()` on a miss.  Cached ON the module (the
+    blob must live as long as any CUDA graph that captured its address), keyed on the weight's storage address, version
+    and device: when the weights change, this module's stale blobs are dropped."""
+    w = m.weight
+    key = (w.data_ptr(), w._version, str(w.device)) + variant
+    cache = m.__dict__.setdefault("_icon_pack", {})
+    blob = cache.get(key)
+    if blob is None:
+        blob = build()
+        for k in [k for k in cache if k[:3] != key[:3]]:
+            del cache[k]
+        cache[key] = blob
     return blob
+
+
+def packed_weight(conv, transposed, cin_pad, n_tile):
+    """torch conv weight -> device blob of K-major SWIZZLE_128B fp16 hi / lo tiles, chunk = (tap, 64-channel block)."""
+    def build():
+        wd = conv.weight.detach().float()
+        if transposed:                               # [Cin, Cout, KH, KW] -> [Cout, taps, Cin]
+            w3 = wd.permute(1, 2, 3, 0).reshape(wd.shape[1], -1, wd.shape[0])
+        else:                                        # [Cout, Cin, KH, KW] -> [Cout, taps, Cin]
+            w3 = wd.permute(0, 2, 3, 1).reshape(wd.shape[0], -1, wd.shape[1])
+        cout, taps, cin = w3.shape
+        if cin_pad != cin:
+            w3 = torch.cat([w3, torch.zeros(cout, taps, cin_pad - cin, device=w3.device)], 2)
+        return pack_tiles(w3.reshape(cout, taps * cin_pad), n_tile)
+    return _cached_blob(conv, (bool(transposed), cin_pad, n_tile), build)
 
 
 def pack_tiles(w2, n_tile):
@@ -387,16 +393,12 @@ def stem_conv7(x, m, reflect, stats=True):
           "icon_stem_pack")
     cpt = Cp8 // 8                                              # 64-wide chunks per tap row
     n_tile = _n_tile(Cout)
-    key = (w.data_ptr(), w._version, str(w.device), "stem", Cp8, n_tile)
-    cache = m.__dict__.setdefault("_icon_pack", {})
-    blob = cache.get(key)
-    if blob is None:
+
+    def build():
         wk = torch.zeros(Cout, 7, 8, Cp8, dtype=torch.float32, device=w.device)      # [co][ky][kx (8th = 0)][c]
         wk[:, :, :7, :Cin] = w.detach().float().permute(0, 2, 3, 1)
-        blob = pack_tiles(wk.reshape(Cout, 7 * 8 * Cp8), n_tile)
-        for k in [k for k in cache if k[:3] != key[:3]]:
-            del cache[k]
-        cache[key] = blob
+        return pack_tiles(wk.reshape(Cout, 7 * 8 * Cp8), n_tile)
+    blob = _cached_blob(m, ("stem", Cp8, n_tile), build)
     out = torch.empty(N, OH, OW, Cout, dtype=torch.float32, device=dev)
     st = new_stats(N, Cout, dev) if stats else None
     bias = m.bias.detach().float().contiguous() if m.bias is not None else None
@@ -489,32 +491,16 @@ def conv7_head(op, m, tanh):
     dev = op.hi.device
     ncol = 49 * Cout
     n_tile = _n_tile(ncol)
-    key = (w.data_ptr(), w._version, str(w.device), "head", op.Cp, n_tile)
-    cache = m.__dict__.setdefault("_icon_pack", {})
-    blob = cache.get(key)
-    if blob is None:
+
+    def build():
         w2 = torch.zeros(ncol, op.Cp, dtype=torch.float32, device=w.device)          # row (ky*7+kx)*Cout + co
         w2[:, :Cin] = w.detach().float().permute(2, 3, 0, 1).reshape(ncol, Cin)
-        blob = pack_tiles(w2, n_tile)
-        for k in [k for k in cache if k[:3] != key[:3]]:
-            del cache[k]
-        cache[key] = blob
+        return pack_tiles(w2, n_tile)
+    blob = _cached_blob(m, ("head", op.Cp, n_tile), build)
     Ps = (ncol + 3) // 4 * 4
     P = torch.empty(op.N, op.H, op.W, Ps, dtype=torch.float32, device=dev)
     _launch(op, blob, op.Cp // 64, None, P, 0, ncol, op.H, op.W, 1, 1, 0, 0, [(0, 0, 0, 0)], op.Cp // 64, n_tile, None)
     y = torch.empty(op.N, Cout, op.H, op.W, dtype=torch.float32, device=dev)
     b = m.bias.detach().float().contiguous() if m.bias is not None else None
     check(lib.icon_col2im7(_p(P), _p(b), _p(y), op.N, op.H, op.W, Cout, Ps, 2 if tanh else 0, _stream()), "icon_col2im7")
-    return y
-
-
-def conv7_head_fp32(x_f32, m, tanh):
-    """ReflectionPad2d(3) + Conv2d(64, <= 3, 7) (+ Tanh) from fp32 NHWC to NCHW (FBNet.py:258-261)."""
-    N, H, W, C = x_f32.shape
-    w = m.weight.detach().float().contiguous()
-    Cout = w.shape[0]
-    y = torch.empty(N, Cout, H, W, dtype=torch.float32, device=x_f32.device)
-    b = m.bias.detach().float().contiguous() if m.bias is not None else None
-    check(lib.icon_conv7_head(_p(x_f32), _p(w), _p(b), _p(y), N, H, W, C, Cout, 2 if tanh else 0, _stream()),
-          "icon_conv7_head")
     return y

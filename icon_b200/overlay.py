@@ -53,8 +53,9 @@ def _patches():
         def define_G(input_nc, output_nc, ngf, netG, n_downsample_global=3, n_blocks_global=9, n_local_enhancers=1,
                      n_blocks_local=3, norm="instance", gpu_ids=[], last_op=nn.Tanh()):
             """lib/net/FBNet.py:52-90: the one configuration the path builds (NormalNet.py:67-70: 'global' +
-            'instance') returns the icon_b200 generator; everything else is the reference's own."""
-            if netG == "global" and norm == "instance":
+            'instance', ngf 64, at most 3 output channels) returns the icon_b200 generator; everything else is the
+            reference's own."""
+            if netG == "global" and norm == "instance" and ngf == 64 and output_nc <= 3:
                 return encoders.GlobalGenerator(input_nc, output_nc, ngf, n_downsample_global, n_blocks_global, last_op)
             return reference_define_G(input_nc, output_nc, ngf, netG, n_downsample_global, n_blocks_global,
                                       n_local_enhancers, n_blocks_local, norm, gpu_ids, last_op)

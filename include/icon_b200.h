@@ -198,26 +198,18 @@ size_t icon_visibility_workspace_bytes(int image_size);
 int icon_visibility(const float *xyz, int V, const int64_t *faces, int F, int image_size, float *vis,
                     void *ws, size_t ws_bytes, icon_stream_t stream);
 
-/* ------------------------------------------------------------------ encoder operators (NCHW fp32)
- * Replace the cuDNN / torch calls inside HGFilter (lib/net/HGFilters.py:161-197, ConvBlock
- * lib/net/net_util.py:258-280), GlobalGenerator / ResnetBlock (lib/net/FBNet.py:216-319) and
- * NormalNet.forward (lib/net/NormalNet.py:84-97).
- * icon_conv2d: nn.Conv2d (zero padding, or reflect = ReflectionPad2d(pad) folded in) or, with
- * transposed = 1, nn.ConvTranspose2d(stride, padding = pad, output_padding = out_pad); weights in
- * torch layout; optional bias, residual add and activation (0 none, 1 ReLU, 2 tanh) in the epilogue.
- * icon_group_norm: nn.GroupNorm(groups, C) with affine (gamma, beta), or nn.InstanceNorm2d(C) when
- * groups == C and gamma == beta == NULL; optional residual add and ReLU fused. */
-int icon_conv2d(const float *x, const float *w, const float *bias, const float *res, float *y, int N, int Cin,
-                int H, int W, int Cout, int KH, int KW, int stride, int pad, int out_pad, int reflect,
-                int transposed, int act, icon_stream_t stream);
-/* Tensor-core (wgmma, fp16 hi/lo x3, fp32-class accuracy) variant for Cin % 64 == 0; same semantics.
- * wt_packed: per output-channel tile (n_tile rows, zero padded) and per 64-wide K-chunk (k = tap*Cin + ci) a
- * K-major SWIZZLE_128B tile of the fp16 hi parts followed by one of the lo parts (icon_b200/conv_ops.py packs
- * it).  splits > 1 = split-K over the chunks, partial sums in `ws` (icon_conv2d_tc_workspace_bytes). */
-size_t icon_conv2d_tc_workspace_bytes(int N, int Cout, int OH, int OW, int splits);
-int icon_conv2d_tc(const float *x, const void *wt_packed, const float *bias, const float *res, float *y, int N,
-                   int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int out_pad, int reflect,
-                   int transposed, int act, int n_tile, int splits, void *ws, size_t ws_bytes, icon_stream_t stream);
+/* ------------------------------------------------------------------ encoder operators
+ * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
+ * two take NCHW fp32 tensors; every 2-D convolution and normalisation runs on the NHWC path after them. */
+/* y = x / ||x||_2 (over 3 channels, no eps) * (sum_c |image| != 0): NormalNet.forward (NormalNet.py:84-97) */
+int icon_normalize_mask(const float *x, const float *image, float *y, int N, int Cimg, int64_t HW,
+                        icon_stream_t stream);
+/* nn.Conv3d (B = 1, Cout <= 8, cubic kernel / stride / padding / dilation) followed by eval-mode BatchNorm3d
+ * folded into per-channel (scale, shift), optional residual add and ReLU: the layers of PaMIR's VolumeEncoder
+ * (lib/net/VE.py:96-183).  x [Cin,D,H,W], w [Cout,Cin,k,k,k], y [Cout,OD,OH,OW]. */
+int icon_conv3d(const float *x, const float *w, const float *scale, const float *shift, const float *res, float *y,
+                int Cin, int Cout, int D, int H, int W, int k, int stride, int pad, int dil, int relu,
+                icon_stream_t stream);
 /* ---- NHWC encoder path (csrc/conv_nhwc.cu, csrc/act_nhwc.cu): activations between layers are NHWC, pre-split
  * x = hi + lo into two fp16 tensors [N * nplanes][Hp][Wp][Cp] (Cp % 64 == 0) by icon_act_nhwc.
  *
@@ -237,8 +229,7 @@ int icon_conv2d_tc(const float *x, const void *wt_packed, const float *bias, con
  *   s2d = 1: four parity planes for a stride-2 consumer; channels padded to Cp with zeros) and / or fp32 NHWC.
  * icon_ew_nhwc: mode 0 a + b (+ c), 1 avg_pool2(a), 2 b + bicubic_up2(a, align_corners), 3 relu(a * scale + shift) with
  *   b = the [N][C] (scale, shift) table of icon_norm_finalize; optional stats of the result.
- * icon_nchw_to_nhwc / icon_nhwc_to_nchw: layout adaptors (the former with optional stats).
- * icon_conv7_head: 7 x 7 reflection-padded 64 -> (1..3) channel convolution from fp32 NHWC to NCHW, act 2 = tanh. */
+ * icon_nchw_to_nhwc / icon_nhwc_to_nchw: layout adaptors (the former with optional stats). */
 size_t icon_conv_nhwc_workspace_bytes(int N, int Ht, int Wt, int Cout, int splits);
 int icon_conv_nhwc(const void *a_hi, const void *a_lo, const int64_t *dims, const int64_t *strides, const void *wt_packed,
                    int wt_chunks, const float *bias, float *out, int OHf, int OWf, int Cs, int co_off, int Cout, int N,
@@ -272,8 +263,6 @@ int icon_nhwc_to_nchw(const float *x, float *y, int N, int C, int Cs, int c_off,
  * map whose W stride is sx * Cp8 elements). */
 int icon_stem_pack(const float *x, void *hi, void *lo, int N, int Cin, int H, int W, int Cp8, int Wp, int Hrows, int sy,
                    int reflect, icon_stream_t stream);
-int icon_conv7_head(const float *x, const float *w, const float *bias, float *y, int N, int H, int W, int Cin, int Cout,
-                    int act, icon_stream_t stream);
 /* ---- clean_mesh (csrc/clean.cu; reference lib/dataset/mesh_util.py:778-791: trimesh split + largest component).
  * faces int64 [nf][3] indexing nv vertices.  _count: union-find over the vertices, picks the component with the most
  * vertices (ties: the one containing the smallest vertex id), leaves the kept counts in d_counts[0..1] and the
@@ -283,27 +272,6 @@ int icon_clean_mesh_count(const int64_t *faces, int64_t nv, int64_t nf, void *ws
                           icon_stream_t stream);
 int icon_clean_mesh_emit(const void *verts, int verts_f64, const int64_t *faces, int64_t nv, int64_t nf, const void *ws,
                          float *out_verts, int32_t *out_faces, icon_stream_t stream);
-int icon_group_norm(const float *x, const float *gamma, const float *beta, const float *res, float *y, int N,
-                    int C, int HW, int groups, float eps, int relu, void *stats_ws /* 16*N*groups bytes or NULL */,
-                    icon_stream_t stream);
-/* nn.Conv3d (B = 1, Cout <= 8, cubic kernel / stride / padding / dilation) followed by eval-mode BatchNorm3d
- * folded into per-channel (scale, shift), optional residual add and ReLU: the layers of PaMIR's VolumeEncoder
- * (lib/net/VE.py:96-183).  x [Cin,D,H,W], w [Cout,Cin,k,k,k], y [Cout,OD,OH,OW]. */
-int icon_conv3d(const float *x, const float *w, const float *scale, const float *shift, const float *res, float *y,
-                int Cin, int Cout, int D, int H, int W, int k, int stride, int pad, int dil, int relu,
-                icon_stream_t stream);
-/* F.avg_pool2d(x, 2, stride=2); planes = N*C */
-int icon_avg_pool2(const float *x, float *y, int64_t planes, int H, int W, icon_stream_t stream);
-/* y = add + F.interpolate(x, scale_factor=2, mode="bicubic", align_corners=True) (HGFilters.py:70-76) */
-int icon_bicubic_up2_add(const float *x, const float *add, float *y, int64_t planes, int H, int W,
-                         icon_stream_t stream);
-/* y = cat(a, b, c, dim=1) + res (ConvBlock, net_util.py:273-278) */
-int icon_cat3_add(const float *a, const float *b, const float *c, const float *res, float *y, int N, int C1, int C2,
-                  int C3, int64_t HW, icon_stream_t stream);
-int icon_add3(const float *a, const float *b, const float *c, float *y, int64_t n, icon_stream_t stream);
-/* y = x / ||x||_2 (over 3 channels, no eps) * (sum_c |image| != 0)  (NormalNet.py:88-97) */
-int icon_normalize_mask(const float *x, const float *image, float *y, int N, int Cimg, int64_t HW,
-                        icon_stream_t stream);
 
 #ifdef __cplusplus
 }

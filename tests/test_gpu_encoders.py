@@ -1,12 +1,11 @@
-"""Encoder kernels (csrc/conv.cu) against torch's CPU operators and against outputs of the
-reference's own HGFilter / GlobalGenerator (tests/golden/encoders.npz, reference imported live)."""
+"""The encoders of icon_b200/encoders.py end to end against outputs of the reference's own HGFilter /
+GlobalGenerator / NormalNet / VolumeEncoder (tests/golden/encoders*.npz) and against torch's CPU operators.
+The NHWC layers they are built from are tested op by op in tests/test_gpu_nhwc.py."""
 import os
 
 import numpy as np
 import pytest
 import torch
-import torch.nn as nn
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
@@ -23,93 +22,32 @@ def _g(seed):
     return torch.Generator().manual_seed(seed)
 
 
-@pytest.mark.parametrize("cin,cout,k,s,p,reflect,hw", [
-    (3, 64, 7, 2, 3, 0, 64), (64, 64, 3, 1, 1, 0, 33), (128, 256, 1, 1, 0, 0, 16), (6, 64, 7, 1, 3, 3, 40),
-    (32, 32, 3, 1, 1, 1, 24), (64, 128, 3, 2, 1, 0, 32), (64, 3, 7, 1, 3, 3, 32), (256, 6, 1, 1, 0, 0, 20)])
-def test_conv2d_matches_torch(cin, cout, k, s, p, reflect, hw):
+def test_normalize_mask_matches_torch():
     dev = _cuda()
     from icon_b200 import conv_ops as C
-    conv = nn.Conv2d(cin, cout, k, stride=s, padding=0 if reflect else p)
-    x = torch.randn(2, cin, hw, hw + 3, generator=_g(cin + cout))
-    with torch.no_grad():
-        ref = conv(F.pad(x, (reflect,) * 4, mode="reflect") if reflect else x)
-        res = torch.randn(ref.shape, generator=_g(7))
-        ref_r = torch.tanh(ref + res)
-    for impl in ("auto", "fp32"):                 # auto = tensor-core kernel when Cin % 64 == 0
-        C.set_conv_impl(impl)
-        try:
-            y = C.conv2d(x.to(dev), conv.to(dev), reflect=reflect)
-            assert y.shape == ref.shape
-            assert (y.cpu() - ref).abs().max() <= 5e-5 * max(1.0, ref.abs().max().item()), impl
-            y2 = C.conv2d(x.to(dev), conv, reflect=reflect, tanh=True, residual=res.to(dev))
-            assert (y2.cpu() - ref_r).abs().max() <= 5e-5, impl
-        finally:
-            C.set_conv_impl("auto")
-
-
-@pytest.mark.parametrize("cin,cout,k,s,p,reflect,hw,relu", [
-    (256, 256, 3, 1, 1, 0, 16, True),        # small spatial -> split-K
-    (1024, 1024, 3, 1, 1, 1, 8, False),      # ResnetBlock shape (reflect), split-K over 144 chunks
-    (128, 96, 3, 2, 1, 0, 40, False),        # Cout not a multiple of the tile, stride 2
-    (64, 32, 1, 1, 0, 0, 64, True)])
-def test_conv2d_tensor_core_shapes(cin, cout, k, s, p, reflect, hw, relu):
-    dev = _cuda()
-    from icon_b200 import conv_ops as C
-    conv = nn.Conv2d(cin, cout, k, stride=s, padding=0 if reflect else p)
-    x = torch.randn(1, cin, hw, hw, generator=_g(cin + k))
-    with torch.no_grad():
-        ref = conv(F.pad(x, (reflect,) * 4, mode="reflect") if reflect else x)
-        if relu:
-            ref = F.relu(ref)
-    y = C.conv2d(x.to(dev), conv.to(dev), reflect=reflect, relu=relu)
-    err = (y.cpu() - ref).abs().max().item()
-    assert err <= 5e-5 * max(1.0, ref.abs().max().item()), err
-
-
-def test_conv_transpose2d_matches_torch():
-    dev = _cuda()
-    from icon_b200 import conv_ops as C
-    for cin, cout in ((48, 24), (128, 64)):          # FP32 kernel / tensor-core kernel
-        ct = nn.ConvTranspose2d(cin, cout, 3, stride=2, padding=1, output_padding=1)
-        x = torch.randn(2, cin, 17, 19, generator=_g(1))
-        with torch.no_grad():
-            ref = ct(x)
-        y = C.conv_transpose2d(x.to(dev), ct.to(dev))
-        assert y.shape == ref.shape
-        assert (y.cpu() - ref).abs().max() <= 5e-5, (cin, cout)
-
-
-def test_norms_pool_bicubic_joins_match_torch():
-    dev = _cuda()
-    from icon_b200 import conv_ops as C
-    x = torch.randn(2, 64, 24, 20, generator=_g(2)) * 2 + 0.5
-    gn = nn.GroupNorm(32, 64)
-    with torch.no_grad():
-        gn.weight.copy_(1 + 0.1 * torch.randn(64, generator=_g(3)))
-        gn.bias.copy_(0.1 * torch.randn(64, generator=_g(4)))
-        ref = F.relu(gn(x))
-    assert (C.group_norm(x.to(dev), gn.to(dev), relu=True).cpu() - ref).abs().max() <= 2e-5
-    inorm = nn.InstanceNorm2d(64, affine=False)
-    with torch.no_grad():
-        ref_i = F.relu(inorm(x))
-        ref_res = x + inorm(x * 0.5 + 1)
-    assert (C.instance_norm(x.to(dev), relu=True).cpu() - ref_i).abs().max() <= 2e-5
-    assert (C.instance_norm((x * 0.5 + 1).to(dev), residual=x.to(dev)).cpu() - ref_res).abs().max() <= 2e-5
-    assert torch.equal(C.avg_pool2(x.to(dev)).cpu(), F.avg_pool2d(x, 2, stride=2)) or \
-        (C.avg_pool2(x.to(dev)).cpu() - F.avg_pool2d(x, 2, stride=2)).abs().max() <= 1e-6
-    lo = torch.randn(1, 8, 9, 11, generator=_g(5))
-    up1 = torch.randn(1, 8, 18, 22, generator=_g(6))
-    ref_b = up1 + F.interpolate(lo, scale_factor=2, mode="bicubic", align_corners=True)
-    assert (C.bicubic_up2_add(lo.to(dev), up1.to(dev)).cpu() - ref_b).abs().max() <= 2e-5
-    a, b, c = (torch.randn(2, n, 6, 5, generator=_g(n)) for n in (8, 4, 4))
-    r = torch.randn(2, 16, 6, 5, generator=_g(9))
-    assert torch.equal(C.cat_add((a.to(dev), b.to(dev), c.to(dev)), r.to(dev)).cpu(), torch.cat((a, b, c), 1) + r)
-    assert torch.equal(C.add3(a.to(dev), a.to(dev) * 2, a.to(dev) * 3).cpu(), a + a * 2 + a * 3)
     nml = torch.randn(1, 3, 10, 10, generator=_g(10))
     img = torch.randn(1, 3, 10, 10, generator=_g(11))
     img[:, :, :3] = 0
     ref_n = nml / torch.norm(nml, dim=1, keepdim=True) * (img.abs().sum(1, keepdim=True) != 0).float()
     assert (C.normalize_mask(nml.to(dev), img.to(dev)).cpu() - ref_n).abs().max() <= 1e-6
+
+
+def test_hourglass_forward_on_nchw_matches_torch():
+    """HourGlass.forward keeps the reference's NCHW contract (lib.net.HGFilters.HourGlass under the overlay)."""
+    dev = _cuda()
+    from icon_b200 import config
+    from icon_b200.encoders import HourGlass
+    from tools import torch_encoders as OE
+    hg = HourGlass(1, 2, 256, config.preset("icon-filter").net)
+    hg.load_state_dict(S.seeded_like(hg.state_dict(), 25))
+    hg.eval()
+    x = torch.randn(1, 256, 16, 24, generator=_g(12))
+    with torch.no_grad():
+        ref = OE.hourglass(hg, hg.depth, x)
+    y = hg.to(dev)(x.to(dev)).cpu()
+    assert y.shape == ref.shape
+    err = (y - ref).abs().max().item()
+    assert err <= 2e-4 * max(1.0, ref.abs().max().item()), err
 
 
 def test_hgfilter_matches_reference_module(golden_dir):
@@ -150,33 +88,6 @@ def test_volume_encoder_matches_reference_module(golden_dir):
     y = ve(torch.from_numpy(g["ve_x"]).to(dev), intermediate_output=False)
     assert len(y) == 1 and tuple(y[0].shape) == tuple(g["ve_y"].shape)
     assert np.abs(y[0].cpu().numpy() - g["ve_y"]).max() <= 1e-4
-
-
-@pytest.mark.parametrize("kind,C,hw", [
-    ("group", 512, 64), ("group", 256, 128), ("group", 64, 512), ("group", 128, 256), ("group", 256, 32),
-    ("instance", 64, 512), ("instance", 128, 256), ("instance", 256, 128), ("instance", 512, 64),
-    ("instance", 1024, 32), ("instance", 1024, 8)])
-def test_every_norm_dispatch_path_matches_torch(kind, C, hw):
-    """icon_group_norm picks one of four kernels from (groups x samples, elements per group) -- csrc/conv.cu
-    icon_group_norm; the shapes here are the ones the 512 x 512 encoders produce (plus small ones), so every
-    branch is compared with torch.nn.GroupNorm(32, C) / InstanceNorm2d."""
-    dev = _cuda()
-    from icon_b200 import conv_ops as C_
-    x = torch.randn(1, C, hw, hw, generator=_g(C + hw)) * 1.7 + 0.3
-    x[:, ::3] *= 4.0
-    if kind == "group":
-        m = nn.GroupNorm(32, C)
-        with torch.no_grad():
-            m.weight.copy_(1 + 0.1 * torch.randn(C, generator=_g(3)))
-            m.bias.copy_(0.1 * torch.randn(C, generator=_g(4)))
-            ref = F.relu(m(x))
-        y = C_.group_norm(x.to(dev), m.to(dev), relu=True)
-    else:
-        with torch.no_grad():
-            ref = F.relu(nn.InstanceNorm2d(C, affine=False)(x))
-        y = C_.instance_norm(x.to(dev), relu=True)
-    err = (y.cpu() - ref).abs().max().item()
-    assert err <= 3e-5, (kind, C, hw, err)
 
 
 def _enc512(golden_dir):

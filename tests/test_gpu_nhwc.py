@@ -24,7 +24,8 @@ def _tol(ref):
 
 @pytest.mark.parametrize("cin,cout,k,pad,h,w", [
     (64, 64, 3, 1, 32, 32), (128, 256, 1, 0, 16, 24), (32, 32, 3, 1, 20, 40), (64, 6, 1, 0, 16, 16), (6, 256, 1, 0, 8, 8),
-    (256, 128, 3, 1, 64, 64), (128, 96, 3, 1, 33, 17), (64, 64, 3, 1, 4, 4), (192, 64, 3, 1, 128, 128)])
+    (256, 128, 3, 1, 64, 64), (128, 96, 3, 1, 33, 17), (64, 64, 3, 1, 4, 4), (192, 64, 3, 1, 128, 128),
+    (64, 64, 3, 1, 33, 36), (256, 256, 3, 1, 16, 16), (256, 6, 1, 0, 20, 23)])
 def test_conv_stride1_zero_pad(cin, cout, k, pad, h, w):
     dev = _cuda()
     from icon_b200 import nhwc as T
@@ -68,9 +69,10 @@ def test_conv_writes_channel_slices_of_one_tensor():
     assert op2.C == 32 and op2.Cp == 64 and (op2.hi[..., 32:] == 0).all()
 
 
-@pytest.mark.parametrize("c,hw", [(64, 16), (1024, 32), (256, 9)])
+@pytest.mark.parametrize("c,hw", [(64, 16), (1024, 32), (256, 9), (32, 24), (1024, 8)])
 def test_reflect_conv_and_split_k(c, hw):
-    """ResnetBlock conv: ReflectionPad2d(1) + Conv2d(k3, padding 0); 1024 channels at 32 x 32 runs split-K."""
+    """ResnetBlock conv: ReflectionPad2d(1) + Conv2d(k3, padding 0); 1024 channels at 32 x 32 runs split-K; 32
+    channels are padded to 64 under the halo."""
     dev = _cuda()
     from icon_b200 import nhwc as T
     conv = nn.Conv2d(c, c, 3, padding=0)
@@ -87,7 +89,7 @@ def test_reflect_conv_and_split_k(c, hw):
     assert torch.allclose(st[..., 1], (ref.double() ** 2).sum(dim=(2, 3)), rtol=1e-4, atol=2e-2)
 
 
-@pytest.mark.parametrize("cin,cout,hw", [(64, 128, 64), (512, 1024, 16), (128, 256, 34)])
+@pytest.mark.parametrize("cin,cout,hw", [(64, 128, 64), (512, 1024, 16), (128, 256, 34), (128, 96, 40)])
 def test_conv_stride2_space_to_depth(cin, cout, hw):
     dev = _cuda()
     from icon_b200 import nhwc as T
@@ -101,7 +103,7 @@ def test_conv_stride2_space_to_depth(cin, cout, hw):
     assert (y - ref).abs().max() <= _tol(ref)
 
 
-@pytest.mark.parametrize("cin,cout,hw", [(128, 64, 17), (1024, 512, 32), (64, 64, 8)])
+@pytest.mark.parametrize("cin,cout,hw", [(128, 64, 17), (1024, 512, 32), (64, 64, 8), (48, 24, 17)])
 def test_conv_transpose_four_phases(cin, cout, hw):
     dev = _cuda()
     from icon_b200 import nhwc as T
@@ -117,7 +119,11 @@ def test_conv_transpose_four_phases(cin, cout, hw):
     assert torch.allclose(out.stats.cpu()[..., 0], ref.double().sum(dim=(2, 3)), rtol=1e-4, atol=2e-2)
 
 
-@pytest.mark.parametrize("kind,c,hw", [("group", 64, 32), ("group", 256, 16), ("instance", 128, 24), ("instance", 1024, 8)])
+@pytest.mark.parametrize("kind,c,hw", [
+    ("group", 64, 32), ("group", 256, 16), ("instance", 128, 24), ("instance", 1024, 8),
+    # the norm shapes of the two encoders at 512 x 512: above 64 x 64 pixels `act` reads a materialised table
+    ("group", 512, 64), ("group", 256, 128), ("group", 64, 512), ("group", 128, 256), ("group", 256, 32),
+    ("instance", 64, 512), ("instance", 128, 256), ("instance", 256, 128), ("instance", 512, 64), ("instance", 1024, 32)])
 def test_finalize_and_act_match_torch_norms(kind, c, hw):
     dev = _cuda()
     from icon_b200 import nhwc as T
@@ -171,7 +177,7 @@ def test_elementwise_ops_and_their_statistics():
     assert (T.to_nchw(r).cpu() - ref).abs().max() <= 2e-5
 
 
-def test_conv7_head_matches_torch():
+def test_conv7_head_gemm_col2im_matches_torch():
     dev = _cuda()
     from icon_b200 import nhwc as T
     conv = nn.Conv2d(64, 3, 7, padding=0)
@@ -179,9 +185,7 @@ def test_conv7_head_matches_torch():
     with torch.no_grad():
         ref = torch.tanh(conv(F.pad(x, (3, 3, 3, 3), mode="reflect")))
     conv = conv.to(dev)
-    y = T.conv7_head_fp32(x.permute(0, 2, 3, 1).contiguous().to(dev), conv, tanh=True).cpu()
-    assert (y - ref).abs().max() <= 2e-5
-    op, _ = T.act(T.raw_from_nchw(x.to(dev)))                      # the shipped path: tensor-core GEMM + col2im
+    op, _ = T.act(T.raw_from_nchw(x.to(dev)))                      # tensor-core GEMM + col2im
     y2 = T.conv7_head(op, conv, tanh=True).cpu()
     assert (y2 - ref).abs().max() <= 2e-5
 

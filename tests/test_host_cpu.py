@@ -205,6 +205,22 @@ def test_state_dict_keys_match_reference(golden_dir):
     assert top == {"if_regressor", "F_filter", "normal_filter"}
 
 
+def test_encoders_reject_inputs_outside_their_preconditions():
+    """HGFilter takes H, W multiples of 2^(num_hourglass + 2); GlobalGenerator multiples of 2^n_downsampling of at least
+    twice that, with ngf 64 and <= 3 outputs.  The checks run before any kernel, so they hold on CPU tensors."""
+    from icon_b200 import config
+    from icon_b200.encoders import GlobalGenerator, HGFilter
+    hg = HGFilter(config.preset("icon-filter").net, 2, 3).eval()
+    with pytest.raises(NotImplementedError, match="HGFilter: H and W must be multiples of 16"):
+        hg(torch.zeros(1, 3, 16 * 4 + 1, 64))
+    gg = GlobalGenerator(6, 3, 64, 4, 1).eval()
+    for h, w in ((64, 72), (16, 16)):
+        with pytest.raises(NotImplementedError, match="GlobalGenerator: H and W must be multiples of 16"):
+            gg(torch.zeros(1, 6, h, w))
+    with pytest.raises(NotImplementedError, match="ngf == 64"):
+        GlobalGenerator(6, 3, 8, 2, 1).eval()(torch.zeros(1, 6, 64, 64))
+
+
 @pytest.mark.parametrize("name,c0", [("icon-filter", 13), ("icon-nofilter", 10), ("pamir", 13), ("pifu", 13)])
 def test_presets_give_reference_mlp_width(name, c0):
     from icon_b200 import config, net

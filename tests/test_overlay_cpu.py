@@ -82,13 +82,14 @@ assert A.batch_mean() == "reference" and A.batch_mean is TU.batch_mean
 assert A.load_checkpoint() == "reference" and MU.load_checkpoint.__module__ == "lib.dataset.mesh_util"
 assert FB.LocalEnhancer.__module__ == "lib.net.FBNet"
 # define_G: the configuration NormalNet builds -> icon_b200 generator, anything else -> the checkout's define_G
-assert isinstance(FB.define_G(6, 3, 8, "global", 2, 1, 1, 3, "instance"), icon_b200.encoders.GlobalGenerator)
+assert isinstance(FB.define_G(6, 3, 64, "global", 2, 1, 1, 3, "instance"), icon_b200.encoders.GlobalGenerator)
+assert FB.define_G(6, 3, 8, "global", 2, 1, 1, 3, "instance") == ("reference", "global", "instance")
 assert FB.define_G(6, 3, 8, "local", 2, 1, 1, 3, "instance") == ("reference", "local", "instance")
 print("OVERLAY_OK")
 '''
 
 
-def test_overlay_replaces_and_patches_a_checkout(tmp_path):
+def test_overlay_replaces_and_patches_a_checkout_and_routes_define_g(tmp_path):
     for rel, text in CHECKOUT.items():
         p = tmp_path / rel
         p.parent.mkdir(parents=True, exist_ok=True)

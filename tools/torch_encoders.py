@@ -65,7 +65,7 @@ def hgfilter(m, x):
 
 def global_generator(m, x):
     # the container IS the reference's nn.Sequential (ReflectionPad2d, Conv2d, InstanceNorm2d, ReLU, ResnetBlock...);
-    # only ResnetBlock.forward is overridden in icon_b200.encoders, so run its conv_block Sequential explicitly
+    # ResnetBlock in icon_b200.encoders has no forward of its own, so run its conv_block Sequential explicitly
     y = x
     for layer in m.model:
         if hasattr(layer, "conv_block"):
