@@ -9,18 +9,21 @@
 // (parity bar 1e-4 on the logit).
 //
 // One persistent CTA per SM, 128 query points per tile, 384 threads (3 warpgroups):
-//   warps 0-7   two consumer warpgroups, warpgroup g owns rows [64 g, 64 g + 64) of the tile.  Per tile:
-//               gather (threads 0..63 of the warpgroup, one point each: bilinear / trilinear samples, SMPL
-//               record, outlier rule) -> x0 operand (fp16 hi / lo, shared memory; column 15 is the constant 1
-//               that carries b0 and b2) -> for each half h of layer 1's 256 outputs: 8 x (layer-0 chunk of 64
-//               outputs, wgmma from shared memory -> LeakyReLU -> hi / lo register fragments -> layer-1 K-chunk
-//               with A from registers, N = 128) -> LeakyReLU(+ b1) of the half -> its two layer-2 K-chunks (A
-//               from registers, N = 128) -> x0 tail of layer 2 -> layer 3 (144 -> 1) as an fp32 dot over the
-//               accumulator fragment, reduced across the 4 lanes that share a row.  Layer 0 is recomputed for
-//               the second half: 16 of 174 k MACs per point, and it keeps the live accumulators at 160 registers.
-//   warps 8-11  weight producer (warp 8, one lane; the warpgroup hands its registers to the consumers with setmaxnreg): 1-D bulk copies (cp.async.bulk, TMA engine) of host-pre-swizzled K-major SWIZZLE_128B
-//               tiles from L2 into a 4 x 32 KB ring, mbarrier complete_tx (per tile 16 half-chunks of layer 1 and 4
-//               chunks of layer 2; layer 0, the x0 tail of layer 2 and the fp32 tail stay resident).
+//   warps 0-7   two consumer warpgroups, warpgroup g owns rows [64 g, 64 g + 64) of the tile.  Per tile, with the
+//               tile's x0 operand (fp16 hi / lo, column 15 is the constant 1 that carries b0 and b2) taken from one of
+//               two shared-memory slots: for each of layer 1's 8 K-chunks j, layer 0's outputs [64 j, 64 j + 64)
+//               (wgmma from shared memory) -> LeakyReLU -> hi / lo register A fragments -> layer-1 K-chunk, N = 256,
+//               A from registers.  Two fragment buffers alternate: layer 0 of chunk j + 1 is issued and converted
+//               while layer 1 of chunk j runs.  Then LeakyReLU(+ b1) of the 256-wide accumulator, 64 columns at a
+//               time, feeds layer 2's four K-chunks (N = 128), each slice converted while the previous chunk runs ->
+//               x0 tail of layer 2 -> layer 3 (144 -> 1) as an fp32 dot over the accumulator fragment, reduced
+//               across the 4 lanes that share a row.
+//   warps 8-11  producer warpgroup (hands its registers to the consumers with setmaxnreg).
+//               warp 8, one lane: 1-D bulk copies (cp.async.bulk, TMA engine) of host-pre-swizzled K-major SWIZZLE_128B
+//               weight tiles from L2 into a 4 x 32 KB ring, mbarrier complete_tx (per tile 8 layer-1 chunks as hi / lo
+//               stage pairs and 4 layer-2 chunks; layer 0, the x0 tail of layer 2 and the fp32 tail stay resident).
+//               warps 9-11: the feature gather of the next tile (bilinear / trilinear samples, SMPL record, outlier
+//               rule) into the free x0 slot, so it runs while the consumers compute the current one.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -31,9 +34,11 @@ namespace icon {
 
 constexpr int TC_THREADS = 384;      // 2 consumer warpgroups + 1 producer warpgroup
 constexpr int TC_M = 128;
-constexpr int NSTAGE = 4;            // weight ring depth
-constexpr int STAGE_BYTES = 32768;   // one SW128 operand of 128 rows x 64 k, hi | lo
-constexpr int STAGES_PER_TILE = 20;
+constexpr int NSTAGE = 4;            // weight ring depth: two layer-1 chunks
+constexpr int STAGE_BYTES = 32768;   // one SW128 operand: 256 rows x 64 k (layer 1, hi or lo) or 128 rows, hi | lo (layer 2)
+constexpr int STAGES_PER_TILE = 20;  // 8 x 2 layer-1 + 4 layer-2; a multiple of NSTAGE, so every tile starts at stage 0
+static_assert(STAGES_PER_TILE % NSTAGE == 0 && NSTAGE % 2 == 0, "layer-1 hi / lo pairs must stay on stages (2i, 2i + 1)");
+constexpr int GATHER_THREADS = 96;   // warps 9-11
 
 // byte offsets inside the packed tensor-core weight blob (host: icon_b200/ops.py pack_mlp)
 constexpr int TCB_W0 = 0;                         // hi 16384 | lo 16384, no swizzle, LBO 8192, SBO 128
@@ -48,22 +53,25 @@ static_assert(TCB_BYTES == ICON_MLP_TC_BYTES, "blob layout");
 // shared memory map (bytes from a 1024-aligned base)
 constexpr int SM_STAGE = 0;                       // NSTAGE x 32768
 constexpr int SM_W0 = NSTAGE * STAGE_BYTES;       // 32768
-constexpr int SM_X0H = SM_W0 + 32768;             // 4096  A tile of x0 (hi), no swizzle, LBO 2048, SBO 128
-constexpr int SM_X0L = SM_X0H + 4096;             // 4096
-constexpr int SM_X0F = SM_X0L + 4096;             // [16][128] fp32 (layer 3 skip connection, row 15 = in_cube)
-constexpr int SM_F32 = SM_X0F + 8192;             // biases etc.
+constexpr int SM_X0 = SM_W0 + 32768;              // 2 x0 slots of X0_SLOT bytes:
+constexpr int X0_H = 0;                           //   4096  A tile of x0 (hi), no swizzle, LBO 2048, SBO 128
+constexpr int X0_L = 4096;                        //   4096
+constexpr int X0_F = 8192;                        //   [16][128] fp32 (layer 3 skip connection, row 15 = in_cube)
+constexpr int X0_SLOT = 16384;
+constexpr int SM_F32 = SM_X0 + 2 * X0_SLOT;       // biases etc.
 constexpr int SM_W2T = (SM_F32 + TCB_F32_FLOATS * 4 + 127) / 128 * 128;   // x0 tail of layer 2 (hi 4096 | lo 4096)
 constexpr int SM_BAR = SM_W2T + 8192;
-constexpr int SM_TOTAL = SM_BAR + (2 * NSTAGE + 1) * 8;
+constexpr int NBAR = 2 * NSTAGE + 5;
+constexpr int SM_TOTAL = SM_BAR + NBAR * 8;
 constexpr int TC_SMEM_BYTES = SM_TOTAL + 1024;    // slack for manual 1024-B alignment
 static_assert(TC_SMEM_BYTES <= 227 * 1024, "shared memory");
 
-enum { B_FULL0 = 0, B_EMPTY0 = NSTAGE, B_W0RDY = 2 * NSTAGE };
+enum { B_FULL0 = 0, B_EMPTY0 = NSTAGE, B_W0RDY = 2 * NSTAGE, B_XFULL0 = 2 * NSTAGE + 1, B_XEMPTY0 = 2 * NSTAGE + 3 };
 
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
+// Register split of setmaxnreg.  At launch the CTA holds 168 registers x 384 threads (the __launch_bounds__ cap), and
+// setmaxnreg.inc only hands out what setmaxnreg.dec returned, so 2 x 128 x CONSUMER + 128 x PRODUCER <= 168 x 384.
+constexpr int REG_CONSUMER = 224, REG_PRODUCER = 56;
+static_assert(2 * 128 * REG_CONSUMER + 128 * REG_PRODUCER <= 168 * TC_THREADS, "register split");
 
 // LeakyReLU(d + bias) of 4 k-steps (64 columns) of an accumulator fragment -> hi / lo register A fragments.
 // d points at the fragment of the chunk's first 8-column block; bias (or null) at the chunk's column 2 (lane % 4).
@@ -81,23 +89,81 @@ __device__ __forceinline__ void act_frag64(const float *d, const float *bias, ui
     }
 }
 
-// f[off + t] = v[t] for a runtime offset off, where off + NV <= 15.  Every index into f is a compile-time constant,
-// so f stays in registers (a runtime index would move it to local memory); columns outside [off, off + NV) keep their
-// value.
-template <int NV>
-__device__ __forceinline__ void place_at(float (&f)[16], int off, const float (&v)[NV]) {
+// Gather of one point into its x0 slot: xf = the point's column of the slot's [16][128] fp32 matrix (stride TC_M).
+// Columns are placed as mlp.cu and the reference do (image channels first, then the prior's own columns); columns
+// c0..14 stay zero, since layer 0, the x0 tail of layer 2 and layer 3's skip connection read all of rows 0..14.  Each
+// value goes to shared memory as soon as it is computed, which keeps the gather inside the producer's register budget.
+template <int MODE>
+__device__ __forceinline__ void gather_point(const QueryParams &q, int64_t pi, float *xf) {
 #pragma unroll
-    for (int j = 0; j < 15; ++j) {
-        float x = f[j];
+    for (int j = 0; j < 15; ++j) xf[j * TC_M] = 0.f;
+    float in_cube = 1.f;
+    if (pi < q.N) {
+        if (MODE == 3) {
+            const int c0 = q.c0;
 #pragma unroll
-        for (int t = 0; t < NV; ++t) x = j - t == off ? v[t] : x;
-        f[j] = x;
+            for (int j = 0; j < 15; ++j)
+                if (j < c0) xf[j * TC_M] = q.raw[(size_t)j * q.N + pi];
+        } else {
+            const float4 xyz = q.xyz4[pi];
+            in_cube = xyz.w;
+            if (MODE == 0) {
+                const int d = q.C / 2;
+                const float4 *rp = (const float4 *)(q.rec + 8 * pi);
+                const float4 r0 = rp[0], r1 = rp[1];
+                const int fb = r1.w != 0.f ? 0 : d;          // feat_select: vis=1 front, vis=0 back
+                float sdf = r0.x, cx = r0.y, cy = r0.z, cz = r0.w;
+                if (fabsf(sdf) >= q.clip) {                  // HGPIFuNet.py:299-304
+                    sdf = sdf > 0.f ? 1.f : -1.f;
+                    const long long K = *q.d_K, k3 = 3ll * (long long)q.krank[pi];
+                    cx = (float)q.signs[k3 % K];
+                    cy = (float)q.signs[(k3 + 1) % K];
+                    cz = (float)q.signs[(k3 + 2) % K];
+                }
+                if (d == 6) {
+#pragma unroll
+                    for (int ch = 0; ch < 6; ++ch)
+                        xf[ch * TC_M] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                } else {                                     // any d in 1..8 (c0 = d + 7 <= 15)
+#pragma unroll
+                    for (int ch = 0; ch < 8; ++ch)
+                        if (ch < d) xf[ch * TC_M] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                }
+                const float smpl[7] = {sdf, cx, cy, cz, r1.x, r1.y, r1.z};
+#pragma unroll
+                for (int t = 0; t < 7; ++t)
+                    if (d + t < 15) xf[(d + t) * TC_M] = smpl[t];
+            } else if (MODE == 1) {
+                if (q.C == 12) {
+#pragma unroll
+                    for (int ch = 0; ch < 12; ++ch)
+                        xf[ch * TC_M] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                } else {                                     // any C in 1..14 (c0 = C + 1 <= 15)
+#pragma unroll
+                    for (int ch = 0; ch < 14; ++ch)
+                        if (ch < q.C) xf[ch * TC_M] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                }
+                if (q.C < 15) xf[q.C * TC_M] = xyz.z;
+            } else {
+                const size_t vs = (size_t)q.VD * q.VD * q.VD;
+                if (q.C == 6) {
+#pragma unroll
+                    for (int ch = 0; ch < 6; ++ch)
+                        xf[ch * TC_M] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                } else {                                     // any C in 1..8 (c0 = C + 7 <= 15)
+#pragma unroll
+                    for (int ch = 0; ch < 8; ++ch)
+                        if (ch < q.C) xf[ch * TC_M] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
+                }
+#pragma unroll
+                for (int ch = 0; ch < 7; ++ch)
+                    if (q.C + ch < 15) xf[(q.C + ch) * TC_M] = trilinear(q.vol + ch * vs, q.VD, xyz.x, xyz.y, xyz.z);
+            }
+        }
     }
+    xf[15 * TC_M] = in_cube;                             // c0 <= 15: row 15 is spare
 }
 
-// MODE: 0 icon, 1 pifu, 2 pamir, 3 raw feature matrix.  The gather places the c0 input columns as mlp.cu and the
-// reference do (image channels first, then the prior's own columns); columns c0..14 stay zero, since layer 0, the x0
-// tail of layer 2 and layer 3's skip connection read all of rows 0..14.
 template <int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, const uint8_t *__restrict__ blob) {
     using namespace wg;
@@ -105,7 +171,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
     const uint32_t raw = s32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t *sm = smem_raw + (base - raw);
-    float *x0f = reinterpret_cast<float *>(sm + SM_X0F);
     const float *sf32 = reinterpret_cast<const float *>(sm + SM_F32);
     const float *sb1 = sf32 + 512, *sw3 = sf32 + 896, *sb3 = sf32 + 1040;     // b0 [0,512) and b2 [768,896) ride in the weight tiles
     const uint32_t bar0 = base + SM_BAR;
@@ -117,215 +182,166 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
     if (tid == 0) {
         for (int s = 0; s < NSTAGE; ++s) { mbar_init(BAR(B_FULL0 + s), 1); mbar_init(BAR(B_EMPTY0 + s), 8); }
         mbar_init(BAR(B_W0RDY), 1);
+        for (int b = 0; b < 2; ++b) { mbar_init(BAR(B_XFULL0 + b), GATHER_THREADS); mbar_init(BAR(B_XEMPTY0 + b), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
     if (warp >= 8) {
-        // ======================================================== weight producer
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-        if (warp == 8 && lane == 0) {
-            mbar_expect_tx(BAR(B_W0RDY), 32768 + TCB_F32_FLOATS * 4 + 8192);
-            bulk_g2s(base + SM_W0, blob + TCB_W0, 32768, BAR(B_W0RDY));
-            bulk_g2s(base + SM_F32, blob + TCB_F32, TCB_F32_FLOATS * 4, BAR(B_W0RDY));
-            bulk_g2s(base + SM_W2T, blob + TCB_W2T, 8192, BAR(B_W0RDY));
-            uint32_t cnt = 0;
-            for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                // consumption order: layer-1 rows [0,128) chunks 0..7, layer-2 chunks 0, 1, rows [128,256), chunks 2, 3
-                for (int i = 0; i < STAGES_PER_TILE; ++i, ++cnt) {
-                    const uint32_t s = cnt % NSTAGE, ph = (cnt / NSTAGE) & 1;
-                    mbar_wait(BAR(B_EMPTY0 + s), ph ^ 1);
-                    const uint32_t dst = base + SM_STAGE + s * STAGE_BYTES, full = BAR(B_FULL0 + s);
-                    mbar_expect_tx(full, STAGE_BYTES);
-                    const int h = i < 10 ? 0 : 1, k = i - 10 * h;
-                    if (k < 8) {
-                        const uint8_t *src = blob + TCB_W1 + (size_t)k * 65536 + h * 16384;
-                        bulk_g2s(dst, src, 16384, full);
-                        bulk_g2s(dst + 16384, src + 32768, 16384, full);
-                    } else {
-                        bulk_g2s(dst, blob + TCB_W2 + (size_t)(2 * h + k - 8) * 32768, 32768, full);
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REG_PRODUCER));
+        if (warp == 8) {
+            // ==================================================== weight producer
+            if (lane == 0) {
+                mbar_expect_tx(BAR(B_W0RDY), 32768 + TCB_F32_FLOATS * 4 + 8192);
+                bulk_g2s(base + SM_W0, blob + TCB_W0, 32768, BAR(B_W0RDY));
+                bulk_g2s(base + SM_F32, blob + TCB_F32, TCB_F32_FLOATS * 4, BAR(B_W0RDY));
+                bulk_g2s(base + SM_W2T, blob + TCB_W2T, 8192, BAR(B_W0RDY));
+                uint32_t cnt = 0;
+                for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+                    // consumption order: layer-1 chunks 0..7 as (hi, lo) stage pairs, then layer-2 chunks 0..3
+                    for (int i = 0; i < STAGES_PER_TILE; ++i, ++cnt) {
+                        const uint32_t s = cnt % NSTAGE, ph = (cnt / NSTAGE) & 1;
+                        mbar_wait(BAR(B_EMPTY0 + s), ph ^ 1);
+                        const uint32_t dst = base + SM_STAGE + s * STAGE_BYTES, full = BAR(B_FULL0 + s);
+                        mbar_expect_tx(full, STAGE_BYTES);
+                        const uint8_t *src = i < 16 ? blob + TCB_W1 + (size_t)i * 32768 : blob + TCB_W2 + (size_t)(i - 16) * 32768;
+                        bulk_g2s(dst, src, STAGE_BYTES, full);
                     }
                 }
+            }
+        } else {
+            // ==================================================== feature gather, one tile ahead of the consumers
+            const int gt = tid - 9 * 32;
+            for (uint32_t it = 0; blockIdx.x + (int64_t)it * gridDim.x < ntiles; ++it) {
+                const int b = it & 1;
+                mbar_wait(BAR(B_XEMPTY0 + b), ((it >> 1) & 1) ^ 1);
+                uint8_t *xs = sm + SM_X0 + b * X0_SLOT;
+                for (int r = gt; r < TC_M; r += GATHER_THREADS) {
+                    float *xf = reinterpret_cast<float *>(xs + X0_F) + r;
+                    gather_point<MODE>(q, (blockIdx.x + (int64_t)it * gridDim.x) * TC_M + r, xf);
+                    uint32_t hi[8], lo[8];
+#pragma unroll
+                    for (int i = 0; i < 7; ++i) split2(xf[2 * i * TC_M], xf[(2 * i + 1) * TC_M], hi[i], lo[i]);
+                    split2(xf[14 * TC_M], 1.f, hi[7], lo[7]);          // column 15 = 1: carries b0 (layer 0) and b2 (x0 tail of layer 2)
+                    const int off = (r >> 3) * 128 + (r & 7) * 16;
+                    *reinterpret_cast<uint4 *>(xs + X0_H + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                    *reinterpret_cast<uint4 *>(xs + X0_H + off + 2048) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+                    *reinterpret_cast<uint4 *>(xs + X0_L + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+                    *reinterpret_cast<uint4 *>(xs + X0_L + off + 2048) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+                }
+                fence_proxy_async();                 // the x0 tiles are read by wgmma (async proxy)
+                mbar_arrive(BAR(B_XFULL0 + b));
             }
         }
         return;
     }
 
     // ============================================================ consumer warpgroups
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    const int g = warp >> 2, tw = tid & 127;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REG_CONSUMER));
+    const int g = warp >> 2;
     const int rf = 64 * g + 16 * (warp & 3) + (lane >> 2);       // fragment rows rf, rf + 8 of the tile
     const int cq = 2 * (lane & 3);                               // fragment column offset inside an 8-column block
-    const int c0 = q.c0;
     uint32_t cnt = 0;
-    auto stage_wait = [&]() {
-        const uint32_t s = cnt % NSTAGE;
-        mbar_wait(BAR(B_FULL0 + s), (cnt / NSTAGE) & 1);
+    auto stage_wait = [&](uint32_t c) {
+        const uint32_t s = c % NSTAGE;
+        mbar_wait(BAR(B_FULL0 + s), (c / NSTAGE) & 1);
         return s;
     };
-    auto stage_release = [&](uint32_t s) {     // after wait<0>(): the wgmmas that read stage s are complete
+    auto warp_arrive = [&](int bar) {          // after the wgmmas / loads that read the buffer are complete
         __syncwarp();
-        if (lane == 0) mbar_arrive(BAR(B_EMPTY0 + s));
+        if (lane == 0) mbar_arrive(BAR(bar));
     };
-    const uint64_t dx0h = desc_nosw(base + SM_X0H + g * 1024, 2048, 128), dx0l = desc_nosw(base + SM_X0L + g * 1024, 2048, 128);
     const uint64_t dw2th = desc_nosw(base + SM_W2T, 2048, 128), dw2tl = desc_nosw(base + SM_W2T + 4096, 2048, 128);
     mbar_wait(BAR(B_W0RDY), 0);
 
-    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        bar_sync(1 + g, 128);                    // the previous tile's layer 3 has read x0f
-        if (tw < 64) {
-            const int r = 64 * g + tw;
-            const int64_t pi = tile * TC_M + r;
-            const bool live = pi < q.N;
-            float f[16], in_cube = 1.f;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) f[j] = 0.f;
-            if (live) {
-                if (MODE == 3) {
-#pragma unroll
-                    for (int j = 0; j < 15; ++j)
-                        if (j < c0) f[j] = q.raw[(size_t)j * q.N + pi];
-                } else {
-                    const float4 xyz = q.xyz4[pi];
-                    in_cube = xyz.w;
-                    if (MODE == 0) {
-                        const int d = q.C / 2;
-                        const float4 *rp = (const float4 *)(q.rec + 8 * pi);
-                        const float4 r0 = rp[0], r1 = rp[1];
-                        const int fb = r1.w != 0.f ? 0 : d;          // feat_select: vis=1 front, vis=0 back
-                        float sdf = r0.x, cx = r0.y, cy = r0.z, cz = r0.w;
-                        if (fabsf(sdf) >= q.clip) {                  // HGPIFuNet.py:299-304
-                            sdf = sdf > 0.f ? 1.f : -1.f;
-                            const long long K = *q.d_K, k3 = 3ll * (long long)q.krank[pi];
-                            cx = (float)q.signs[k3 % K];
-                            cy = (float)q.signs[(k3 + 1) % K];
-                            cz = (float)q.signs[(k3 + 2) % K];
-                        }
-                        if (d == 6) {
-#pragma unroll
-                            for (int ch = 0; ch < 6; ++ch)
-                                f[ch] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                            f[6] = sdf; f[7] = cx; f[8] = cy; f[9] = cz; f[10] = r1.x; f[11] = r1.y; f[12] = r1.z;
-                        } else if (d == 3) {
-#pragma unroll
-                            for (int ch = 0; ch < 3; ++ch)
-                                f[ch] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                            f[3] = sdf; f[4] = cx; f[5] = cy; f[6] = cz; f[7] = r1.x; f[8] = r1.y; f[9] = r1.z;
-                        } else {                                     // any d in 1..8 (c0 = d + 7 <= 15)
-#pragma unroll
-                            for (int ch = 0; ch < 8; ++ch)
-                                if (ch < d) f[ch] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                            const float smpl[7] = {sdf, cx, cy, cz, r1.x, r1.y, r1.z};
-                            place_at(f, d, smpl);
-                        }
-                    } else if (MODE == 1) {
-                        if (q.C == 12) {
-#pragma unroll
-                            for (int ch = 0; ch < 12; ++ch)
-                                f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                            f[12] = xyz.z;
-                        } else {                                     // any C in 1..14 (c0 = C + 1 <= 15)
-#pragma unroll
-                            for (int ch = 0; ch < 14; ++ch)
-                                if (ch < q.C) f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                            const float z[1] = {xyz.z};
-                            place_at(f, q.C, z);
-                        }
-                    } else {
-                        const size_t vs = (size_t)q.VD * q.VD * q.VD;
-                        if (q.C == 6) {
-#pragma unroll
-                            for (int ch = 0; ch < 6; ++ch)
-                                f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-#pragma unroll
-                            for (int ch = 0; ch < 7; ++ch)
-                                f[6 + ch] = trilinear(q.vol + ch * vs, q.VD, xyz.x, xyz.y, xyz.z);
-                        } else {                                     // any C in 1..8 (c0 = C + 7 <= 15)
-#pragma unroll
-                            for (int ch = 0; ch < 8; ++ch)
-                                if (ch < q.C) f[ch] = bilinear(q.feat + (size_t)ch * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                            float v[7];
-#pragma unroll
-                            for (int ch = 0; ch < 7; ++ch) v[ch] = trilinear(q.vol + ch * vs, q.VD, xyz.x, xyz.y, xyz.z);
-                            place_at(f, q.C, v);
-                        }
-                    }
-                }
-            }
-            uint32_t hi[8], lo[8];
-#pragma unroll
-            for (int j = 0; j < 15; ++j) x0f[j * TC_M + r] = f[j];
-            x0f[15 * TC_M + r] = in_cube;                     // c0 <= 15: row 15 is spare
-#pragma unroll
-            for (int i = 0; i < 7; ++i) split2(f[2 * i], f[2 * i + 1], hi[i], lo[i]);
-            split2(f[14], 1.f, hi[7], lo[7]);                 // column 15 = 1: carries b0 (layer 0) and b2 (x0 tail of layer 2)
-            const int off = (r >> 3) * 128 + (r & 7) * 16;
-            *reinterpret_cast<uint4 *>(sm + SM_X0H + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            *reinterpret_cast<uint4 *>(sm + SM_X0H + off + 2048) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-            *reinterpret_cast<uint4 *>(sm + SM_X0L + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-            *reinterpret_cast<uint4 *>(sm + SM_X0L + off + 2048) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-            fence_proxy_async();
-        }
-        bar_sync(1 + g, 128);
+    uint32_t it = 0;
+    for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+        const int b = it & 1;
+        const uint32_t xs = base + SM_X0 + b * X0_SLOT;
+        const uint64_t dx0h = desc_nosw(xs + X0_H + g * 1024, 2048, 128), dx0l = desc_nosw(xs + X0_L + g * 1024, 2048, 128);
+        mbar_wait(BAR(B_XFULL0 + b), (it >> 1) & 1);
 
-        float acc2[64];
-#pragma unroll 1
-        for (int h = 0; h < 2; ++h) {
-            float acc1[64];
-            uint32_t s_prev = 0;
-#pragma unroll 1
-            for (int j = 0; j < 8; ++j) {
-                // layer 0, outputs [64 j, 64 j + 64): K = 16, one k-step
-                float acc0[32];
-                const uint64_t w0h = desc_nosw(base + SM_W0 + j * 1024, 8192, 128), w0l = w0h + (16384 >> 4);
-                fence();
-                mma_ss<64>(acc0, dx0h, w0h, 0);
-                mma_ss<64>(acc0, dx0h, w0l, 1);
-                mma_ss<64>(acc0, dx0l, w0h, 1);
-                commit();
-                wait<0>();                       // also retires layer-1 chunk j - 1
-                fence_regs(acc0);
-                if (j) stage_release(s_prev);
-                uint32_t ah[4][4], al[4][4];
-                act_frag64(acc0, nullptr, ah, al);              // b0 rides on x0 column 15 = 1
-                // layer 1, K-chunk j, outputs [128 h, 128 h + 128)
-                const uint32_t s = stage_wait();
-                const uint64_t bh = desc_sw128(base + SM_STAGE + s * STAGE_BYTES), bl = bh + (16384 >> 4);
-                fence();
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    mma_rs<128>(acc1, ah[kk], bh + 2 * kk, (j | kk) != 0);
-                    mma_rs<128>(acc1, ah[kk], bl + 2 * kk, 1);
-                    mma_rs<128>(acc1, al[kk], bh + 2 * kk, 1);
-                }
-                commit();
-                s_prev = s;
-                ++cnt;
-            }
+        // layer 0, outputs [64 j, 64 j + 64): K = 16, one k-step; b0 rides on x0 column 15 = 1
+        auto layer0 = [&](int j, float (&a0)[32]) {
+            const uint64_t w0h = desc_nosw(base + SM_W0 + j * 1024, 8192, 128), w0l = w0h + (16384 >> 4);
+            fence();
+            mma_ss<64>(a0, dx0h, w0h, 0);
+            mma_ss<64>(a0, dx0h, w0l, 1);
+            mma_ss<64>(a0, dx0l, w0h, 1);
+            commit();
+        };
+        float acc1[128];
+        // layer-1 K-chunk j from fragments (ch, cl), with layer 0 of chunk j + 1 converted into (nh, nl) meanwhile.
+        // On entry layer 1 of chunk j - 1, which read (nh, nl), may still run.
+        auto layer1 = [&](int j, uint32_t (&ch)[4][4], uint32_t (&cl)[4][4], uint32_t (&nh)[4][4], uint32_t (&nl)[4][4]) {
             wait<0>();
-            fence_regs(acc1);
-            stage_release(s_prev);
-            // layer 2, K-chunks 2 h, 2 h + 1 (= this half of layer 1's outputs)
+            if (j) { warp_arrive(B_EMPTY0 + (cnt - 2) % NSTAGE); warp_arrive(B_EMPTY0 + (cnt - 1) % NSTAGE); }
+            float a0[32];
+            if (j < 7) layer0(j + 1, a0);
+            const uint32_t s = stage_wait(cnt);
+            stage_wait(cnt + 1);
+            const uint64_t bh = desc_sw128(base + SM_STAGE + s * STAGE_BYTES), bl = bh + (STAGE_BYTES >> 4);
+            fence();
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                uint32_t ah[4][4], al[4][4];
-                act_frag64(acc1 + 32 * c, sb1 + 128 * h + 64 * c + cq, ah, al);
-                const uint32_t s = stage_wait();
-                const uint64_t bh = desc_sw128(base + SM_STAGE + s * STAGE_BYTES), bl = bh + (16384 >> 4);
-                fence();
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    mma_rs<128>(acc2, ah[kk], bh + 2 * kk, (h | c | kk) != 0);
-                    mma_rs<128>(acc2, ah[kk], bl + 2 * kk, 1);
-                    mma_rs<128>(acc2, al[kk], bh + 2 * kk, 1);
-                }
-                commit();
-                wait<0>();
-                fence_regs(acc2);
-                stage_release(s);
-                ++cnt;
+            for (int kk = 0; kk < 4; ++kk) {
+                mma_rs<256>(acc1, ch[kk], bh + 2 * kk, (j | kk) != 0);
+                mma_rs<256>(acc1, ch[kk], bl + 2 * kk, 1);
+                mma_rs<256>(acc1, cl[kk], bh + 2 * kk, 1);
             }
+            commit();
+            cnt += 2;
+            if (j < 7) {
+                wait<1>();                           // layer 0 of chunk j + 1 is complete; layer 1 of chunk j runs on
+                fence_regs(a0);
+                act_frag64(a0, nullptr, nh, nl);
+            }
+        };
+        uint32_t xh[4][4], xl[4][4], yh[4][4], yl[4][4];
+        {
+            float a0[32];
+            layer0(0, a0);
+            wait<0>();
+            fence_regs(a0);
+            act_frag64(a0, nullptr, xh, xl);
         }
+#pragma unroll
+        for (int j = 0; j < 8; j += 2) {
+            layer1(j, xh, xl, yh, yl);
+            layer1(j + 1, yh, yl, xh, xl);
+        }
+        wait<0>();
+        fence_regs(acc1);
+        warp_arrive(B_EMPTY0 + (cnt - 2) % NSTAGE);
+        warp_arrive(B_EMPTY0 + (cnt - 1) % NSTAGE);
+
+        // layer 2: K-chunk c reads LeakyReLU(acc1 + b1) of layer-1 outputs [64 c, 64 c + 64); slice c + 1 is converted
+        // while chunk c runs
+        float acc2[64];
+        auto layer2 = [&](int c, uint32_t (&ch)[4][4], uint32_t (&cl)[4][4]) {
+            const uint32_t s = stage_wait(cnt);
+            const uint64_t bh = desc_sw128(base + SM_STAGE + s * STAGE_BYTES), bl = bh + (16384 >> 4);
+            fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                mma_rs<128>(acc2, ch[kk], bh + 2 * kk, (c | kk) != 0);
+                mma_rs<128>(acc2, ch[kk], bl + 2 * kk, 1);
+                mma_rs<128>(acc2, cl[kk], bh + 2 * kk, 1);
+            }
+            commit();
+            ++cnt;
+            if (c) {                                 // chunk c - 1 is complete: its stage and fragments are free
+                wait<1>();
+                warp_arrive(B_EMPTY0 + (cnt - 2) % NSTAGE);
+            }
+        };
+        act_frag64(acc1, sb1 + cq, xh, xl);
+        layer2(0, xh, xl);
+        act_frag64(acc1 + 32, sb1 + 64 + cq, yh, yl);
+        layer2(1, yh, yl);
+        act_frag64(acc1 + 64, sb1 + 128 + cq, xh, xl);
+        layer2(2, xh, xl);
+        act_frag64(acc1 + 96, sb1 + 192 + cq, yh, yl);
+        layer2(3, yh, yl);
         // x0 tail of layer 2 (b2 through the constant-1 column)
         fence();
         mma_ss<128>(acc2, dx0h, dw2th, 1);
@@ -334,8 +350,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
         commit();
         wait<0>();
         fence_regs(acc2);
+        warp_arrive(B_EMPTY0 + (cnt - 1) % NSTAGE);
 
         // layer 3: LeakyReLU(acc2) . w3 over this thread's 32 columns of rows rf and rf + 8, then across the quad
+        const float *x0f = reinterpret_cast<const float *>(sm + (xs - base) + X0_F);
         float s0 = 0.f, s1 = 0.f;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
@@ -362,6 +380,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) k_query_mlp_tc(QueryParams q, c
                 q.out[pi] = x0f[15 * TC_M + r] != 0.f ? s : copysignf(0.f, s);
             }
         }
+        warp_arrive(B_XEMPTY0 + b);                  // layer 0, the x0 tail and layer 3 are done with this slot
     }
 }
 
