@@ -94,10 +94,23 @@ constexpr int BVH_MAX_LEVELS = 10;   // 4-ary implicit tree over leaves of 4 Mor
 constexpr int RAY_GRID = 256;        // yz cell grid for the +x ray parity
 constexpr int RAY_LIST_PER_FACE = 64;
 
+// Brick leaf lists for dense lattices (sdf.cu): a 32^3 grid of bricks over [-1,1]^3, one brick = 4^3 of the SDF's
+// 128^3 Morton bins, so every warp of 32 Morton-adjacent lattice points lies inside one brick.
+constexpr int BRICK_AX = 32;
+constexpr int NBRICK = BRICK_AX * BRICK_AX * BRICK_AX;
+constexpr int BRICK_MAX_LEAVES = 4096;           // longest list of one brick (it is sorted in shared memory)
+constexpr int64_t BRICK_LIST_CAP = 1 << 24;      // leaf entries per body (32 MB of uint16)
+static inline int64_t brick_list_cap(int F) {
+    const int64_t all = (int64_t)NBRICK * ((F + 3) / 4);
+    return all < BRICK_LIST_CAP ? all : BRICK_LIST_CAP;
+}
+
 struct MeshHeader {                  // device-resident, written by icon_smpl_prepare
     float y0, z0, inv_cy, inv_cz;    // ray grid origin / inverse cell size over the mesh yz box
     int ray_overflow;                // 1 -> cell lists overflowed: kernels fall back to all faces
-    int pad[3];
+    int brick_built;                 // 1 -> the brick leaf lists are complete (built on the first dense call)
+    int brick_overflow;              // 1 -> they did not fit: dense calls walk the tree
+    int pad;
 };
 
 struct MeshView {
@@ -118,6 +131,15 @@ struct MeshView {
     int32_t *rlist;       // [F * RAY_LIST_PER_FACE]
     MeshHeader *hdr;
     void *scan_ws;
+    // brick leaf lists (CSR): built lazily by the first call that takes the dense path
+    float4 *bxyz;         // [NBRICK] brick centres (build input)
+    int32_t *bperm;       // [NBRICK] identity (build input)
+    float *brec;          // [NBRICK][8] build scratch
+    int32_t *bface;       // [NBRICK] original id of the face nearest the brick centre
+    float *bub;           // [NBRICK] bound on the nearest distance of every point of the brick (inflated)
+    int32_t *boff;        // [NBRICK + 1] list offsets
+    unsigned short *blist;   // [brick_cap] leaf ids, ascending box distance to the brick per list
+    int64_t brick_cap;
     int V, F;
     int nlevels;
     int lvl_cnt[BVH_MAX_LEVELS];
@@ -125,6 +147,7 @@ struct MeshView {
 };
 size_t mesh_ws_bytes(int V, int F);
 MeshView mesh_view(const void *ws, int V, int F);
+void bricks_forget(const MeshView &m);   // icon_smpl_prepare (re)fills a workspace: its brick lists are gone
 
 // stage timing for bench.py (icon_profile_*): mark(i) records event i on `stream` when enabled
 void profile_mark(int i, cudaStream_t stream);

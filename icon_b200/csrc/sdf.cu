@@ -14,6 +14,8 @@
 //                 support function) before the exact Ericson distance.  A subtree / face is skipped only when its
 //                 bound is strictly farther than the current best (float slack on every bound); ties resolve to
 //                 the lowest ORIGINAL face index, exactly like the brute-force scan.
+//                 Dense lattices (PPW = 32) replace A and B by a per-body leaf list of the warp's brick (32^3 bricks
+//                 over [-1,1]^3, built by the body's first dense call), sorted by distance, so C can stop early.
 //   sign          the faces listed in the point's yz cell (256 x 256 grid over the mesh's yz
 //                 box) are the only ones a +x ray can hit; each is tested with the same
 //                 Moller-Trumbore code as the brute-force scan, so the hit COUNT is identical.
@@ -21,6 +23,11 @@
 // the pruning is conservative and the per-face arithmetic is the same code (geom.cuh).
 #include <float.h>
 #include <stdlib.h>
+
+#include <algorithm>
+#include <mutex>
+#include <type_traits>
+#include <unordered_set>
 
 #include "common.cuh"
 #include "geom.cuh"
@@ -162,13 +169,40 @@ __device__ unsigned long long g_stats[8];   // warps, overflow warps, sum leaves
 #define STAT(i, v) do { } while (0)
 #endif
 
-template <int FR_CAP>
-struct WarpSmem {
-    unsigned short fr[2][FR_CAP];      // node / leaf ids (leaf count <= 65535 is checked by the host)
+struct ChunkSmem {
     float4 sph[32];                    // bounding spheres of the surviving faces of the current chunk (compacted)
     float4 tri[32][3];                 // their (a, ab, ac) records
     int kk[32];                        // their sorted positions
 };
+template <int FR_CAP>
+struct WarpSmem : ChunkSmem {
+    unsigned short fr[2][FR_CAP];      // node / leaf ids (leaf count <= 65535 is checked by the host)
+};
+// the brick path reads its leaf list from global memory and needs no frontier (a third of the shared memory; at 64
+// registers per thread, registers then bound residency at 32 warps per SM)
+template <int PPW, bool BRICK>
+using SdfSmem = typename std::conditional<BRICK, ChunkSmem, WarpSmem<fr_cap(PPW)>>::type;
+template <int PPW, bool BRICK>
+constexpr size_t sdf_smem_bytes() { return sizeof(SdfSmem<PPW, BRICK>) * (SW_T / 32); }
+
+constexpr float BRICK_W = 2.0f / BRICK_AX;           // brick corners -1 + i / 16 are exact floats
+constexpr float BRICK_HALF_DIAG = 0.0541266f;        // > BRICK_W * sqrt(3) / 2 = 0.05412659
+
+// brick b = (bz * 32 + by) * 32 + bx covers [-1 + bx W, -1 + (bx + 1) W] x ...
+__device__ __forceinline__ void brick_box(int b, float4 &lo, float4 &hi) {
+    const int bx = b % BRICK_AX, by = (b / BRICK_AX) % BRICK_AX, bz = b / (BRICK_AX * BRICK_AX);
+    lo = make_float4(-1.f + bx * BRICK_W, -1.f + by * BRICK_W, -1.f + bz * BRICK_W, 0.f);
+    hi = make_float4(-1.f + (bx + 1) * BRICK_W, -1.f + (by + 1) * BRICK_W, -1.f + (bz + 1) * BRICK_W, 0.f);
+}
+
+// squared distance between the box of leaf l and a brick: the build's sort key, recomputed bit for bit by the kernel
+__device__ __forceinline__ float leaf_key(const MeshView &m, int l, float4 lo, float4 hi) {
+    const float4 a = __ldg(m.nodes + 2 * (size_t)l), z = __ldg(m.nodes + 2 * (size_t)l + 1);
+    const float gx = fmaxf(fmaxf(a.x - hi.x, lo.x - z.x), 0.f);
+    const float gy = fmaxf(fmaxf(a.y - hi.y, lo.y - z.y), 0.f);
+    const float gz = fmaxf(fmaxf(a.z - hi.z, lo.z - z.z), 0.f);
+    return fmaf(gz, gz, fmaf(gy, gy, gx * gx));
+}
 
 __device__ __forceinline__ float box_far2(V3 p, float4 lo, float4 hi) {   // squared distance to the farthest corner
     float dx = fmaxf(fabsf(lo.x - p.x), fabsf(hi.x - p.x));
@@ -183,17 +217,18 @@ __device__ __forceinline__ float box_far2(V3 p, float4 lo, float4 hi) {   // squ
 // span a large box and the shared candidate list explodes; with PPW = 1 the warp box is a point, the lists are the
 // per-point minimum and the 32 lanes only share the work.  The kernel is bound by the latency of the dependent
 // tree loads, so the shared-memory footprint (fr_cap) is kept small enough for >= 36 resident warps per SM.
-template <int PPW>
-__global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xyz4, const int32_t *__restrict__ perm,
-                                                   int64_t N, MeshView m, float *__restrict__ rec,
-                                                   int32_t *__restrict__ face, int order) {
+// BRICK (PPW = 32, dense lattices): a warp whose box lies inside one brick skips phases A and B: its first bound is
+// the brick's, its first candidate the face nearest the brick centre, and phase C scans the brick's leaf list.
+template <int PPW, bool BRICK>
+__device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, const float4 *__restrict__ xyz4,
+                                         const int32_t *__restrict__ perm, int64_t N, const MeshView &m,
+                                         float *__restrict__ rec, int32_t *__restrict__ face, int order,
+                                         int32_t *__restrict__ defer, int32_t *__restrict__ ndefer) {
     constexpr int REP = 32 / PPW;
     constexpr int FR_CAP = fr_cap(PPW);
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    WarpSmem<FR_CAP> &S = reinterpret_cast<WarpSmem<FR_CAP> *>(smem_raw)[wib];
+    const int lane = threadIdx.x & 31;
     const int sub = lane % PPW, rep_id = lane / PPW;           // which point of the warp, which replica
-    const int64_t pos0 = ((int64_t)blockIdx.x * (SW_T / 32) + wib) * PPW;
+    const int64_t pos0 = wid * PPW;
     const int64_t pos = pos0 + sub;
     if (pos0 >= N) return;                                   // whole warp out of range
     const bool live = pos < N;
@@ -207,113 +242,140 @@ __global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xy
     // the warp's bounding box (tighter than the sphere for the flat 4x4x2 blocks of a lattice)
     const float4 wlo = make_float4(warp_min(p.x) - 1e-6f, warp_min(p.y) - 1e-6f, warp_min(p.z) - 1e-6f, 0.f);
     const float4 whi = make_float4(warp_max(p.x) + 1e-6f, warp_max(p.y) + 1e-6f, warp_max(p.z) + 1e-6f, 0.f);
+    const MeshHeader h = *m.hdr;
 
     float best = FLT_MAX;
     int bi = 0x7fffffff;
-    auto try_face = [&](int k) {                             // exact test of sorted face k for this lane
-        const Tri tr = load_tri(m.tri_s + 3 * (size_t)k);
-        const float d = tri_sqdist(p, tr.a, tr.ab, tr.ac);
-        const int f = __ldg(m.order + k);
-        if (d < best || (d == best && f < bi)) { best = d; bi = f; }
-    };
-
-    // ---- phase A: greedy descent towards the warp centre -> a first bound for every lane
-    {
-        int node = 0;
-        for (int lvl = m.nlevels - 1; lvl > 0; --lvl) {
-            const int ch = 4 * node + (lane & 3);
-            float a = FLT_MAX;
-            int ai = ch;
-            if (ch < m.lvl_cnt[lvl - 1]) {
-                const float4 *nb = m.nodes + 2 * ((size_t)m.lvl_off[lvl - 1] + ch);
-                a = box_dist2(c, __ldg(nb), __ldg(nb + 1));
-            }
-            for (int o = 1; o <= 2; o <<= 1) {               // min over the 4 children (lanes 4j..4j+3)
-                const float ob = __shfl_xor_sync(0xffffffffu, a, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, ai, o);
-                if (ob < a || (ob == a && oi < ai)) { a = ob; ai = oi; }
-            }
-            node = __shfl_sync(0xffffffffu, ai, 0);
-        }
-        for (int k = 4 * node; k < min(4 * node + 4, m.F); ++k) try_face(k);
-    }
-    const float ubw = warp_max(sqrtf(best));                  // every lane's nearest is within ubw
-    float ubw2 = ubw;                                         // bound on d(lane, its nearest face), all lanes
-    float ub2 = (ubw2 * 1.00001f + 1e-6f) * (ubw2 * 1.00001f + 1e-6f);
-
-    // ---- phase B: breadth-first cull of the tree, 32 child boxes per step.  The bound also
-    //      tightens on the way down: some face lies within the nearest far-corner distance of c,
-    //      so every lane's nearest face is within that + 2 rw of c.
-    int cur = 0, n = 1;
+    float ubw2;                                               // bound on d(lane, its nearest face), all lanes
+    int cur = 0, n = 1;                                       // tree path: frontier buffer and length
     bool overflow = false;
-    if (lane == 0) S.fr[0][0] = 0;
-    __syncwarp();
-    for (int lvl = m.nlevels - 1; lvl > 0 && !overflow; --lvl) {
-        int nn = 0;
-        float far2 = FLT_MAX;
-        const int ccnt = m.lvl_cnt[lvl - 1];
-        const float4 *nodes = m.nodes + 2 * (size_t)m.lvl_off[lvl - 1];
-        for (int base = 0; base < n; base += 8) {
-            const int slot = base + (lane >> 2);
-            bool pass = false;
-            int ch = 0;
-            if (slot < n) {
-                ch = 4 * (int)S.fr[cur][slot] + (lane & 3);
-                if (ch < ccnt) {
-                    const float4 lo = __ldg(nodes + 2 * (size_t)ch), hi = __ldg(nodes + 2 * (size_t)ch + 1);
-                    // distance between the node's box and the warp's box bounds every lane's distance to the node
+    int b = 0;                                                // brick path: the warp's brick and its box
+    float4 blo, bhi;
+    if constexpr (BRICK) {
+        bool ok = h.brick_built && !h.brick_overflow && c.x >= -1.f && c.x < 1.f && c.y >= -1.f && c.y < 1.f &&
+                  c.z >= -1.f && c.z < 1.f;
+        if (ok) {
+            const int bx = min(BRICK_AX - 1, (int)((c.x + 1.f) * (BRICK_AX * 0.5f)));
+            const int by = min(BRICK_AX - 1, (int)((c.y + 1.f) * (BRICK_AX * 0.5f)));
+            const int bz = min(BRICK_AX - 1, (int)((c.z + 1.f) * (BRICK_AX * 0.5f)));
+            b = (bz * BRICK_AX + by) * BRICK_AX + bx;
+            brick_box(b, blo, bhi);
+            ok = wlo.x >= blo.x && wlo.y >= blo.y && wlo.z >= blo.z && whi.x <= bhi.x && whi.y <= bhi.y && whi.z <= bhi.z;
+        }
+        if (!ok) {                     // straddles bricks, leaves the cube or the lists overflowed: the tree walk takes it
+            if (lane == 0) defer[atomicAdd(ndefer, 1)] = (int32_t)wid;
+            return;
+        }
+        const int f = __ldg(m.bface + b);
+        const Tri tr = load_tri(m.tri + 3 * (size_t)f);
+        best = tri_sqdist(p, tr.a, tr.ab, tr.ac);
+        bi = f;
+        ubw2 = fminf(warp_max(sqrtf(best)), __ldg(m.bub + b));
+        STAT(0, 1);
+    } else {
+        auto try_face = [&](int k) {                             // exact test of sorted face k for this lane
+            const Tri tr = load_tri(m.tri_s + 3 * (size_t)k);
+            const float d = tri_sqdist(p, tr.a, tr.ab, tr.ac);
+            const int f = __ldg(m.order + k);
+            if (d < best || (d == best && f < bi)) { best = d; bi = f; }
+        };
+
+        // ---- phase A: greedy descent towards the warp centre -> a first bound for every lane
+        {
+            int node = 0;
+            for (int lvl = m.nlevels - 1; lvl > 0; --lvl) {
+                const int ch = 4 * node + (lane & 3);
+                float a = FLT_MAX;
+                int ai = ch;
+                if (ch < m.lvl_cnt[lvl - 1]) {
+                    const float4 *nb = m.nodes + 2 * ((size_t)m.lvl_off[lvl - 1] + ch);
+                    a = box_dist2(c, __ldg(nb), __ldg(nb + 1));
+                }
+                for (int o = 1; o <= 2; o <<= 1) {               // min over the 4 children (lanes 4j..4j+3)
+                    const float ob = __shfl_xor_sync(0xffffffffu, a, o);
+                    const int oi = __shfl_xor_sync(0xffffffffu, ai, o);
+                    if (ob < a || (ob == a && oi < ai)) { a = ob; ai = oi; }
+                }
+                node = __shfl_sync(0xffffffffu, ai, 0);
+            }
+            for (int k = 4 * node; k < min(4 * node + 4, m.F); ++k) try_face(k);
+        }
+        const float ubw = warp_max(sqrtf(best));                  // every lane's nearest is within ubw
+        ubw2 = ubw;
+        float ub2 = (ubw2 * 1.00001f + 1e-6f) * (ubw2 * 1.00001f + 1e-6f);
+
+        // ---- phase B: breadth-first cull of the tree, 32 child boxes per step.  The bound also
+        //      tightens on the way down: some face lies within the nearest far-corner distance of c,
+        //      so every lane's nearest face is within that + 2 rw of c.
+        if (lane == 0) S.fr[0][0] = 0;
+        __syncwarp();
+        for (int lvl = m.nlevels - 1; lvl > 0 && !overflow; --lvl) {
+            int nn = 0;
+            float far2 = FLT_MAX;
+            const int ccnt = m.lvl_cnt[lvl - 1];
+            const float4 *nodes = m.nodes + 2 * (size_t)m.lvl_off[lvl - 1];
+            for (int base = 0; base < n; base += 8) {
+                const int slot = base + (lane >> 2);
+                bool pass = false;
+                int ch = 0;
+                if (slot < n) {
+                    ch = 4 * (int)S.fr[cur][slot] + (lane & 3);
+                    if (ch < ccnt) {
+                        const float4 lo = __ldg(nodes + 2 * (size_t)ch), hi = __ldg(nodes + 2 * (size_t)ch + 1);
+                        // distance between the node's box and the warp's box bounds every lane's distance to the node
+                        const float gx = fmaxf(fmaxf(lo.x - whi.x, wlo.x - hi.x), 0.f);
+                        const float gy = fmaxf(fmaxf(lo.y - whi.y, wlo.y - hi.y), 0.f);
+                        const float gz = fmaxf(fmaxf(lo.z - whi.z, wlo.z - hi.z), 0.f);
+                        pass = fmaf(gz, gz, fmaf(gy, gy, gx * gx)) <= ub2;
+                        far2 = fminf(far2, box_far2(c, lo, hi));
+                    }
+                }
+                const unsigned mask = __ballot_sync(0xffffffffu, pass);
+                const int at = nn + __popc(mask & ((1u << lane) - 1u));
+                if (pass && at < FR_CAP) S.fr[cur ^ 1][at] = (unsigned short)ch;
+                nn += __popc(mask);
+            }
+            if (nn > FR_CAP) overflow = true;
+            n = nn;
+            cur ^= 1;
+            // some face lies within the nearest far-corner distance of c -> within that + rw of every lane
+            const float l2 = sqrtf(warp_min(far2)) + rw;
+            if (l2 < ubw2) { ubw2 = l2; ub2 = (ubw2 * 1.00001f + 1e-6f) * (ubw2 * 1.00001f + 1e-6f); }
+            __syncwarp();
+        }
+        // ---- near-first order of the surviving leaves.  The lanes' bounds only tighten while faces are tested, and the
+        //      warp-level cull of a chunk uses the LOOSEST lane bound: leaves that can beat even the tightest current
+        //      bound (box distance <= min over lanes of sqrt(best)) go first, so that the bounds are (nearly) final
+        //      before the long tail of barely-surviving leaves is looked at -- most of the tail then fails the one
+        //      warp-level test instead of 32 per-lane tests.  Order does not affect results (ties: lowest face index).
+        if (order && !overflow && n > 8) {
+            const float ubmin = warp_min(best * rsqrtf(fmaxf(best, 1e-30f))) * 1.00001f + 1e-6f;
+            const float t2 = ubmin * ubmin;
+            int n1 = 0, n2 = 0;
+            for (int base = 0; base < n; base += 32) {
+                const int slot = base + lane;
+                const bool valid = slot < n;
+                int leaf = 0;
+                bool near = false;
+                if (valid) {
+                    leaf = (int)S.fr[cur][slot];
+                    const float4 lo = __ldg(m.nodes + 2 * (size_t)leaf), hi = __ldg(m.nodes + 2 * (size_t)leaf + 1);
                     const float gx = fmaxf(fmaxf(lo.x - whi.x, wlo.x - hi.x), 0.f);
                     const float gy = fmaxf(fmaxf(lo.y - whi.y, wlo.y - hi.y), 0.f);
                     const float gz = fmaxf(fmaxf(lo.z - whi.z, wlo.z - hi.z), 0.f);
-                    pass = fmaf(gz, gz, fmaf(gy, gy, gx * gx)) <= ub2;
-                    far2 = fminf(far2, box_far2(c, lo, hi));
+                    near = fmaf(gz, gz, fmaf(gy, gy, gx * gx)) <= t2;
                 }
+                const unsigned mn = __ballot_sync(0xffffffffu, valid && near), mf = __ballot_sync(0xffffffffu, valid && !near);
+                const unsigned lt = (1u << lane) - 1u;
+                if (valid && near) S.fr[cur ^ 1][n1 + __popc(mn & lt)] = (unsigned short)leaf;
+                if (valid && !near) S.fr[cur ^ 1][n - 1 - (n2 + __popc(mf & lt))] = (unsigned short)leaf;
+                n1 += __popc(mn); n2 += __popc(mf);
             }
-            const unsigned mask = __ballot_sync(0xffffffffu, pass);
-            const int at = nn + __popc(mask & ((1u << lane) - 1u));
-            if (pass && at < FR_CAP) S.fr[cur ^ 1][at] = (unsigned short)ch;
-            nn += __popc(mask);
+            cur ^= 1;
+            __syncwarp();
         }
-        if (nn > FR_CAP) overflow = true;
-        n = nn;
-        cur ^= 1;
-        // some face lies within the nearest far-corner distance of c -> within that + rw of every lane
-        const float l2 = sqrtf(warp_min(far2)) + rw;
-        if (l2 < ubw2) { ubw2 = l2; ub2 = (ubw2 * 1.00001f + 1e-6f) * (ubw2 * 1.00001f + 1e-6f); }
-        __syncwarp();
+        STAT(0, 1); STAT(1, overflow ? 1 : 0); STAT(2, n);
     }
-    // ---- near-first order of the surviving leaves.  The lanes' bounds only tighten while faces are tested, and the
-    //      warp-level cull of a chunk uses the LOOSEST lane bound: leaves that can beat even the tightest current
-    //      bound (box distance <= min over lanes of sqrt(best)) go first, so that the bounds are (nearly) final
-    //      before the long tail of barely-surviving leaves is looked at -- most of the tail then fails the one
-    //      warp-level test instead of 32 per-lane tests.  Order does not affect results (ties: lowest face index).
-    if (order && !overflow && n > 8) {
-        const float ubmin = warp_min(best * rsqrtf(fmaxf(best, 1e-30f))) * 1.00001f + 1e-6f;
-        const float t2 = ubmin * ubmin;
-        int n1 = 0, n2 = 0;
-        for (int base = 0; base < n; base += 32) {
-            const int slot = base + lane;
-            const bool valid = slot < n;
-            int leaf = 0;
-            bool near = false;
-            if (valid) {
-                leaf = (int)S.fr[cur][slot];
-                const float4 lo = __ldg(m.nodes + 2 * (size_t)leaf), hi = __ldg(m.nodes + 2 * (size_t)leaf + 1);
-                const float gx = fmaxf(fmaxf(lo.x - whi.x, wlo.x - hi.x), 0.f);
-                const float gy = fmaxf(fmaxf(lo.y - whi.y, wlo.y - hi.y), 0.f);
-                const float gz = fmaxf(fmaxf(lo.z - whi.z, wlo.z - hi.z), 0.f);
-                near = fmaf(gz, gz, fmaf(gy, gy, gx * gx)) <= t2;
-            }
-            const unsigned mn = __ballot_sync(0xffffffffu, valid && near), mf = __ballot_sync(0xffffffffu, valid && !near);
-            const unsigned lt = (1u << lane) - 1u;
-            if (valid && near) S.fr[cur ^ 1][n1 + __popc(mn & lt)] = (unsigned short)leaf;
-            if (valid && !near) S.fr[cur ^ 1][n - 1 - (n2 + __popc(mf & lt))] = (unsigned short)leaf;
-            n1 += __popc(mn); n2 += __popc(mf);
-        }
-        cur ^= 1;
-        __syncwarp();
-    }
-    STAT(0, 1); STAT(1, overflow ? 1 : 0); STAT(2, n);
     // ---- phases C+D: 32 faces (8 leaves) at a time: cull by bounding sphere against the warp's box and bound,
     //      stage the survivors (sphere + triangle) compacted in shared memory, then every lane tests them against
     //      its own best through two cheap lower bounds (bounding sphere, then the support-function bound
@@ -344,43 +406,60 @@ __global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xy
                 if (!(d > 0.f)) sbA = 1e-6f;
             }
         };
-        if (!overflow) {
+        // one step: this lane's slot holds `leaf` (-1: none), 4 lanes per leaf, 8 leaves = 32 faces
+        auto chunk = [&](int leaf) {
+            bool pass = false;
+            int k = 0;
+            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (leaf >= 0) {
+                k = 4 * leaf + (lane & 3);
+                if (k < m.F) {
+                    s = __ldg(m.sph_s + k);
+                    const float l2 = ubA + s.w;                // sphere vs the warp's box: some lane may be that close
+                    pass = box_dist2(mk3(s.x, s.y, s.z), wlo, whi) <= l2 * l2;
+                }
+            }
+            const unsigned mask = __ballot_sync(0xffffffffu, pass);
+            const int cnt = __popc(mask);
+            STAT(3, cnt);
+            if (pass) {
+                const int at = __popc(mask & ((1u << lane) - 1u));
+                const float4 *tp = m.tri_s + 3 * (size_t)k;
+                S.sph[at] = s;
+                S.kk[at] = k;
+                S.tri[at][0] = __ldg(tp); S.tri[at][1] = __ldg(tp + 1); S.tri[at][2] = __ldg(tp + 2);
+            }
+            __syncwarp();
+            for (int j = rep_id; j < cnt; j += REP) lane_test(S.kk[j], S.sph[j], &S.tri[j][0]);
+            if (REP > 1) {                                      // replicas of a point share their best
+#pragma unroll
+                for (int o = PPW; o < 32; o <<= 1) {
+                    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+                    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                    if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+                }
+                sbA = best > 0.f ? best * rsqrtf(best) * 1.00001f + 1e-6f : 1e-6f;
+            }
+            ubA = fminf(ubA, warp_max(sbA));                   // the lanes' bounds only shrink: cull the next chunk harder
+            __syncwarp();
+        };
+        if constexpr (BRICK) {
+            // the list is sorted by box distance to the brick, which bounds from below every lane's distance to the
+            // leaf's faces: once a step's first leaf is farther than the loosest lane bound, so is the rest of the list
+            const int o1 = __ldg(m.boff + b + 1);
+            for (int base = __ldg(m.boff + b); base < o1; base += 8) {
+                const int slot = base + (lane >> 2);
+                const int leaf = slot < o1 ? (int)__ldg(m.blist + slot) : -1;
+                float key = 0.f;
+                if (lane == 0) key = leaf_key(m, leaf, blo, bhi);
+                if (__shfl_sync(0xffffffffu, key, 0) > ubA * ubA) break;
+                STAT(2, min(8, o1 - base));
+                chunk(leaf);
+            }
+        } else if (!overflow) {
             for (int base = 0; base < n; base += 8) {
                 const int slot = base + (lane >> 2);
-                bool pass = false;
-                int k = 0;
-                float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (slot < n) {
-                    k = 4 * (int)S.fr[cur][slot] + (lane & 3);
-                    if (k < m.F) {
-                        s = __ldg(m.sph_s + k);
-                        const float l2 = ubA + s.w;            // sphere vs the warp's box: some lane may be that close
-                        pass = box_dist2(mk3(s.x, s.y, s.z), wlo, whi) <= l2 * l2;
-                    }
-                }
-                const unsigned mask = __ballot_sync(0xffffffffu, pass);
-                const int cnt = __popc(mask);
-                STAT(3, cnt);
-                if (pass) {
-                    const int at = __popc(mask & ((1u << lane) - 1u));
-                    const float4 *tp = m.tri_s + 3 * (size_t)k;
-                    S.sph[at] = s;
-                    S.kk[at] = k;
-                    S.tri[at][0] = __ldg(tp); S.tri[at][1] = __ldg(tp + 1); S.tri[at][2] = __ldg(tp + 2);
-                }
-                __syncwarp();
-                for (int j = rep_id; j < cnt; j += REP) lane_test(S.kk[j], S.sph[j], &S.tri[j][0]);
-                if (REP > 1) {                                  // replicas of a point share their best
-#pragma unroll
-                    for (int o = PPW; o < 32; o <<= 1) {
-                        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-                        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                        if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-                    }
-                    sbA = best > 0.f ? best * rsqrtf(best) * 1.00001f + 1e-6f : 1e-6f;
-                }
-                ubA = fminf(ubA, warp_max(sbA));               // the lanes' bounds only shrink: cull the next chunk harder
-                __syncwarp();
+                chunk(slot < n ? (int)S.fr[cur][slot] : -1);
             }
         } else {
             for (int k = rep_id; k < m.F; k += REP) {
@@ -398,7 +477,6 @@ __global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xy
     }
     // ---- +x ray parity
     int hits = 0;
-    const MeshHeader h = *m.hdr;
     if (!h.ray_overflow) {
         const float fy = (p.y - h.y0) * h.inv_cy, fz = (p.z - h.z0) * h.inv_cz;
         if (fy >= 0.f && fy < (float)RAY_GRID && fz >= 0.f && fz < (float)RAY_GRID) {
@@ -422,6 +500,100 @@ __global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xy
         for (int o = PPW; o < 32; o <<= 1) hits += __shfl_xor_sync(0xffffffffu, hits, o);
     }
     if (live && rep_id == 0) emit_record(p, bi, best, hits, m, rec, face, idx);
+}
+
+// Without `defer`, warp i of the grid takes the points of warp i.  BRICK appends the warps it leaves to the tree walk
+// to defer[] (count *ndefer); the tree walk given `defer` strides over those warps instead.
+template <int PPW, bool BRICK>
+__global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xyz4, const int32_t *__restrict__ perm,
+                                                   int64_t N, MeshView m, float *__restrict__ rec,
+                                                   int32_t *__restrict__ face, int order, int32_t *__restrict__ defer,
+                                                   int32_t *__restrict__ ndefer) {
+    static_assert(!BRICK || PPW == 32, "brick lists serve dense lattices: 32 points per warp");
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    SdfSmem<PPW, BRICK> &S = reinterpret_cast<SdfSmem<PPW, BRICK> *>(smem_raw)[threadIdx.x >> 5];
+    const bool listed = !BRICK && defer != nullptr;
+    const int64_t nw = listed ? (int64_t)*ndefer : (N + PPW - 1) / PPW;
+    for (int64_t i = (int64_t)blockIdx.x * (SW_T / 32) + (threadIdx.x >> 5); i < nw; i += (int64_t)gridDim.x * (SW_T / 32))
+        sdf_warp<PPW, BRICK>(listed ? (int64_t)defer[i] : i, S, xyz4, perm, N, m, rec, face, order, defer, ndefer);
+}
+
+// ---------------------------------------------------------------- brick leaf lists (built once per body)
+__global__ void k_brick_centres(MeshView m) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= NBRICK) return;
+    float4 lo, hi;
+    brick_box(b, lo, hi);
+    m.bxyz[b] = make_float4(0.5f * (lo.x + hi.x), 0.5f * (lo.y + hi.y), 0.5f * (lo.z + hi.z), 0.f);
+    m.bperm[b] = b;
+}
+
+// bound of the brick (every point of it is within sqrt(d) + half-diagonal of the face nearest its centre) and the
+// length of its list: the leaves whose box lies within that bound of the brick's box
+__global__ void __launch_bounds__(128) k_brick_count(MeshView m) {
+    __shared__ int s_cnt;
+    const int b = blockIdx.x;
+    float4 lo, hi;
+    brick_box(b, lo, hi);
+    const float4 cc = m.bxyz[b];
+    const Tri t = load_tri(m.tri + 3 * (size_t)m.bface[b]);
+    const float d = tri_sqdist(mk3(cc.x, cc.y, cc.z), t.a, t.ab, t.ac);
+    const float ub = (sqrtf(d) + BRICK_HALF_DIAG) * 1.00001f + 1e-6f, ub2 = ub * ub;
+    if (threadIdx.x == 0) s_cnt = 0;
+    __syncthreads();
+    int cnt = 0;
+    for (int l = threadIdx.x; l < m.lvl_cnt[0]; l += blockDim.x) cnt += leaf_key(m, l, lo, hi) <= ub2;
+    for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&s_cnt, cnt);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        m.bub[b] = ub;
+        m.boff[b] = s_cnt;
+        if (s_cnt > BRICK_MAX_LEAVES) m.hdr->brick_overflow = 1;
+        if (b == 0) m.boff[NBRICK] = 0;
+    }
+}
+
+// after the scan: the brick's leaves compacted in leaf order, then rank-sorted by key (ties: leaf order)
+__global__ void __launch_bounds__(128) k_brick_fill(MeshView m, int64_t cap) {
+    __shared__ float s_key[BRICK_MAX_LEAVES];
+    __shared__ unsigned short s_leaf[BRICK_MAX_LEAVES];
+    __shared__ int s_wcnt[4];
+    if (m.hdr->brick_overflow || m.boff[NBRICK] > cap) return;      // k_brick_done records the overflow
+    const int b = blockIdx.x, o0 = m.boff[b], lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    float4 lo, hi;
+    brick_box(b, lo, hi);
+    const float ub = m.bub[b], ub2 = ub * ub;
+    const int nleaf = m.lvl_cnt[0];
+    int n = 0;
+    for (int l0 = 0; l0 < nleaf; l0 += 128) {
+        const int l = l0 + threadIdx.x;
+        float key = 0.f;
+        if (l < nleaf) key = leaf_key(m, l, lo, hi);
+        const bool in = l < nleaf && key <= ub2;
+        const unsigned bal = __ballot_sync(0xffffffffu, in);
+        if (lane == 0) s_wcnt[wib] = __popc(bal);
+        __syncthreads();
+        int at = n + __popc(bal & ((1u << lane) - 1u));
+        for (int w = 0; w < wib; ++w) at += s_wcnt[w];
+        if (in) { s_key[at] = key; s_leaf[at] = (unsigned short)l; }
+        n += s_wcnt[0] + s_wcnt[1] + s_wcnt[2] + s_wcnt[3];
+        __syncthreads();
+    }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const float k = s_key[i];
+        int r = 0;
+        for (int j = 0; j < n; ++j) {
+            const float kj = s_key[j];
+            r += kj < k || (kj == k && j < i);
+        }
+        m.blist[o0 + r] = s_leaf[i];
+    }
+}
+
+__global__ void k_brick_done(MeshView m, int64_t cap) {
+    if (m.boff[NBRICK] > cap) m.hdr->brick_overflow = 1;
+    m.hdr->brick_built = 1;
 }
 
 // brute force: every point against every face, faces staged through shared memory
@@ -457,11 +629,25 @@ __global__ void __launch_bounds__(256) k_sdf_brute(const float *__restrict__ pts
 static int64_t g_sdf_ppw32_from = 6000000, g_sdf_ppw8_from = 300000;
 static int g_sdf_order = -1;          // near-first leaf order: experimental, OFF unless ICON_B200_SDF_ORDER=1
 static int g_sdf_ppw_force = 0;
+static int g_sdf_bricks = 1;              // brick leaf lists on PPW = 32 calls (icon_set_sdf_bricks)
+static int64_t g_brick_max_entries = 0;   // > 0: a build may use at most this many list entries
+
+// Prepared bodies whose brick lists have been enqueued, by mesh header.  icon_smpl_prepare forgets its workspace, so
+// a new body -- also one that reuses freed memory -- gets fresh lists.  The kernel itself only trusts the header.
+static std::mutex g_brick_mu;
+static std::unordered_set<const void *> g_brick_ready;
+static int64_t g_brick_builds = 0;
+
+void bricks_forget(const MeshView &m) {
+    std::lock_guard<std::mutex> lk(g_brick_mu);
+    g_brick_ready.erase(m.hdr);
+}
 
 // ---------------------------------------------------------------- host-side pipeline pieces
 struct SdfWs {
     float4 *xyz4;
     int32_t *bid, *perm, *count, *offset;
+    int32_t *defer, *ndefer;              // warps the brick path leaves to the tree walk
     void *scan_ws;
 };
 static SdfWs carve_sdf(Carver &c, int64_t N) {
@@ -471,8 +657,31 @@ static SdfWs carve_sdf(Carver &c, int64_t N) {
     w.perm = c.take<int32_t>((size_t)N);
     w.count = c.take<int32_t>(NBIN + 1);
     w.offset = c.take<int32_t>(NBIN + 1);
+    w.defer = c.take<int32_t>((size_t)(N + 31) / 32);
+    w.ndefer = c.take<int32_t>(1);
     w.scan_ws = c.take<char>(scan_ws_bytes(NBIN + 1));
     return w;
+}
+
+// The brick leaf lists of one body (DESIGN.md 4.2): the exact nearest face of each brick centre (the SDF kernel on
+// the 32768 centres) bounds the nearest distance of every point of the brick; count, scan and fill the lists of leaves
+// within that bound, each sorted by box distance.  Stream-ordered: the header's flag is set last.
+static int build_bricks(const MeshView &m, cudaStream_t stream) {
+    const int64_t cap = g_brick_max_entries > 0 ? std::min(g_brick_max_entries, m.brick_cap) : m.brick_cap;
+    k_brick_centres<<<NBRICK / 256, 256, 0, stream>>>(m);
+    ICON_LAUNCHED();
+    k_sdf_warp<1, false><<<NBRICK / (SW_T / 32), SW_T, sdf_smem_bytes<1, false>(), stream>>>(
+        m.bxyz, m.bperm, NBRICK, m, m.brec, m.bface, 0, nullptr, nullptr);
+    ICON_LAUNCHED();
+    k_brick_count<<<NBRICK, 128, 0, stream>>>(m);
+    ICON_LAUNCHED();
+    int rc = scan_exclusive_i32(m.boff, m.boff, NBRICK + 1, nullptr, m.scan_ws, stream);
+    if (rc) return rc;
+    k_brick_fill<<<NBRICK, 128, 0, stream>>>(m, cap);
+    ICON_LAUNCHED();
+    k_brick_done<<<1, 1, 0, stream>>>(m, cap);
+    ICON_LAUNCHED();
+    return ICON_OK;
 }
 size_t sdf_ws_bytes(int64_t N) {
     Carver c(nullptr);
@@ -509,9 +718,10 @@ int run_sdf(const float *points, int64_t sc, int64_t sn, int64_t N, const float 
     ICON_LAUNCHED();
     static bool attr_set[ICON_MAX_DEVICES] = {};
     if (device_needs_setup(attr_set)) {
-#define ICON_SDF_ATTR(P) ICON_CUDA(cudaFuncSetAttribute(k_sdf_warp<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                                        (int)(sizeof(WarpSmem<fr_cap(P)>) * (SW_T / 32))))
-        ICON_SDF_ATTR(32); ICON_SDF_ATTR(16); ICON_SDF_ATTR(8); ICON_SDF_ATTR(4); ICON_SDF_ATTR(2); ICON_SDF_ATTR(1);
+#define ICON_SDF_ATTR(P, B) ICON_CUDA(cudaFuncSetAttribute(k_sdf_warp<P, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                                           (int)sdf_smem_bytes<P, B>()))
+        ICON_SDF_ATTR(32, true); ICON_SDF_ATTR(32, false); ICON_SDF_ATTR(16, false); ICON_SDF_ATTR(8, false);
+        ICON_SDF_ATTR(4, false); ICON_SDF_ATTR(2, false); ICON_SDF_ATTR(1, false);
 #undef ICON_SDF_ATTR
     }
     profile_mark(1, stream);
@@ -529,15 +739,39 @@ int run_sdf(const float *points, int64_t sc, int64_t sn, int64_t N, const float 
     const int wpb = SW_T / 32;
     const int64_t nwarps = (N + ppw - 1) / ppw;
     const unsigned nblk_w = (unsigned)((nwarps + wpb - 1) / wpb);
-#define ICON_SDF_LAUNCH(P) k_sdf_warp<P><<<nblk_w, SW_T, sizeof(WarpSmem<fr_cap(P)>) * (SW_T / 32), stream>>>( \
-        w.xyz4, w.perm, N, m, rec, face, g_sdf_order)
-    switch (ppw) {
-        case 32: ICON_SDF_LAUNCH(32); break;
-        case 16: ICON_SDF_LAUNCH(16); break;
-        case 8: ICON_SDF_LAUNCH(8); break;
-        case 4: ICON_SDF_LAUNCH(4); break;
-        case 2: ICON_SDF_LAUNCH(2); break;
-        default: ICON_SDF_LAUNCH(1); break;
+#define ICON_SDF_LAUNCH(P) k_sdf_warp<P, false><<<nblk_w, SW_T, sdf_smem_bytes<P, false>(), stream>>>( \
+        w.xyz4, w.perm, N, m, rec, face, g_sdf_order, nullptr, nullptr)
+    if (ppw == 32 && g_sdf_bricks) {
+        // dense call: the brick lists of this body, built by its first dense call, then the brick path and the tree
+        // walk over the warps it leaves (those straddling bricks or outside the cube; all of them if the lists
+        // overflowed), on a grid that fills the GPU once
+        bool build;
+        {
+            std::lock_guard<std::mutex> lk(g_brick_mu);
+            build = g_brick_ready.insert(m.hdr).second;
+        }
+        if (build) {
+            rc = build_bricks(m, stream);
+            std::lock_guard<std::mutex> lk(g_brick_mu);
+            if (rc) { g_brick_ready.erase(m.hdr); return rc; }
+            ++g_brick_builds;
+        }
+        ICON_CUDA(cudaMemsetAsync(w.ndefer, 0, sizeof(int32_t), stream));
+        k_sdf_warp<32, true><<<nblk_w, SW_T, sdf_smem_bytes<32, true>(), stream>>>(
+            w.xyz4, w.perm, N, m, rec, face, g_sdf_order, w.defer, w.ndefer);
+        ICON_LAUNCHED();
+        const unsigned nblk_d = (unsigned)std::min<int64_t>(nblk_w, (int64_t)device_sm_count() * 16);
+        k_sdf_warp<32, false><<<nblk_d, SW_T, sdf_smem_bytes<32, false>(), stream>>>(
+            w.xyz4, w.perm, N, m, rec, face, g_sdf_order, w.defer, w.ndefer);
+    } else {
+        switch (ppw) {
+            case 32: ICON_SDF_LAUNCH(32); break;
+            case 16: ICON_SDF_LAUNCH(16); break;
+            case 8: ICON_SDF_LAUNCH(8); break;
+            case 4: ICON_SDF_LAUNCH(4); break;
+            case 2: ICON_SDF_LAUNCH(2); break;
+            default: ICON_SDF_LAUNCH(1); break;
+        }
     }
 #undef ICON_SDF_LAUNCH
     ICON_LAUNCHED();
@@ -581,6 +815,32 @@ extern "C" int icon_set_sdf_policy(int force_ppw, int64_t ppw8_from, int64_t ppw
     icon::g_sdf_ppw_force = force_ppw;
     if (ppw8_from >= 0) icon::g_sdf_ppw8_from = ppw8_from;
     if (ppw32_from >= 0) icon::g_sdf_ppw32_from = ppw32_from;
+    return ICON_OK;
+}
+
+extern "C" int icon_set_sdf_bricks(int enable, int64_t max_entries) {
+    ICON_CHECK_ARG(enable == 0 || enable == 1, "icon_set_sdf_bricks: enable must be 0 or 1");
+    icon::g_sdf_bricks = enable;
+    icon::g_brick_max_entries = max_entries > 0 ? max_entries : 0;
+    return ICON_OK;
+}
+
+extern "C" int icon_sdf_brick_info(const void *mesh_ws, int V, int F, int64_t *out) {
+    ICON_CHECK_ARG(mesh_ws && out && V > 0 && F > 0, "icon_sdf_brick_info: bad argument");
+    MeshView m = mesh_view(mesh_ws, V, F);
+    MeshHeader h;
+    int32_t total = 0;
+    ICON_CUDA(cudaDeviceSynchronize());
+    ICON_CUDA(cudaMemcpy(&h, m.hdr, sizeof(h), cudaMemcpyDeviceToHost));
+    if (h.brick_built) ICON_CUDA(cudaMemcpy(&total, m.boff + NBRICK, sizeof(total), cudaMemcpyDeviceToHost));
+    out[0] = h.brick_built;
+    out[1] = h.brick_overflow;
+    out[2] = total;
+    out[3] = m.brick_cap;
+    {
+        std::lock_guard<std::mutex> lk(icon::g_brick_mu);
+        out[4] = icon::g_brick_builds;
+    }
     return ICON_OK;
 }
 

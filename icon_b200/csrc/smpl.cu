@@ -43,6 +43,14 @@ static MeshView carve_mesh(Carver &c, int V, int F) {
     m.rlist = c.take<int32_t>((size_t)F * RAY_LIST_PER_FACE);
     m.hdr = c.take<MeshHeader>(1);
     m.scan_ws = c.take<char>(scan_ws_bytes(RAY_GRID * RAY_GRID + 1));
+    m.bxyz = c.take<float4>(NBRICK);
+    m.bperm = c.take<int32_t>(NBRICK);
+    m.brec = c.take<float>((size_t)NBRICK * 8);
+    m.bface = c.take<int32_t>(NBRICK);
+    m.bub = c.take<float>(NBRICK);
+    m.boff = c.take<int32_t>(NBRICK + 1);
+    m.brick_cap = brick_list_cap(F);
+    m.blist = c.take<unsigned short>((size_t)m.brick_cap);
     m.vnormals = c.take<float>((size_t)V * 3);      // last: tests read it from the tail
     return m;
 }
@@ -216,7 +224,7 @@ __global__ void __launch_bounds__(1024) k_build_tree(const float4 *__restrict__ 
         h.inv_cy = (float)RAY_GRID / ((hi.y + pad) - h.y0);
         h.inv_cz = (float)RAY_GRID / ((hi.z + pad) - h.z0);
         h.ray_overflow = 0;
-        h.pad[0] = h.pad[1] = h.pad[2] = 0;
+        h.brick_built = h.brick_overflow = h.pad = 0;
         *m.hdr = h;
     }
 }
@@ -275,6 +283,7 @@ extern "C" int icon_smpl_prepare(const float *verts, const int64_t *faces, const
     }
     Carver c(mesh_ws);
     MeshView m = carve_mesh(c, V, F);
+    bricks_forget(m);
     void *scan_ws = m.scan_ws;
     k_vertex_normals<<<(V + 127) / 128, 128, 0, stream>>>(verts, faces, V, F, m.vnormals);
     ICON_LAUNCHED();
