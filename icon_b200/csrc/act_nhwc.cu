@@ -1,8 +1,8 @@
 // NHWC companions of conv_nhwc.cu: everything between two convolutions of the encoders in ONE pass each.
 //
-//   k_norm_finalize   per-(image, channel) sums from the producing kernel's epilogue -> (scale, shift) per channel for
+//   k_norm_finalize   per-(image, channel) sums from the producing kernel's epilogue -> (scale, mean, beta) per channel for
 //                     nn.InstanceNorm2d(affine=False) / nn.GroupNorm(32, C)        (FBNet.py:216-261, net_util.py:258-280)
-//   k_act_nhwc        y = [relu]( x * scale + shift ) [+ residual]  ->  fp16 hi / lo NHWC operand tensors in the layout the
+//   k_act_nhwc        y = [relu]( (x - mean) * scale + beta ) [+ residual]  ->  fp16 hi / lo NHWC operand tensors in the layout the
 //                     CONSUMING convolution wants (reflection halo, space-to-depth planes for stride 2, channel padding
 //                     to 64) and / or an fp32 NHWC tensor
 //   k_ew_nhwc         add2 / add3 / 2x2 average pool / bicubic x2 upsample + add (HGFilters.py:49-79), each also
@@ -14,10 +14,13 @@
 
 namespace icon {
 
-// ---------------------------------------------------------------------------------------- statistics -> scale / shift
-// stats [N][C][2] doubles (sum, sum of squares over `count` pixels).  groups == 0: per channel (instance norm).
+// ---------------------------------------------------------------------------------------- statistics -> scale / mean / beta
+// stats [N][C][6] doubles (sum, sum of squares over `count` pixels: stats_add in common.cuh) -> ss [N][C][3] (scale, mean,
+// beta).  Consumers compute (x - mean) * scale + beta like torch, so a constant channel gives exactly beta (its mean is
+// exact), which a folded shift = beta - mean * scale would miss by the rounding of mean * scale.  groups == 0: per
+// channel (instance norm).
 __global__ void k_norm_finalize(const double *__restrict__ stats, const float *__restrict__ gamma,
-                                const float *__restrict__ beta, float2 *__restrict__ ss, int N, int C, int groups,
+                                const float *__restrict__ beta, float *__restrict__ ss, int N, int C, int groups,
                                 double count, float eps) {
     pdl_launch_dependents();
     pdl_wait();
@@ -26,12 +29,12 @@ __global__ void k_norm_finalize(const double *__restrict__ stats, const float *_
     const int n = i / C, c = i % C;
     double s = 0.0, q = 0.0, cnt = count;
     if (groups <= 0) {
-        s = stats[(size_t)i * 2]; q = stats[(size_t)i * 2 + 1];
+        s = stats_sum(stats + (size_t)i * 6); q = stats_sumsq(stats + (size_t)i * 6);
     } else {
         const int cg = C / groups, g0 = (c / cg) * cg;
         for (int k = 0; k < cg; ++k) {
-            s += stats[((size_t)n * C + g0 + k) * 2];
-            q += stats[((size_t)n * C + g0 + k) * 2 + 1];
+            s += stats_sum(stats + ((size_t)n * C + g0 + k) * 6);
+            q += stats_sumsq(stats + ((size_t)n * C + g0 + k) * 6);
         }
         cnt = count * cg;
     }
@@ -40,14 +43,14 @@ __global__ void k_norm_finalize(const double *__restrict__ stats, const float *_
     if (var < 0.0) var = 0.0;
     const float rstd = (float)(1.0 / sqrt(var + (double)eps));
     const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
-    ss[i] = make_float2(rstd * g, b - (float)mean * rstd * g);
+    ss[(size_t)i * 3] = rstd * g; ss[(size_t)i * 3 + 1] = (float)mean; ss[(size_t)i * 3 + 2] = b;
 }
 
 // ---------------------------------------------------------------------------------------- normalise + split
 struct ActParams {
     const float *x;          // fp32 NHWC [N][H][W][Cs_in], channels [ci_off, ci_off + C)
-    const float2 *ss;        // [N][C] scale / shift or null
-    const double *stats;     // or: [N][C][2] sums straight from the producer (normalisation folded in here); both null =
+    const float *ss;         // [N][C][3] scale / mean / beta (k_norm_finalize) or null
+    const double *stats;     // or: [N][C][6] sums straight from the producer (normalisation folded in here); both null =
     const float *gamma, *beta;   // identity.  gamma / beta: GroupNorm affine or null
     int cg;                  // channels per normalisation group (1 = instance norm), 8 % cg == 0
     double inv_count;        // 1 / (pixels * cg)
@@ -91,25 +94,24 @@ __global__ void k_act_nhwc(const __grid_constant__ ActParams p) {
         for (int k = 0; k < 8; ++k) v[k] = (c0 + k < p.C) ? xs[k] : 0.f;
     }
     if (p.ss) {
-        const float2 *ss = p.ss + (size_t)n * p.C + c0;
+        const float *ss = p.ss + ((size_t)n * p.C + c0) * 3;
 #pragma unroll
         for (int k = 0; k < 8; ++k)
-            if (c0 + k < p.C) { const float2 s = __ldg(ss + k); v[k] = fmaf(v[k], s.x, s.y); }
+            if (c0 + k < p.C) v[k] = fmaf(v[k] - __ldg(ss + 3 * k + 1), __ldg(ss + 3 * k), __ldg(ss + 3 * k + 2));
     } else if (p.stats) {
-        // scale / shift from the producer's sums: a thread's 8 channels hold whole groups (cg in {1, 2, 4, 8})
-        const double *st = p.stats + ((size_t)n * p.C + c0) * 2;
+        // mean / scale from the producer's sums: a thread's 8 channels hold whole groups (cg in {1, 2, 4, 8})
+        const double *st = p.stats + ((size_t)n * p.C + c0) * 6;
         for (int g0 = 0; g0 < 8; g0 += p.cg) {
             if (c0 + g0 >= p.C) break;
             double s = 0.0, q = 0.0;
-            for (int k = 0; k < p.cg; ++k) { s += st[(g0 + k) * 2]; q += st[(g0 + k) * 2 + 1]; }
+            for (int k = 0; k < p.cg; ++k) { s += stats_sum(st + (g0 + k) * 6); q += stats_sumsq(st + (g0 + k) * 6); }
             const double mean = s * p.inv_count;
             const float var = fmaxf((float)(q * p.inv_count - mean * mean), 0.f);
-            const float rstd = rsqrtf(var + p.eps);
+            const float rstd = rsqrtf(var + p.eps), mf = (float)mean;
             for (int k = 0; k < p.cg; ++k) {
                 const int c = c0 + g0 + k;
                 const float ga = p.gamma ? __ldg(p.gamma + c) : 1.f, be = p.beta ? __ldg(p.beta + c) : 0.f;
-                const float sc = rstd * ga;
-                v[g0 + k] = fmaf(v[g0 + k], sc, be - (float)mean * sc);
+                v[g0 + k] = fmaf(v[g0 + k] - mf, rstd * ga, be);
             }
         }
     }
@@ -177,7 +179,7 @@ struct SkActParams {
 
 __global__ void __launch_bounds__(256) k_splitk_in_act(const __grid_constant__ SkActParams p) {
     extern __shared__ float4 sval[];                           // [H*W][2]: 8 channels per pixel
-    __shared__ float sw[8][8];
+    __shared__ double sw[8][8];
     __shared__ float s_mean[8], s_rstd[8];
     pdl_launch_dependents();
     pdl_wait();
@@ -187,7 +189,7 @@ __global__ void __launch_bounds__(256) k_splitk_in_act(const __grid_constant__ S
     const size_t split_stride = (size_t)p.N * HW * p.C;
     float4 b0 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = b0;
     if (p.bias) { b0 = *reinterpret_cast<const float4 *>(p.bias + c0); b1 = *reinterpret_cast<const float4 *>(p.bias + c0 + 4); }
-    float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    double s[8] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};   // fp64: the centred pass is only as good as this mean
     for (int pix = tid; pix < HW; pix += 256) {
         const float *src = p.partial + ((size_t)n * HW + pix) * p.C + c0;
         float4 v0 = b0, v1 = b1;
@@ -200,7 +202,7 @@ __global__ void __launch_bounds__(256) k_splitk_in_act(const __grid_constant__ S
         sval[2 * pix] = v0; sval[2 * pix + 1] = v1;
         s[0] += v0.x; s[1] += v0.y; s[2] += v0.z; s[3] += v0.w; s[4] += v1.x; s[5] += v1.y; s[6] += v1.z; s[7] += v1.w;
     }
-    auto block_sum8 = [&](float (&x)[8], float *out8) {        // deterministic: shuffle tree, then warps in order
+    auto block_sum8 = [&](auto (&x)[8], float *out8) {         // deterministic: shuffle tree, then warps in order
 #pragma unroll
         for (int k = 0; k < 8; ++k)
 #pragma unroll
@@ -212,7 +214,7 @@ __global__ void __launch_bounds__(256) k_splitk_in_act(const __grid_constant__ S
         __syncthreads();
         if (tid < 8) {
             double t = 0.0;
-            for (int ww = 0; ww < 8; ++ww) t += (double)sw[ww][tid];
+            for (int ww = 0; ww < 8; ++ww) t += sw[ww][tid];
             out8[tid] = (float)(t / (double)HW);
         }
         __syncthreads();
@@ -274,11 +276,11 @@ __global__ void __launch_bounds__(256) k_splitk_in_act(const __grid_constant__ S
 struct EwParams {
     const float *a, *b, *c;  // fp32 NHWC
     float *y;
-    double *stats;           // [N][C][2] or null
+    double *stats;           // [N][C][6] (stats_add in common.cuh) or null
     int N, H, W, C;          // OUTPUT dims
     int mode;                // 0: a + b (+ c)   1: avg_pool2(a) (a is [N][2H][2W][C])   2: b + bicubic_up2(a) (a is [N][H/2][W/2][C])
-                             // 3: relu(a * scale + shift), scale / shift = ss[n][c]   (a norm whose RESULT feeds another norm)
-    const float2 *ss;
+                             // 3: relu((a - mean) * scale + beta) from ss[n][c][3]   (a norm whose RESULT feeds another norm)
+    const float *ss;
 };
 
 __device__ __forceinline__ void cubic_w4(float t, float (&w)[4]) {     // torch upsample_bicubic2d, A = -0.75
@@ -295,13 +297,13 @@ constexpr int EW_PIX = 64;           // pixels per block (more blocks = more sam
 __global__ void __launch_bounds__(256) k_ew_nhwc(const __grid_constant__ EwParams p) {
     pdl_launch_dependents();
     pdl_wait();
-    __shared__ float sred[2][256 * 4];                         // [sum | sum of squares][row][channel]: rows * C = 1024
+    __shared__ double sred[2][256 * 4];                        // [sum | sum of squares][row][channel]: rows * C = 1024
     const int quads = p.C / 4, rows = 256 / quads;
     const int q = threadIdx.x % quads, r0 = threadIdx.x / quads;
     const int n = blockIdx.y;
     const unsigned hw = (unsigned)p.H * (unsigned)p.W;
     const unsigned pix0 = blockIdx.x * EW_PIX;
-    float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1;
+    double s1[4] = {0.0, 0.0, 0.0, 0.0}, s2[4] = {0.0, 0.0, 0.0, 0.0};
     for (int pr = r0; pr < EW_PIX; pr += rows) {
         const unsigned pix = pix0 + pr;
         if (pix >= hw) break;
@@ -317,9 +319,9 @@ __global__ void __launch_bounds__(256) k_ew_nhwc(const __grid_constant__ EwParam
             }
         } else if (p.mode == 3) {
             v = *reinterpret_cast<const float4 *>(p.a + o);
-            const float2 *ss = p.ss + (size_t)n * p.C + q * 4;
-            v.x = fmaxf(fmaf(v.x, ss[0].x, ss[0].y), 0.f); v.y = fmaxf(fmaf(v.y, ss[1].x, ss[1].y), 0.f);
-            v.z = fmaxf(fmaf(v.z, ss[2].x, ss[2].y), 0.f); v.w = fmaxf(fmaf(v.w, ss[3].x, ss[3].y), 0.f);
+            const float *ss = p.ss + ((size_t)n * p.C + q * 4) * 3;
+            v.x = fmaxf(fmaf(v.x - ss[1], ss[0], ss[2]), 0.f); v.y = fmaxf(fmaf(v.y - ss[4], ss[3], ss[5]), 0.f);
+            v.z = fmaxf(fmaf(v.z - ss[7], ss[6], ss[8]), 0.f); v.w = fmaxf(fmaf(v.w - ss[10], ss[9], ss[11]), 0.f);
         } else if (p.mode == 1) {
             const int oy = (int)(pix / p.W), ox = (int)(pix % p.W);
             const int W2 = 2 * p.W;
@@ -358,19 +360,21 @@ __global__ void __launch_bounds__(256) k_ew_nhwc(const __grid_constant__ EwParam
             v = make_float4(acc.x + b.x, acc.y + b.y, acc.z + b.z, acc.w + b.w);
         }
         *reinterpret_cast<float4 *>(p.y + o) = v;
-        s1.x += v.x; s1.y += v.y; s1.z += v.z; s1.w += v.w;
-        s2.x = fmaf(v.x, v.x, s2.x); s2.y = fmaf(v.y, v.y, s2.y); s2.z = fmaf(v.z, v.z, s2.z); s2.w = fmaf(v.w, v.w, s2.w);
+        if (p.stats) {
+            const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) { s1[j] += e[j]; s2[j] = fma((double)e[j], (double)e[j], s2[j]); }
+        }
     }
     if (!p.stats) return;
     // per-channel sums of the block in a fixed order (row 0, 1, ...): deterministic, no shared-memory atomics
-    *reinterpret_cast<float4 *>(&sred[0][r0 * p.C + q * 4]) = s1;
-    *reinterpret_cast<float4 *>(&sred[1][r0 * p.C + q * 4]) = s2;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { sred[0][r0 * p.C + q * 4 + j] = s1[j]; sred[1][r0 * p.C + q * 4 + j] = s2[j]; }
     __syncthreads();
-    for (int i = threadIdx.x; i < 2 * p.C; i += 256) {
-        const int w = i / p.C, c = i - w * p.C;
-        double t = 0.0;
-        for (int r = 0; r < rows; ++r) t += (double)sred[w][r * p.C + c];
-        atomicAdd(p.stats + ((size_t)n * p.C + c) * 2 + w, t);
+    for (int c = threadIdx.x; c < p.C; c += 256) {
+        double t1 = 0.0, t2 = 0.0;
+        for (int r = 0; r < rows; ++r) { t1 += sred[0][r * p.C + c]; t2 += sred[1][r * p.C + c]; }
+        stats_add(p.stats + ((size_t)n * p.C + c) * 6, t1, t2);
     }
 }
 
@@ -391,16 +395,13 @@ __global__ void __launch_bounds__(256) k_nchw_to_nhwc(const float *__restrict__ 
         const float v = pix < HW ? x[((size_t)n * C + c) * HW + pix] : 0.f;
         tile[lane * (CB + 1) + cc] = v;
         if (stats) {
-            float s1 = v, s2 = v * v;
+            double s1 = v, s2 = (double)v * v;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
                 s1 += __shfl_xor_sync(0xffffffffu, s1, o);
                 s2 += __shfl_xor_sync(0xffffffffu, s2, o);
             }
-            if (lane == 0) {
-                atomicAdd(stats + ((size_t)n * C + c) * 2, (double)s1);
-                atomicAdd(stats + ((size_t)n * C + c) * 2 + 1, (double)s2);
-            }
+            if (lane == 0) stats_add(stats + ((size_t)n * C + c) * 6, s1, s2);
         }
     }
     __syncthreads();
@@ -517,7 +518,7 @@ extern "C" int icon_norm_finalize(const double *stats, const float *gamma, const
     ICON_CHECK_ARG(stats && scale_shift && N > 0 && C > 0 && count > 0, "icon_norm_finalize: bad argument");
     ICON_CHECK_ARG(groups <= 0 || C % groups == 0, "icon_norm_finalize: C %% groups != 0");
     ICON_CHECK_ARG((gamma == nullptr) == (beta == nullptr), "icon_norm_finalize: gamma and beta go together");
-    ICON_CUDA(launch_pdl(k_norm_finalize, dim3((N * C + 127) / 128), dim3(128), 0, stream, stats, gamma, beta, (float2 *)scale_shift, N,
+    ICON_CUDA(launch_pdl(k_norm_finalize, dim3((N * C + 127) / 128), dim3(128), 0, stream, stats, gamma, beta, scale_shift, N,
                          C, groups, count, eps));
     ICON_LAUNCHED();
     return ICON_OK;
@@ -543,7 +544,7 @@ extern "C" int icon_act_nhwc(const float *x, int Cs_in, int ci_off, const float 
         ICON_CHECK_ARG(p.cg == 1 || p.cg == 2 || p.cg == 4 || p.cg == 8, "icon_act_nhwc: %d channels per group (use icon_norm_finalize)", p.cg);
         p.inv_count = 1.0 / ((double)H * W * p.cg);
     }
-    p.x = x; p.ss = (const float2 *)scale_shift; p.res = res; p.hi = (__half *)hi; p.lo = (__half *)lo; p.f32 = f32;
+    p.x = x; p.ss = scale_shift; p.res = res; p.hi = (__half *)hi; p.lo = (__half *)lo; p.f32 = f32;
     p.N = N; p.H = H; p.W = W; p.C = C; p.Cs_in = Cs_in; p.ci_off = ci_off; p.Cp = Cp; p.P = halo; p.s2d = s2d; p.relu = relu;
     const int64_t total = (int64_t)N * (s2d ? H : H + 2 * halo) * (s2d ? W : W + 2 * halo) * (Cp / 8);
     ICON_CHECK_ARG(total < (int64_t)1 << 31, "icon_act_nhwc: activation too large for 32-bit indexing");
@@ -583,7 +584,7 @@ extern "C" int icon_ew_nhwc(int mode, const float *a, const float *b, const floa
     ICON_CHECK_ARG(mode != 2 || (H % 2 == 0 && W % 2 == 0), "icon_ew_nhwc: upsample output must be even");
     EwParams p{};
     p.a = a; p.b = mode == 3 ? nullptr : b; p.c = c; p.y = y; p.stats = stats; p.N = N; p.H = H; p.W = W; p.C = C; p.mode = mode;
-    p.ss = mode == 3 ? (const float2 *)b : nullptr;
+    p.ss = mode == 3 ? b : nullptr;
     dim3 grid((unsigned)(((int64_t)H * W + EW_PIX - 1) / EW_PIX), (unsigned)N);
     ICON_CUDA(launch_pdl(k_ew_nhwc, grid, dim3(256), 0, stream, p));
     ICON_LAUNCHED();

@@ -72,6 +72,26 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
     cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
+
+// Normalisation statistics of one (image, channel): st[6] = {sum x, sum x^2}, each as three fp64 words that hold the
+// multiples of 1, of 2^-32 and of 2^-64; zeroed by the caller.  Producers accumulate their partial sums in fp64 (x^2 of
+// an fp32 x is exact there, so the variance E[x^2] - E[x]^2 keeps ~1e-16 * (mean / std)^2 relative accuracy) and add
+// them here.  A partial is cut into its integer part, its fraction rounded to 2^-32 and the rest rounded to 2^-64, so
+// every fp64 atomic add below is exact while the integer parts stay under 2^53 and a channel receives fewer than 2^21
+// partials: the totals do not depend on the order in which blocks arrive (bitwise reproducible results, which CUDA-graph
+// replay relies on).  A partial moves by at most 2^-65; the sum of a constant channel is exact, so its mean equals the
+// value and the channel normalises to exactly beta.
+__device__ __forceinline__ void stats_add3(double *w, double s) {
+    const double a = trunc(s), r = s - a;
+    const double b = rint(r * 4294967296.0) * (1.0 / 4294967296.0);
+    const double c = rint((r - b) * 18446744073709551616.0) * (1.0 / 18446744073709551616.0);
+    if (a != 0.0) atomicAdd(w, a);
+    if (b != 0.0) atomicAdd(w + 1, b);
+    if (c != 0.0) atomicAdd(w + 2, c);
+}
+__device__ __forceinline__ void stats_add(double *st, double s1, double s2) { stats_add3(st, s1); stats_add3(st + 3, s2); }
+__device__ __forceinline__ double stats_sum(const double *st) { return st[0] + (st[1] + st[2]); }
+__device__ __forceinline__ double stats_sumsq(const double *st) { return st[3] + (st[4] + st[5]); }
 #endif
 
 // carve a workspace

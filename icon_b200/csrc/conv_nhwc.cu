@@ -18,8 +18,8 @@
 //   warps 0-7   two consumer warpgroups (warpgroup g: pixels [64 g, 64 g + 64) of the tile, M = 64, N = NT), then the
 //               epilogue: accumulators -> shared memory -> one column (channel) per thread walking the pixels:
 //               coalesced fp32 NHWC stores (optionally into a channel slice of a wider tensor = torch.cat for free),
-//               +bias, and per-(image, channel) sum / sum-of-squares for the Instance/GroupNorm that follows (fp64
-//               atomics), so the norm needs no statistics pass.
+//               +bias, and per-(image, channel) sum / sum-of-squares for the Instance/GroupNorm that follows (fp64,
+//               added with exact atomics: stats_add), so the norm needs no statistics pass.
 //   warp 8      producer: 2 tensor-map loads (A hi, A lo) + 1 bulk copy (B hi|lo) per chunk, STAGES-deep ring
 // Small spatial extents (the 32 x 32 ResnetBlocks) fill the machine through split-K (partials + k_splitk_nhwc).
 #include <cuda.h>
@@ -38,7 +38,7 @@ struct ConvNhwcParams {
     const float *bias;       // [Cout] or null
     float *out;              // fp32 NHWC [N][OHf][OWf][Cs], this conv writes channels [co_off, co_off + Cout)
     float *partial;          // splits > 1: [splits][N][Ht][Wt][Cout]
-    double *stats;           // [N][Cout][2] (sum, sum of squares) or null
+    double *stats;           // [N][Cout][6] (sum, sum of squares: stats_add in common.cuh) or null
     int N, Ht, Wt;           // logical output grid of this launch (per image)
     int BW, BH, tiles_x, tiles_y;
     int OHf, OWf, osy, osx, ooy, oox;     // out (y, x) = (a * osy + ooy, b * osx + oox)
@@ -158,29 +158,26 @@ k_conv_nhwc(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ 
     const int bw_shift = 31 - __clz(p.BW), bw_mask = p.BW - 1;
     const size_t split_stride = (size_t)p.N * p.Ht * p.Wt * p.Cout;
     const float bias = (fin && p.bias) ? __ldg(p.bias + co) : 0.f;
-    float s1 = 0.f, s2 = 0.f;
+    double s1 = 0.0, s2 = 0.0;
     for (int row = row0; row < 128; row += RSTEP) {
         const int a = y0 + (row >> bw_shift), b = x0 + (row & bw_mask);
         if (a >= p.Ht || b >= p.Wt) continue;
         const float val = tile[row * LD + col] + bias;
         if (fin) {
             p.out[(((size_t)n * p.OHf + (size_t)(a * p.osy + p.ooy)) * p.OWf + (size_t)(b * p.osx + p.oox)) * p.Cs + p.co_off + co] = val;
-            s1 += val; s2 = fmaf(val, val, s2);
+            s1 += val; s2 = fma((double)val, (double)val, s2);
         } else {
             p.partial[(size_t)blockIdx.z * split_stride + (((size_t)n * p.Ht + a) * p.Wt + b) * p.Cout + co] = val;
         }
     }
-    if (fin && p.stats) {
-        atomicAdd(p.stats + ((size_t)n * p.Cout + co) * 2, (double)s1);
-        atomicAdd(p.stats + ((size_t)n * p.Cout + co) * 2 + 1, (double)s2);
-    }
+    if (fin && p.stats) stats_add(p.stats + ((size_t)n * p.Cout + co) * 6, s1, s2);
 }
 
 // split-K finish: out = bias + sum_s partial[s] in split order (deterministic) + per-(image, channel) statistics.
 // Block = 32 pixels x 128 channels, 256 threads: lane = channel quad (128-bit loads, coalesced), warp = pixel slot,
 // 4 pixels per thread, every load of a thread independent.  grid (ceil(HW / 32), ceil(Cout / 128), N).
 __global__ void __launch_bounds__(256) k_splitk_nhwc(const __grid_constant__ ConvNhwcParams p) {
-    __shared__ float4 sred[2][8][32];
+    __shared__ double sred[2][8][128];
     pdl_launch_dependents();
     pdl_wait();
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -191,7 +188,7 @@ __global__ void __launch_bounds__(256) k_splitk_nhwc(const __grid_constant__ Con
     const bool cv = c < p.Cout;                                 // Cout % 4 == 0 is checked by the host for this kernel
     float4 bias = make_float4(0.f, 0.f, 0.f, 0.f);
     if (cv && p.bias) bias = *reinterpret_cast<const float4 *>(p.bias + c);
-    float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1;
+    double s1[4] = {0.0, 0.0, 0.0, 0.0}, s2[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
         const int64_t pix = (int64_t)blockIdx.x * 32 + k * 8 + w;
@@ -205,18 +202,19 @@ __global__ void __launch_bounds__(256) k_splitk_nhwc(const __grid_constant__ Con
         const int a = (int)(pix / p.Wt), b = (int)(pix % p.Wt);
         *reinterpret_cast<float4 *>(p.out + (((size_t)n * p.OHf + (size_t)(a * p.osy + p.ooy)) * p.OWf + (size_t)(b * p.osx + p.oox)) * p.Cs +
                                     p.co_off + c) = v;
-        s1.x += v.x; s1.y += v.y; s1.z += v.z; s1.w += v.w;
-        s2.x = fmaf(v.x, v.x, s2.x); s2.y = fmaf(v.y, v.y, s2.y); s2.z = fmaf(v.z, v.z, s2.z); s2.w = fmaf(v.w, v.w, s2.w);
+        const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { s1[j] += e[j]; s2[j] = fma((double)e[j], (double)e[j], s2[j]); }
     }
     if (!p.stats) return;
-    sred[0][w][lane] = s1; sred[1][w][lane] = s2;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { sred[0][w][lane * 4 + j] = s1[j]; sred[1][w][lane * 4 + j] = s2[j]; }
     __syncthreads();
-    const int t = threadIdx.x;                                  // 256 threads = 2 x 128 channels
-    const int which = t >> 7, cc = t & 127, co = blockIdx.y * 128 + cc;
-    if (co < p.Cout) {
-        double tot = 0.0;
-        for (int k = 0; k < 8; ++k) tot += (double)reinterpret_cast<const float *>(&sred[which][k][cc >> 2])[cc & 3];
-        atomicAdd(p.stats + ((size_t)n * p.Cout + co) * 2 + which, tot);
+    const int cc = threadIdx.x, co = blockIdx.y * 128 + cc;
+    if (cc < 128 && co < p.Cout) {                              // the block's 8 pixel slots in a fixed order
+        double t1 = 0.0, t2 = 0.0;
+        for (int k = 0; k < 8; ++k) { t1 += sred[0][k][cc]; t2 += sred[1][k][cc]; }
+        stats_add(p.stats + ((size_t)n * p.Cout + co) * 6, t1, t2);
     }
 }
 

@@ -24,12 +24,19 @@ from .ops import _need_cuda, _p, _sm_count, _stream
 
 
 class Raw:
-    """fp32 NHWC activation: channels [c_off, c_off + C) of tensor `t` [N, H, W, Cs]; `stats` [N, C, 2] float64 or None."""
+    """fp32 NHWC activation: channels [c_off, c_off + C) of tensor `t` [N, H, W, Cs].  `sums` is the float64
+    [N, C, 2, 3] buffer its producer's kernels accumulated the per-channel sum and sum of squares into (each as three
+    words, so that their atomic adds are exact: csrc/common.cuh stats_add) or None; `stats` reads it as [N, C, 2]
+    (sum, sum of squares)."""
 
-    def __init__(self, t, C=None, c_off=0, stats=None):
-        self.t, self.c_off, self.stats = t, c_off, stats
+    def __init__(self, t, C=None, c_off=0, sums=None):
+        self.t, self.c_off, self.sums = t, c_off, sums
         self.N, self.H, self.W, self.Cs = t.shape
         self.C = self.Cs if C is None else C
+
+    @property
+    def stats(self):
+        return None if self.sums is None else self.sums.sum(-1)
 
     def dense(self):
         return self.t if (self.c_off == 0 and self.C == self.Cs) else self.t[..., self.c_off:self.c_off + self.C].contiguous()
@@ -51,7 +58,7 @@ class _Arena:
     of one fill kernel per layer)."""
     cur = None
 
-    def __init__(self, device, doubles=1 << 18):
+    def __init__(self, device, doubles=3 << 18):
         self.buf = torch.zeros(doubles, dtype=torch.float64, device=device)
         self.off = 0
 
@@ -80,10 +87,10 @@ class stats_arena:
 def new_stats(N, C, device):
     a = _Arena.cur
     if a is not None and a.buf.device == torch.device(device):
-        v = a.take(N * C * 2)
+        v = a.take(N * C * 6)
         if v is not None:
-            return v[:N * C * 2].view(N, C, 2)
-    return torch.zeros(N, C, 2, dtype=torch.float64, device=device)
+            return v.view(N, C, 2, 3)
+    return torch.zeros(N, C, 2, 3, dtype=torch.float64, device=device)
 
 
 # ------------------------------------------------------------------------------------------------ layout adaptors
@@ -95,7 +102,7 @@ def raw_from_nchw(x, stats=True):
     y = torch.empty(N, H, W, C, dtype=torch.float32, device=x.device)
     st = new_stats(N, C, x.device) if stats else None
     check(lib.icon_nchw_to_nhwc(_p(x), _p(y), _p(st), N, C, H * W, _stream()), "icon_nchw_to_nhwc")
-    return Raw(y, stats=st)
+    return Raw(y, sums=st)
 
 
 def to_nchw(raw):
@@ -108,10 +115,11 @@ def to_nchw(raw):
 # ------------------------------------------------------------------------------------------------ normalisation
 class NormSpec:
     """A pending normalisation of `raw`: the producer's sums + the norm layer.  `act` folds it into its own pass when
-    a group has 1, 2, 4 or 8 channels (every norm of the two encoders); `table()` materialises [N, C, 2] scale / shift."""
+    a group has 1, 2, 4 or 8 channels (every norm of the two encoders); `table()` materialises [N, C, 3]
+    (scale, mean, beta): y = (x - mean) * scale + beta."""
 
     def __init__(self, raw, norm):
-        if raw.stats is None:
+        if raw.sums is None:
             raise _C.IconError("finalize: the producer of this activation accumulated no statistics")
         self.raw, self.norm = raw, norm
         self.groups = 0 if norm is None else norm.num_groups
@@ -125,8 +133,8 @@ class NormSpec:
 
     def table(self):
         raw = self.raw
-        ss = torch.empty(raw.N, raw.C, 2, dtype=torch.float32, device=raw.t.device)
-        check(lib.icon_norm_finalize(_p(raw.stats), _p(self.gamma), _p(self.beta), _p(ss), raw.N, raw.C, self.groups,
+        ss = torch.empty(raw.N, raw.C, 3, dtype=torch.float32, device=raw.t.device)
+        check(lib.icon_norm_finalize(_p(raw.sums), _p(self.gamma), _p(self.beta), _p(ss), raw.N, raw.C, self.groups,
                                      float(raw.H * raw.W), self.eps, _stream()), "icon_norm_finalize")
         return ss
 
@@ -137,7 +145,8 @@ def finalize(raw, norm=None):
 
 
 def act(raw, ss=None, relu=False, res=None, operand=True, halo=0, s2d=False, f32=False):
-    """y = [relu](x * scale + shift) [+ res] -> (Operand or None, fp32 NHWC tensor or None)."""
+    """y = [relu]((x - mean) * scale + beta) [+ res] -> (Operand or None, fp32 NHWC tensor or None); `ss` is a NormSpec,
+    a [N, C, 3] (scale, mean, beta) table or None (identity)."""
     dev = raw.t.device
     N, H, W, C = raw.N, raw.H, raw.W, raw.C
     Cp = _pad64(C)
@@ -160,7 +169,7 @@ def act(raw, ss=None, relu=False, res=None, operand=True, halo=0, s2d=False, f32
             raise _C.IconError("act: the NormSpec belongs to another activation")
         if ss.foldable() and N * H * W <= 64 * 64:
             # small activation: the pass is launch-bound, fold the statistics -> scale / shift step into it
-            stats, gamma, beta, groups, eps = raw.stats, ss.gamma, ss.beta, ss.groups, ss.eps
+            stats, gamma, beta, groups, eps = raw.sums, ss.gamma, ss.beta, ss.groups, ss.eps
         else:
             table = ss.table()
     else:
@@ -322,7 +331,7 @@ def conv(op, m, out=None, co_off=0, stats=True):
     st = new_stats(op.N, Cout, dev) if stats else None
     bias = m.bias.detach().float().contiguous() if m.bias is not None else None
     _launch(op, blob, ntap * cpt, bias, out, co_off, Cout, OH, OW, 1, 1, 0, 0, taps, cpt, n_tile, st)
-    return Raw(out, C=Cout, c_off=co_off, stats=st)
+    return Raw(out, C=Cout, c_off=co_off, sums=st)
 
 
 def conv_instnorm_act(op, m, relu=False, res=None, halo=0, f32=False):
@@ -410,7 +419,7 @@ def stem_conv7(x, m, reflect, stats=True):
     check(lib.icon_conv_nhwc(_p(hi), _p(lo), dims, strides, _p(blob), 7 * cpt, _p(bias), _p(out), OH, OW, Cout, 0, Cout, N,
                              OH, OW, 1, 1, 0, 0, s, 7, tap_arr, cpt, n_tile, 1, _p(st), None, 0, _stream()),
           "icon_conv_nhwc(stem)")
-    return Raw(out, stats=st)
+    return Raw(out, sums=st)
 
 
 def conv_transpose(op, m, stats=True):
@@ -442,7 +451,7 @@ def conv_transpose(op, m, stats=True):
                         continue
                     taps.append(((py + pad - kh) // 2, (px + pad - kw) // 2, 0, kh * KW + kw))
             _launch(op, blob, KH * KW * cpt, bias, out, 0, Cout, op.H, op.W, 2, 2, py, px, taps, cpt, n_tile, st)
-    return Raw(out, stats=st)
+    return Raw(out, sums=st)
 
 
 # ------------------------------------------------------------------------------------------------ elementwise
@@ -451,7 +460,7 @@ def _ew(mode, a, b, c, N, H, W, C, stats):
     y = torch.empty(N, H, W, C, dtype=torch.float32, device=dev)
     st = new_stats(N, C, dev) if stats else None
     check(lib.icon_ew_nhwc(mode, _p(a), _p(b), _p(c), _p(y), _p(st), N, H, W, C, _stream()), "icon_ew_nhwc")
-    return Raw(y, stats=st)
+    return Raw(y, sums=st)
 
 
 def add(a, b, c=None, stats=True):
@@ -474,7 +483,7 @@ def bicubic_up2_add(low, up, stats=True):
 
 
 def norm_relu(raw, ss, stats=True):
-    """relu(x * scale + shift) as fp32 NHWC WITH the statistics of the result: a normalisation whose output is read
+    """relu((x - mean) * scale + beta) as fp32 NHWC WITH the statistics of the result: a normalisation whose output is read
     by another normalisation (HGFilter: relu(bn1(conv1(x))) feeds conv2.bn1, HGFilters.py:162-164)."""
     return _ew(3, raw.dense(), ss.table() if isinstance(ss, NormSpec) else ss, None, raw.N, raw.H, raw.W, raw.C, stats)
 

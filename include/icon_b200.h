@@ -230,14 +230,18 @@ int icon_conv3d(const float *x, const float *w, const float *scale, const float 
  *   fp32 NHWC tensor with Cs channels (channel slices = concatenation for free; osy = 2 = one phase of a transposed
  *   convolution).  `taps`: ntaps x (dy, dx, plane, wtap) -- the A box of tap t is read at (y0 + dy, x0 + dx) of image
  *   n * nplanes + plane (out-of-range coordinates read zeros = zero padding).  stats (optional, zeroed by the
- *   caller): [N][Cout][2] doubles receive per-channel sum / sum of squares of the result (bias included).
- * icon_norm_finalize: stats -> [N][C] (scale, shift) for InstanceNorm2d (groups = 0) / GroupNorm(groups) with affine.
- * icon_act_nhwc: y = [relu](x * scale + shift) [+ res], scale / shift either from `scale_shift` or folded in from the
+ *   caller): [N][Cout][6] doubles receive per-channel sum / sum of squares of the result (bias included), each as
+ *   three words (sum = stats[0] + stats[1] + stats[2], sum of squares = stats[3] + stats[4] + stats[5]) so that the
+ *   atomic adds are exact and the result does not depend on block order.  icon_ew_nhwc and icon_nchw_to_nhwc write the
+ *   same.
+ * icon_norm_finalize: stats -> [N][C][3] (scale, mean, beta) for InstanceNorm2d (groups = 0) / GroupNorm(groups) with
+ *   affine; a consumer computes y = (x - mean) * scale + beta, so a constant channel gives exactly beta.
+ * icon_act_nhwc: y = [relu]((x - mean) * scale + beta) [+ res], from the `scale_shift` table or folded in from the
  *   producer's `stats` (+ GroupNorm gamma / beta, groups = 0: instance norm; 1, 2, 4 or 8 channels per group)
  *   -> hi / lo operand tensors (halo > 0: reflection halo;
  *   s2d = 1: four parity planes for a stride-2 consumer; channels padded to Cp with zeros) and / or fp32 NHWC.
- * icon_ew_nhwc: mode 0 a + b (+ c), 1 avg_pool2(a), 2 b + bicubic_up2(a, align_corners), 3 relu(a * scale + shift) with
- *   b = the [N][C] (scale, shift) table of icon_norm_finalize; optional stats of the result.
+ * icon_ew_nhwc: mode 0 a + b (+ c), 1 avg_pool2(a), 2 b + bicubic_up2(a, align_corners), 3 relu((a - mean) * scale + beta)
+ *   with b = the [N][C][3] table of icon_norm_finalize; optional stats of the result.
  * icon_nchw_to_nhwc / icon_nhwc_to_nchw: layout adaptors (the former with optional stats). */
 size_t icon_conv_nhwc_workspace_bytes(int N, int Ht, int Wt, int Cout, int splits);
 int icon_conv_nhwc(const void *a_hi, const void *a_lo, const int64_t *dims, const int64_t *strides, const void *wt_packed,
