@@ -47,8 +47,8 @@ _SIGS = {
     "icon_grid_init_points": (_i, [_i, _i, _vp, _vp, _vp, _vp]),
     "icon_grid_count_above": (_i, [_vp, _i64, _f, _vp, _vp]),
     "icon_conv_nhwc_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
-    "icon_conv_nhwc": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i,
-                           _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "icon_conv_nhwc": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i,
+                           _i, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
     "icon_norm_finalize": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, ctypes.c_double, _f, _vp]),
     "icon_act_nhwc": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _i, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "icon_splitk_instnorm_act": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _vp]),

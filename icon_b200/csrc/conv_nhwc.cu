@@ -35,6 +35,7 @@ constexpr int MAX_TAPS = 49;
 
 struct ConvNhwcParams {
     const uint8_t *wt;       // [n tiles][wt_chunks] x (hi NT*128 B | lo NT*128 B)
+    const float *wt_scale;   // [Cout] powers of two the packed weight rows were multiplied by the inverse of, or null (1)
     const float *bias;       // [Cout] or null
     float *out;              // fp32 NHWC [N][OHf][OWf][Cs], this conv writes channels [co_off, co_off + Cout)
     float *partial;          // splits > 1: [splits][N][Ht][Wt][Cout]
@@ -107,6 +108,11 @@ k_conv_nhwc(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ 
 
     // ---------------------------------------------------------------- consumers: mainloop
     const int g = warp >> 2;
+    const int col = tid % NT, co = blockIdx.y * NT + col;     // this thread's channel in the epilogue
+    // the weight row was packed as w * 2^e (nhwc.pack_tiles) so that its fp16 lo half stays normal; the epilogue undoes
+    // it exactly with 2^-e, for every path: direct store, split-K partials (the finish adds the bias), stem, 7x7 head
+    // GEMM.  Loaded here so that its latency hides behind the main loop.
+    const float wsc = (p.wt_scale && co < p.Cout) ? __ldg(p.wt_scale + co) : 1.f;
     float acc[NT / 2];
 #pragma unroll
     for (int i = 0; i < NT / 2; ++i) acc[i] = 0.f;
@@ -150,9 +156,8 @@ k_conv_nhwc(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ 
         }
     }
     bar_sync(1, 256);
-    const int col = tid % NT, row0 = tid / NT;
+    const int row0 = tid / NT;
     constexpr int RSTEP = 256 / NT;
-    const int co = blockIdx.y * NT + col;
     if (co >= p.Cout) return;
     const bool fin = p.splits == 1;
     const int bw_shift = 31 - __clz(p.BW), bw_mask = p.BW - 1;
@@ -162,7 +167,7 @@ k_conv_nhwc(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ 
     for (int row = row0; row < 128; row += RSTEP) {
         const int a = y0 + (row >> bw_shift), b = x0 + (row & bw_mask);
         if (a >= p.Ht || b >= p.Wt) continue;
-        const float val = tile[row * LD + col] + bias;
+        const float val = tile[row * LD + col] * wsc + bias;
         if (fin) {
             p.out[(((size_t)n * p.OHf + (size_t)(a * p.osy + p.ooy)) * p.OWf + (size_t)(b * p.osx + p.oox)) * p.Cs + p.co_off + co] = val;
             s1 += val; s2 = fma((double)val, (double)val, s2);
@@ -276,8 +281,8 @@ extern "C" size_t icon_conv_nhwc_workspace_bytes(int N, int Ht, int Wt, int Cout
 }
 
 extern "C" int icon_conv_nhwc(const void *a_hi, const void *a_lo, const int64_t *dims, const int64_t *strides,
-                              const void *wt_packed, int wt_chunks, const float *bias, float *out, int OHf, int OWf, int Cs,
-                              int co_off, int Cout, int N, int Ht, int Wt, int osy, int osx, int ooy, int oox, int nplanes,
+                              const void *wt_packed, int wt_chunks, const float *wt_scale, const float *bias, float *out,
+                              int OHf, int OWf, int Cs, int co_off, int Cout, int N, int Ht, int Wt, int osy, int osx, int ooy, int oox, int nplanes,
                               int ntaps, const int *taps /* ntaps x (dy, dx, plane, wtap) */, int cpt, int n_tile, int splits,
                               double *stats, void *ws, size_t ws_bytes, icon_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -292,7 +297,8 @@ extern "C" int icon_conv_nhwc(const void *a_hi, const void *a_lo, const int64_t 
                    "icon_conv_nhwc: tensor-map strides must be multiples of 16 bytes");
     ICON_CHECK_ARG(co_off >= 0 && co_off + Cout <= Cs, "icon_conv_nhwc: channel slice outside the output tensor");
     ConvNhwcParams p{};
-    p.wt = (const uint8_t *)wt_packed; p.bias = bias; p.out = out; p.stats = splits == 1 ? stats : nullptr;
+    p.wt = (const uint8_t *)wt_packed; p.wt_scale = wt_scale; p.bias = bias; p.out = out;
+    p.stats = splits == 1 ? stats : nullptr;
     p.N = N; p.Ht = Ht; p.Wt = Wt;
     int bw = 1;
     while (bw < Wt && bw < 16) bw <<= 1;                       // 8 x 16 pixel tiles (taps of neighbouring tiles overlap

@@ -187,9 +187,9 @@ def _n_tile(cout):
 
 
 def _cached_blob(m, variant, build):
-    """Packed-weight blob of module `m` for `variant` (a tuple), made by `build()` on a miss.  Cached ON the module (the
-    blob must live as long as any CUDA graph that captured its address), keyed on the weight's storage address, version
-    and device: when the weights change, this module's stale blobs are dropped."""
+    """Packed weights (blob, row factors) of module `m` for `variant` (a tuple), made by `build()` on a miss.  Cached ON
+    the module (both tensors must live as long as any CUDA graph that captured their addresses), keyed on the weight's
+    storage address, version and device: when the weights change, this module's stale blobs are dropped."""
     w = m.weight
     key = (w.data_ptr(), w._version, str(w.device)) + variant
     cache = m.__dict__.setdefault("_icon_pack", {})
@@ -203,7 +203,8 @@ def _cached_blob(m, variant, build):
 
 
 def packed_weight(conv, transposed, cin_pad, n_tile):
-    """torch conv weight -> device blob of K-major SWIZZLE_128B fp16 hi / lo tiles, chunk = (tap, 64-channel block)."""
+    """torch conv weight -> (device blob of K-major SWIZZLE_128B fp16 hi / lo tiles, chunk = (tap, 64-channel block),
+    per output channel factors): pack_tiles."""
     def build():
         wd = conv.weight.detach().float()
         if transposed:                               # [Cin, Cout, KH, KW] -> [Cout, taps, Cin]
@@ -218,13 +219,24 @@ def packed_weight(conv, transposed, cin_pad, n_tile):
 
 
 def pack_tiles(w2, n_tile):
-    """[Cout, K] fp32 (K % 64 == 0) -> uint8 blob [n tiles][K / 64][hi | lo][n_tile rows][128 B swizzled]."""
+    """[Cout, K] fp32 (K % 64 == 0) -> (uint8 blob [n tiles][K / 64][hi | lo][n_tile rows][128 B swizzled],
+    fp32 [n tiles * n_tile] row factors 2^-e).
+
+    Row r is stored as hi + lo = w * 2^e, with e chosen so that max|w_r| * 2^e lies in [2^14, 2^15) (all-zero rows:
+    e = 0), and the conv epilogue multiplies the row's result by 2^-e, which is exact.  Without the exponent, lo of a
+    weight under 2^-3 is an fp16 subnormal and the pair has a fixed absolute error of up to 2^-25, so small weight rows
+    (xavier 0.02: |w| ~ 1e-4) lose most of their significant bits; with it a weight keeps 22 significant bits down to
+    2^-17 of its row's maximum, and the absolute error of smaller ones is at most 2^-39 of that maximum."""
     cout, K = w2.shape
     ntl = (cout + n_tile - 1) // n_tile
+    w2 = w2.float()
     if ntl * n_tile != cout:
         w2 = torch.cat([w2, torch.zeros(ntl * n_tile - cout, K, device=w2.device)], 0)
-    hi = w2.half()
-    lo = (w2 - hi.float()).half()
+    amax = w2.abs().amax(1)
+    e = torch.where(amax > 0, 15 - torch.frexp(amax).exponent, 0).clamp(max=126)   # amax = m * 2^E, m in [0.5, 1)
+    ws = torch.ldexp(w2, e[:, None].float())
+    hi = ws.half()
+    lo = (ws - hi.float()).half()
     nch = K // 64
     r = torch.arange(n_tile, device=w2.device)
     cpos = torch.arange(8, device=w2.device)
@@ -235,7 +247,8 @@ def pack_tiles(w2, n_tile):
         t = m.view(ntl, n_tile, nch, 8, 8)                               # [tile, row, chunk, c16, elem]
         return t.gather(3, index).permute(0, 2, 1, 3, 4)                 # -> [tile, chunk, row, c16', elem]
 
-    return torch.stack([tiles(hi), tiles(lo)], dim=2).contiguous().view(torch.uint8).reshape(-1)
+    blob = torch.stack([tiles(hi), tiles(lo)], dim=2).contiguous().view(torch.uint8).reshape(-1)
+    return blob, torch.ldexp(torch.ones_like(amax), -e.float())
 
 
 def invalidate_packed(module):
@@ -259,7 +272,8 @@ def _splits(n_pix_tiles, n_ch_tiles, chunks):
     return max(1, min(16, sms // items, chunks))
 
 
-def _launch(op, blob, wt_chunks, bias, out, co_off, Cout, Ht, Wt, osy, osx, ooy, oox, taps, cpt, n_tile, stats):
+def _launch(op, packed, wt_chunks, bias, out, co_off, Cout, Ht, Wt, osy, osx, ooy, oox, taps, cpt, n_tile, stats):
+    blob, wscale = packed
     dev = out.device
     N = op.N
     nplanes = 4 if op.s2d else 1
@@ -279,9 +293,9 @@ def _launch(op, blob, wt_chunks, bias, out, co_off, Cout, Ht, Wt, osy, osx, ooy,
     nbytes = lib.icon_conv_nhwc_workspace_bytes(N, Ht, Wt, Cout, splits)
     ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
     OHf, OWf, Cs = out.shape[1], out.shape[2], out.shape[3]
-    check(lib.icon_conv_nhwc(_p(op.hi), _p(op.lo), dims, strides, _p(blob), wt_chunks, _p(bias), _p(out), OHf, OWf, Cs,
-                             co_off, Cout, N, Ht, Wt, osy, osx, ooy, oox, nplanes, len(taps), tap_arr, cpt, n_tile, splits,
-                             _p(stats), _p(ws), nbytes, _stream()), "icon_conv_nhwc")
+    check(lib.icon_conv_nhwc(_p(op.hi), _p(op.lo), dims, strides, _p(blob), wt_chunks, _p(wscale), _p(bias), _p(out), OHf,
+                             OWf, Cs, co_off, Cout, N, Ht, Wt, osy, osx, ooy, oox, nplanes, len(taps), tap_arr, cpt, n_tile,
+                             splits, _p(stats), _p(ws), nbytes, _stream()), "icon_conv_nhwc")
 
 
 def _conv_taps(op, m):
@@ -324,13 +338,13 @@ def conv(op, m, out=None, co_off=0, stats=True):
     Cout = m.weight.shape[0]
     cpt = op.Cp // 64
     n_tile = _n_tile(Cout)
-    blob = packed_weight(m, False, op.Cp, n_tile)
+    packed = packed_weight(m, False, op.Cp, n_tile)
     dev = op.hi.device
     if out is None:
         out = torch.empty(op.N, OH, OW, Cout, dtype=torch.float32, device=dev)
     st = new_stats(op.N, Cout, dev) if stats else None
     bias = m.bias.detach().float().contiguous() if m.bias is not None else None
-    _launch(op, blob, ntap * cpt, bias, out, co_off, Cout, OH, OW, 1, 1, 0, 0, taps, cpt, n_tile, st)
+    _launch(op, packed, ntap * cpt, bias, out, co_off, Cout, OH, OW, 1, 1, 0, 0, taps, cpt, n_tile, st)
     return Raw(out, C=Cout, c_off=co_off, sums=st)
 
 
@@ -355,7 +369,7 @@ def conv_instnorm_act(op, m, relu=False, res=None, halo=0, f32=False):
     if splits == 1 or Cout % 64 or OH * OW * 32 > 200 * 1024:
         r = conv(op, m)
         return act(r, finalize(r), relu=relu, res=res, halo=halo, f32=f32)
-    blob = packed_weight(m, False, op.Cp, n_tile)
+    blob, wscale = packed_weight(m, False, op.Cp, n_tile)
     nbytes = lib.icon_conv_nhwc_workspace_bytes(N, OH, OW, Cout, splits)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     NI, Hd, Wd, Cp = op.hi.shape
@@ -363,9 +377,9 @@ def conv_instnorm_act(op, m, relu=False, res=None, halo=0, f32=False):
     strides = (ctypes.c_int64 * 3)(Cp, Wd * Cp, Hd * Wd * Cp)
     flat = [int(v) for t in taps for v in t]
     tap_arr = (ctypes.c_int * len(flat))(*flat)
-    check(lib.icon_conv_nhwc(_p(op.hi), _p(op.lo), dims, strides, _p(blob), ntap * cpt, None, None, OH, OW, Cout, 0, Cout, N,
-                             OH, OW, 1, 1, 0, 0, 4 if op.s2d else 1, len(taps), tap_arr, cpt, n_tile, splits, None, _p(ws),
-                             nbytes, _stream()), "icon_conv_nhwc(park)")
+    check(lib.icon_conv_nhwc(_p(op.hi), _p(op.lo), dims, strides, _p(blob), ntap * cpt, _p(wscale), None, None, OH, OW, Cout,
+                             0, Cout, N, OH, OW, 1, 1, 0, 0, 4 if op.s2d else 1, len(taps), tap_arr, cpt, n_tile, splits,
+                             None, _p(ws), nbytes, _stream()), "icon_conv_nhwc(park)")
     hi = torch.empty(N, OH + 2 * halo, OW + 2 * halo, Cout, dtype=torch.float16, device=dev)
     lo = torch.empty_like(hi)
     out = torch.empty(N, OH, OW, Cout, dtype=torch.float32, device=dev) if f32 else None
@@ -402,12 +416,7 @@ def stem_conv7(x, m, reflect, stats=True):
           "icon_stem_pack")
     cpt = Cp8 // 8                                              # 64-wide chunks per tap row
     n_tile = _n_tile(Cout)
-
-    def build():
-        wk = torch.zeros(Cout, 7, 8, Cp8, dtype=torch.float32, device=w.device)      # [co][ky][kx (8th = 0)][c]
-        wk[:, :, :7, :Cin] = w.detach().float().permute(0, 2, 3, 1)
-        return pack_tiles(wk.reshape(Cout, 7 * 8 * Cp8), n_tile)
-    blob = _cached_blob(m, ("stem", Cp8, n_tile), build)
+    blob, wscale = _cached_blob(m, ("stem", Cp8, n_tile), lambda: pack_tiles(stem_weight_rows(w, Cp8), n_tile))
     out = torch.empty(N, OH, OW, Cout, dtype=torch.float32, device=dev)
     st = new_stats(N, Cout, dev) if stats else None
     bias = m.bias.detach().float().contiguous() if m.bias is not None else None
@@ -416,10 +425,26 @@ def stem_conv7(x, m, reflect, stats=True):
     strides = (ctypes.c_int64 * 3)(s * Cp8, Wp * Cp8, Hrows * Wp * Cp8)
     flat = [int(v) for t in taps for v in t]
     tap_arr = (ctypes.c_int * len(flat))(*flat)
-    check(lib.icon_conv_nhwc(_p(hi), _p(lo), dims, strides, _p(blob), 7 * cpt, _p(bias), _p(out), OH, OW, Cout, 0, Cout, N,
-                             OH, OW, 1, 1, 0, 0, s, 7, tap_arr, cpt, n_tile, 1, _p(st), None, 0, _stream()),
+    check(lib.icon_conv_nhwc(_p(hi), _p(lo), dims, strides, _p(blob), 7 * cpt, _p(wscale), _p(bias), _p(out), OH, OW, Cout,
+                             0, Cout, N, OH, OW, 1, 1, 0, 0, s, 7, tap_arr, cpt, n_tile, 1, _p(st), None, 0, _stream()),
           "icon_conv_nhwc(stem)")
     return Raw(out, sums=st)
+
+
+def stem_weight_rows(w, Cp8):
+    """7 x 7 stem weight [Cout, Cin, 7, 7] -> [Cout, 7 * 8 * Cp8] GEMM rows: [co][ky][kx (8th = 0)][c (padded to Cp8)]."""
+    Cout, Cin = w.shape[:2]
+    wk = torch.zeros(Cout, 7, 8, Cp8, dtype=torch.float32, device=w.device)
+    wk[:, :, :7, :Cin] = w.detach().float().permute(0, 2, 3, 1)
+    return wk.reshape(Cout, 7 * 8 * Cp8)
+
+
+def head_weight_rows(w, Cp):
+    """7 x 7 head weight [Cout, Cin, 7, 7] -> [49 * Cout, Cp] rows of the 1 x 1 GEMM: row (ky * 7 + kx) * Cout + co."""
+    Cout, Cin = w.shape[:2]
+    w2 = torch.zeros(49 * Cout, Cp, dtype=torch.float32, device=w.device)
+    w2[:, :Cin] = w.detach().float().permute(2, 3, 0, 1).reshape(49 * Cout, Cin)
+    return w2
 
 
 def conv_transpose(op, m, stats=True):
@@ -435,7 +460,7 @@ def conv_transpose(op, m, stats=True):
         raise NotImplementedError("conv_transpose: output must be exactly 2x (k3 s2 p1 op1)")
     cpt = op.Cp // 64
     n_tile = _n_tile(Cout)
-    blob = packed_weight(m, True, op.Cp, n_tile)
+    packed = packed_weight(m, True, op.Cp, n_tile)
     dev = op.hi.device
     out = torch.empty(op.N, OH, OW, Cout, dtype=torch.float32, device=dev)
     st = new_stats(op.N, Cout, dev) if stats else None
@@ -450,7 +475,7 @@ def conv_transpose(op, m, stats=True):
                     if (px + pad - kw) % 2:
                         continue
                     taps.append(((py + pad - kh) // 2, (px + pad - kw) // 2, 0, kh * KW + kw))
-            _launch(op, blob, KH * KW * cpt, bias, out, 0, Cout, op.H, op.W, 2, 2, py, px, taps, cpt, n_tile, st)
+            _launch(op, packed, KH * KW * cpt, bias, out, 0, Cout, op.H, op.W, 2, 2, py, px, taps, cpt, n_tile, st)
     return Raw(out, sums=st)
 
 
@@ -500,15 +525,10 @@ def conv7_head(op, m, tanh):
     dev = op.hi.device
     ncol = 49 * Cout
     n_tile = _n_tile(ncol)
-
-    def build():
-        w2 = torch.zeros(ncol, op.Cp, dtype=torch.float32, device=w.device)          # row (ky*7+kx)*Cout + co
-        w2[:, :Cin] = w.detach().float().permute(2, 3, 0, 1).reshape(ncol, Cin)
-        return pack_tiles(w2, n_tile)
-    blob = _cached_blob(m, ("head", op.Cp, n_tile), build)
+    packed = _cached_blob(m, ("head", op.Cp, n_tile), lambda: pack_tiles(head_weight_rows(w, op.Cp), n_tile))
     Ps = (ncol + 3) // 4 * 4
     P = torch.empty(op.N, op.H, op.W, Ps, dtype=torch.float32, device=dev)
-    _launch(op, blob, op.Cp // 64, None, P, 0, ncol, op.H, op.W, 1, 1, 0, 0, [(0, 0, 0, 0)], op.Cp // 64, n_tile, None)
+    _launch(op, packed, op.Cp // 64, None, P, 0, ncol, op.H, op.W, 1, 1, 0, 0, [(0, 0, 0, 0)], op.Cp // 64, n_tile, None)
     y = torch.empty(op.N, Cout, op.H, op.W, dtype=torch.float32, device=dev)
     b = m.bias.detach().float().contiguous() if m.bias is not None else None
     check(lib.icon_col2im7(_p(P), _p(b), _p(y), op.N, op.H, op.W, Cout, Ps, 2 if tanh else 0, _stream()), "icon_col2im7")

@@ -225,7 +225,9 @@ int icon_conv3d(const float *x, const float *w, const float *scale, const float 
  * icon_conv_nhwc: implicit-GEMM convolution on wgmma, A operand staged by 4-D tiled TMA loads straight from the
  *   hi / lo tensors (`dims` = tensor-map extents innermost first, `strides` = element strides of dims 1..3), weights
  *   from `wt_packed` (per n_tile output channels and per chunk a K-major SWIZZLE_128B fp16 hi tile followed by the lo
- *   tile; `wt_chunks` chunks per tile, chunk index = wtap * cpt + channel block).  The launch covers a logical
+ *   tile; `wt_chunks` chunks per tile, chunk index = wtap * cpt + channel block).  `wt_scale` (optional, NULL = 1):
+ *   per output channel factor 2^-e applied to the products before the bias, for rows packed as w * 2^e so that the
+ *   fp16 lo half stays a normal number (icon_b200/nhwc.py pack_tiles).  The launch covers a logical
  *   Ht x Wt grid per image; output pixel (a, b) is written to out[n][a * osy + ooy][b * osx + oox][co_off + co] of an
  *   fp32 NHWC tensor with Cs channels (channel slices = concatenation for free; osy = 2 = one phase of a transposed
  *   convolution).  `taps`: ntaps x (dy, dx, plane, wtap) -- the A box of tap t is read at (y0 + dy, x0 + dx) of image
@@ -245,7 +247,8 @@ int icon_conv3d(const float *x, const float *w, const float *scale, const float 
  * icon_nchw_to_nhwc / icon_nhwc_to_nchw: layout adaptors (the former with optional stats). */
 size_t icon_conv_nhwc_workspace_bytes(int N, int Ht, int Wt, int Cout, int splits);
 int icon_conv_nhwc(const void *a_hi, const void *a_lo, const int64_t *dims, const int64_t *strides, const void *wt_packed,
-                   int wt_chunks, const float *bias, float *out, int OHf, int OWf, int Cs, int co_off, int Cout, int N,
+                   int wt_chunks, const float *wt_scale, const float *bias, float *out, int OHf, int OWf, int Cs, int co_off,
+                   int Cout, int N,
                    int Ht, int Wt, int osy, int osx, int ooy, int oox, int nplanes, int ntaps, const int *taps, int cpt,
                    int n_tile, int splits, double *stats, void *ws, size_t ws_bytes, icon_stream_t stream);
 int icon_norm_finalize(const double *stats, const float *gamma, const float *beta, float *scale_shift, int N, int C,

@@ -28,6 +28,12 @@ def test_library_exports_every_declared_symbol(built_lib):
         assert hasattr(lib, name), f"{name} declared in include/icon_b200.h but not exported"
     from icon_b200 import _C
     assert set(_C.EXPORTS) == declared          # the ctypes table covers the whole header
+    # ... with the header's parameter count: an argument added on one side only would shift every later one
+    decls = re.findall(r"\b(icon_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", hdr)
+    assert {n for n, _ in decls} == declared
+    for name, params in decls:
+        count = 0 if params.strip() in ("", "void") else params.count(",") + 1
+        assert len(getattr(_C.lib, name).argtypes) == count, name
     assert _C.lib.icon_version() == 1
     # size queries are host-only and must work without a GPU
     assert _C.lib.icon_smpl_workspace_bytes(6890, 13776) > 13776 * 64
@@ -177,6 +183,163 @@ def _check_tc_blob_emulation(c0, inputs):
         assert err.max() < 2e-5                                  # fp16 hi + lo operands: 22 significant bits
     if inputs == "wide_range":
         assert (acts[0][0, :, -n // 4:] < 0).double().mean() > 0.9      # the negative LeakyReLU branch is exercised
+
+
+# ------------------------------------------------------------------------------------------------ encoder conv weights
+WEIGHT_KINDS = ("fan_in", "init_net", "rows", "outlier")
+
+
+def _conv_weights(m, kind, seed):
+    """Weights of nn.Conv2d / nn.ConvTranspose2d `m` (a row = one output channel):
+    fan_in    N(0, 1/fan_in) (synthetic.seeded_like, nn.Conv2d defaults);
+    init_net  icon_b200.net.init_net: xavier-normal, gain 0.02 (std 2e-4 for a 1024 -> 1024 3x3 conv), zero bias;
+    rows      fan_in rows scaled log-uniformly over 1e-6 ... 10, one row all zero;
+    outlier   one weight per row of magnitude 1e-3 ... 1, the others 1e-4 of it."""
+    from icon_b200.net import init_net
+    if kind == "init_net":
+        torch.manual_seed(seed)
+        return init_net(m)
+    w = m.weight.detach()
+    rows = w.transpose(0, 1) if isinstance(m, torch.nn.ConvTranspose2d) else w
+    cout, fan = rows.shape[0], rows[0].numel()
+    g = torch.Generator().manual_seed(seed)
+    r = torch.randn(rows.shape, generator=g) / fan ** 0.5
+    if kind == "rows":
+        r *= (10.0 ** (-6 + 7 * torch.rand(cout, generator=g)))[:, None, None, None]
+        r[cout // 2] = 0.0
+    elif kind == "outlier":
+        big = torch.where(torch.rand(cout, generator=g) < 0.5, -1.0, 1.0) * 10.0 ** (-3 * torch.rand(cout, generator=g))
+        flat = 1e-4 * big[:, None] * torch.randn(cout, fan, generator=g)
+        flat[torch.arange(cout), torch.randint(fan, (cout,), generator=g)] = big
+        r = flat.view(rows.shape)
+    elif kind != "fan_in":
+        raise ValueError(kind)
+    with torch.no_grad():
+        rows.copy_(r)
+    return m
+
+
+def _decode_conv_blob(packed, n_rows, K, n_tile):
+    """Inverse of nhwc.pack_tiles: (blob, row factors) -> hi, lo [padded rows, K] and the factors, as float64."""
+    import numpy as np
+    blob, scale = packed
+    buf = blob.cpu().numpy().tobytes()
+    ntl, nb = -(-n_rows // n_tile), n_tile * 128
+    assert len(buf) == ntl * (K // 64) * 2 * nb
+    assert scale.dtype == torch.float32 and tuple(scale.shape) == (ntl * n_tile,)
+    hi, lo = np.zeros((ntl * n_tile, K)), np.zeros((ntl * n_tile, K))
+    o = 0
+    for t in range(ntl):
+        for c in range(K // 64):
+            for part in (hi, lo):                                # [tile][chunk][hi | lo][n_tile rows][128 B]
+                part[t * n_tile:(t + 1) * n_tile, 64 * c:64 * c + 64] = _unswizzle128(buf[o:o + nb], n_tile)
+                o += nb
+    return hi, lo, scale.cpu().double().numpy()
+
+
+def _check_decoded_rows(hi, lo, sc, ref):
+    """ref [rows, K]: the weights in the kernel's row layout (zero padding included), float64."""
+    import numpy as np
+    R = ref.shape[0]
+    assert (hi[R:] == 0).all() and (lo[R:] == 0).all() and (sc[R:] == 1).all()      # padded rows of the last tile
+    assert (np.frexp(sc)[0] == 0.5).all()                                            # powers of two
+    amax, hmax = np.abs(ref).max(1), np.abs(hi[:R]).max(1)
+    nz = amax > 0
+    assert (sc[:R][~nz] == 1).all() and (hmax[nz] >= 2.0 ** 14).all() and (hmax[nz] <= 2.0 ** 15).all()
+    err = np.abs((hi[:R] + lo[:R]) * sc[:R, None] - ref)
+    # 22 significant bits, and half the fp16 subnormal spacing 2^-24 over the row's 2^14 scale
+    bar = 2.0 ** -22 * np.abs(ref) + 2.0 ** -39 * amax[:, None]
+    assert (err <= bar).all(), (err / np.maximum(bar, 1e-300)).max()
+
+
+PACKERS = [("conv", 3, 6), ("conv", 48, 96), ("conv", 192, 200), ("conv", 48, 147), ("transposed", 48, 96),
+           ("transposed", 3, 147), ("stem", 3, 64), ("stem", 9, 64), ("head", 64, 1), ("head", 64, 2), ("head", 48, 3)]
+
+
+@pytest.mark.parametrize("kind", WEIGHT_KINDS)
+@pytest.mark.parametrize("packer,cin,cout", PACKERS)
+def test_conv_weight_blob_round_trip(built_lib, packer, cin, cout, kind):
+    """Decode every packer's tiles (packed_weight plain and transposed, the 7x7 stem's rows, the 7x7 head's 49-tap rows):
+    Cout with a remainder in its last N tile (n_tile 64 / 128 / 256), Cin padded to 64, the 128-byte swizzle, and the
+    per-row exponent, which keeps 22 significant bits at any weight scale."""
+    import numpy as np
+    from icon_b200 import nhwc as T
+    seed = cin * 1000 + cout
+    if packer == "transposed":
+        m = _conv_weights(torch.nn.ConvTranspose2d(cin, cout, 3, stride=2, padding=1, output_padding=1), kind, seed)
+        w = m.weight.detach().double().numpy().transpose(1, 0, 2, 3)           # [Cout, Cin, kh, kw]
+    else:
+        k = 3 if packer == "conv" else 7
+        m = _conv_weights(torch.nn.Conv2d(cin, cout, k), kind, seed)
+        w = m.weight.detach().double().numpy()
+    if packer in ("conv", "transposed"):                      # row co, column (ky * 3 + kx) * Cp + ci
+        Cp = -(-cin // 64) * 64
+        ref = np.zeros((cout, 3, 3, Cp))
+        ref[..., :cin] = w.transpose(0, 2, 3, 1)
+        ref = ref.reshape(cout, -1)
+        n_tile = T._n_tile(cout)
+        packed = T.packed_weight(m, packer == "transposed", Cp, n_tile)
+    elif packer == "stem":                                    # row co, column (ky * 8 + kx) * Cp8 + ci, kx = 7 is zero
+        Cp8 = 8 if cin <= 8 else 16
+        ref = np.zeros((cout, 7, 8, Cp8))
+        ref[:, :, :7, :cin] = w.transpose(0, 2, 3, 1)
+        ref = ref.reshape(cout, -1)
+        n_tile = T._n_tile(cout)
+        packed = T.pack_tiles(T.stem_weight_rows(m.weight, Cp8), n_tile)
+    else:                                                     # row (ky * 7 + kx) * Cout + co, column ci
+        ref = np.zeros((49 * cout, 64))
+        ref[:, :cin] = w.transpose(2, 3, 0, 1).reshape(49 * cout, cin)
+        n_tile = T._n_tile(49 * cout)
+        packed = T.pack_tiles(T.head_weight_rows(m.weight, 64), n_tile)
+    _check_decoded_rows(*_decode_conv_blob(packed, ref.shape[0], ref.shape[1], n_tile), ref)
+
+
+def _conv_bar(x, w, ref):
+    """Per-element bar of a convolution of x (float64, the decoded operand) with w: 2^-19 sum |w| |x| + 2^-24 |ref|."""
+    F = torch.nn.functional
+    return 2.0 ** -19 * F.conv2d(x.abs(), w.abs(), padding=1) + 2.0 ** -24 * ref.abs()
+
+
+def _emulated_conv_ratio(kind, scaled):
+    """One 512 -> 128 3x3 conv evaluated the way k_conv_nhwc does: activations split into fp16 hi + lo, weights decoded
+    from the blob (scaled: the per-row exponent of pack_tiles; otherwise the plain split hi = fp16(w), lo = fp16(w - hi)),
+    hi*Whi + hi*Wlo + lo*Whi in float64.  Returns max |y - ref| / bar against the float64 conv of x = hi + lo."""
+    import numpy as np
+    from icon_b200 import nhwc as T
+    F = torch.nn.functional
+    cin, cout, hw = 512, 128, 12
+    m = _conv_weights(torch.nn.Conv2d(cin, cout, 3, padding=1, bias=False), kind, seed=5)
+    x = torch.randn(1, cin, hw, hw, generator=torch.Generator().manual_seed(6))
+    xh, xl = (torch.from_numpy(v) for v in _split_hi_lo(x.numpy()))
+    if scaled:
+        hi, lo, sc = _decode_conv_blob(T.packed_weight(m, False, cin, T._n_tile(cout)), cout, 9 * cin, T._n_tile(cout))
+        Wh, Wl = (torch.from_numpy((v[:cout] * sc[:cout, None]).reshape(cout, 3, 3, cin)).permute(0, 3, 1, 2)
+                  for v in (hi, lo))
+    else:
+        Wh, Wl = (torch.from_numpy(v) for v in _split_hi_lo(m.weight.detach().numpy()))
+    y = F.conv2d(xh, Wh, padding=1) + F.conv2d(xh, Wl, padding=1) + F.conv2d(xl, Wh, padding=1)
+    w = m.weight.detach().double()
+    ref = F.conv2d(xh + xl, w, padding=1)
+    assert np.isfinite(y.numpy()).all()
+    return ((y - ref).abs() / _conv_bar(xh + xl, w, ref).clamp(min=1e-300)).max().item()     # all-zero rows: 0 / 0
+
+
+@pytest.mark.parametrize("kind", WEIGHT_KINDS)
+def test_conv_blob_emulation_meets_the_fp64_bar(built_lib, kind):
+    """The conv bar of tests/test_gpu_conv_fp64.py holds for the kernel's operand arithmetic at every weight scale.  Per
+    product, the weight pair is off by <= 2^-22 |w| and the dropped lo*Wlo term is <= 2^-22 |w| |x|: a quarter of the
+    bar at most, which a row dominated by one weight (outlier) approaches; the rest is left to the fp32 accumulation."""
+    r = _emulated_conv_ratio(kind, scaled=True)
+    print(f"{kind}: err/bar {r:.3f}")
+    assert r <= 0.25
+
+
+def test_unscaled_weight_split_fails_the_bar_at_init_net_scale(built_lib):
+    """Without the row exponent, the lo half of an init_net weight (|w| ~ 4e-4) is an fp16 subnormal: the bar must
+    catch that, or it would not catch the packing losing its precision again."""
+    r = _emulated_conv_ratio("init_net", scaled=False)
+    print(f"init_net unscaled: err/bar {r:.2f}")
+    assert r > 2.0
 
 
 def test_pack_mlp_refuses_16_input_channels(built_lib):
