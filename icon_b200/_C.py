@@ -32,6 +32,8 @@ _SIGS = {
     "icon_get_mlp_impl": (_i, []),
     "icon_query": (_i, [_i, _vp, _i64, _i64, _i64, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _i, _f,
                         _vp, _vp, _sz, _vp]),
+    "icon_query_feats": (_i, [_i, _vp, _i64, _i64, _i64, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _i, _f,
+                              _i, _vp, _vp, _sz, _vp]),
     "icon_set_sdf_policy": (_i, [_i, _i64, _i64]),
     "icon_set_sdf_bricks": (_i, [_i, _i64]),
     "icon_sdf_brick_info": (_i, [_vp, _i, _i, _vp]),

@@ -5,7 +5,8 @@ The reference reads a yacs CfgNode (`lib/common/config.py:21-162` defaults merge
 dict that is enough for the keys the hot path reads, and any object with the same
 attributes (a real yacs node included) can be passed to HGPIFuNet / NormalNet instead.
 `preset(name)` restates the four inference YAMLs named by BASELINE.json
-(configs/icon-filter.yaml, icon-nofilter.yaml, pamir.yaml, pifu.yaml).
+(configs/icon-filter.yaml, icon-nofilter.yaml, pamir.yaml, pifu.yaml) and the ICON-MVP prior
+(configs/train/icon-mvp.yaml with the test_mode that `apps/train.py -test` forces).
 """
 import copy
 
@@ -66,6 +67,11 @@ _PRESETS = {
     "icon-nofilter": {"net": dict(_COMMON_NET, prior_type="icon", use_filter=False,
                                   in_geo=(("normal_F", 3), ("normal_B", 3)),
                                   smpl_feats=["sdf", "norm", "vis", "cmap"], hourglass_dim=6, smpl_dim=7)},
+    # configs/train/icon-mvp.yaml, the paper's ICON-MVP prior (SMPL sdf only, no filter), evaluated as `-test` runs it
+    "icon-mvp": {"net": dict(_COMMON_NET, prior_type="icon", use_filter=False,
+                             in_geo=(("normal_F", 3), ("normal_B", 3)), smpl_feats=["sdf"], ctype="resnet34",
+                             N_freqs=10, geo_w=0.1, norm_w=0.001, dc_w=1.0, hourglass_dim=6, voxel_dim=32, smpl_dim=1),
+                 "sdf_clip": 15.0, "test_mode": True},
     "pamir": {"net": dict(_COMMON_NET, prior_type="pamir", use_filter=True,
                           in_geo=(("image", 3), ("normal_F", 3), ("normal_B", 3)), hourglass_dim=6, voxel_dim=7)},
     "pifu": {"net": dict(_COMMON_NET, prior_type="pifu", use_filter=True,

@@ -66,7 +66,9 @@ __global__ void __launch_bounds__(MT, 2) k_query_mlp(QueryParams q) {
         } else {
             float4 xyz = live ? q.xyz4[pi] : make_float4(0.f, 0.f, 0.f, 0.f);
             if (MODE == 0) {
-                const int d = q.C / 2;   // 6 (filter) or 3 (nofilter)
+                // columns: L image channels, sdf, [cmap xyz], [norm xyz] (include/icon_b200.h icon_query_feats)
+                const bool has_vis = q.feats & ICON_FEAT_VIS;
+                const int d = has_vis ? q.C / 2 : q.C;
                 float4 r0 = make_float4(0.f, 0.f, 0.f, 0.f), r1 = r0;
                 if (live) {
                     const float4 *r = (const float4 *)(q.rec + 8 * pi);
@@ -75,26 +77,32 @@ __global__ void __launch_bounds__(MT, 2) k_query_mlp(QueryParams q) {
                 const float vis = r1.w;
                 if (grp == 0) {
                     float sdf = r0.x, cx = r0.y, cy = r0.z, cz = r0.w;
-                    if (live && fabsf(sdf) >= q.clip) {
-                        // HGPIFuNet.py:299-304: sdf <- sign; cmap[k][c] <- s[(3k+c) mod K]
-                        sdf = sdf > 0.f ? 1.f : -1.f;
-                        long long K = *q.d_K;
-                        long long k3 = 3ll * (long long)q.krank[pi];
-                        cx = (float)q.signs[(k3) % K];
-                        cy = (float)q.signs[(k3 + 1) % K];
-                        cz = (float)q.signs[(k3 + 2) % K];
+                    const bool outlier = live && fabsf(sdf) >= q.clip;
+                    if (outlier) sdf = sdf > 0.f ? 1.f : -1.f;   // HGPIFuNet.py:299-302
+                    int col = d;
+                    x0s[col++ * MP + pl] = sdf;
+                    if (q.feats & ICON_FEAT_CMAP) {
+                        if (outlier) {
+                            // HGPIFuNet.py:303-304: cmap[k][c] <- s[(3k+c) mod K]
+                            long long K = *q.d_K;
+                            long long k3 = 3ll * (long long)q.krank[pi];
+                            cx = (float)q.signs[(k3) % K];
+                            cy = (float)q.signs[(k3 + 1) % K];
+                            cz = (float)q.signs[(k3 + 2) % K];
+                        }
+                        x0s[col++ * MP + pl] = cx;
+                        x0s[col++ * MP + pl] = cy;
+                        x0s[col++ * MP + pl] = cz;
                     }
-                    x0s[(d + 0) * MP + pl] = sdf;
-                    x0s[(d + 1) * MP + pl] = cx;
-                    x0s[(d + 2) * MP + pl] = cy;
-                    x0s[(d + 3) * MP + pl] = cz;
-                    x0s[(d + 4) * MP + pl] = r1.x;
-                    x0s[(d + 5) * MP + pl] = r1.y;
-                    x0s[(d + 6) * MP + pl] = r1.z;
-                    for (int r = d + 7; r < 16; ++r) x0s[r * MP + pl] = 0.f;
+                    if (q.feats & ICON_FEAT_NORM) {
+                        x0s[col++ * MP + pl] = r1.x;
+                        x0s[col++ * MP + pl] = r1.y;
+                        x0s[col++ * MP + pl] = r1.z;
+                    }
+                    for (int r = col; r < 16; ++r) x0s[r * MP + pl] = 0.f;
                 } else {
-                    // feat_select: vis=1 -> channels [0,d), vis=0 -> [d,2d)
-                    const int base = vis != 0.f ? 0 : d;
+                    // feat_select: vis=1 -> channels [0,d), vis=0 -> [d,2d); without vis all C channels
+                    const int base = !has_vis || vis != 0.f ? 0 : d;
                     for (int ch = grp - 1; ch < d; ch += 3) {
                         float v = live ? bilinear(q.feat + (size_t)(base + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y) : 0.f;
                         x0s[ch * MP + pl] = v;
@@ -370,7 +378,16 @@ extern "C" int icon_query(int prior, const float *points, int64_t stride_c, int6
                           const float *h_calib, const float *feat, int C, int H, int W,
                           const float *vol_feat, int VD, const void *mesh_ws, int V, int F,
                           const float *mlp_packed, const void *mlp_tc, int c0, float sdf_clip, float *out,
-                          void *ws, size_t ws_bytes, icon_stream_t stream_) {
+                          void *ws, size_t ws_bytes, icon_stream_t stream) {
+    return icon_query_feats(prior, points, stride_c, stride_n, N, h_calib, feat, C, H, W, vol_feat, VD, mesh_ws, V, F,
+                            mlp_packed, mlp_tc, c0, sdf_clip, ICON_FEAT_ALL, out, ws, ws_bytes, stream);
+}
+
+extern "C" int icon_query_feats(int prior, const float *points, int64_t stride_c, int64_t stride_n, int64_t N,
+                                const float *h_calib, const float *feat, int C, int H, int W,
+                                const float *vol_feat, int VD, const void *mesh_ws, int V, int F,
+                                const float *mlp_packed, const void *mlp_tc, int c0, float sdf_clip, int smpl_feats,
+                                float *out, void *ws, size_t ws_bytes, icon_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     ICON_CHECK_ARG(N >= 0 && N < (int64_t)INT32_MAX, "icon_query: N=%lld out of range", (long long)N);
     if (N == 0) return ICON_OK;
@@ -393,19 +410,31 @@ extern "C" int icon_query(int prior, const float *points, int64_t stride_c, int6
     q.mlp = mlp_packed; q.c0 = c0; q.clip = sdf_clip; q.out = out; q.N = N;
     if (prior == ICON_PRIOR_ICON) {
         ICON_CHECK_ARG(mesh_ws && V > 0 && F > 0, "icon_query: icon prior needs a prepared body mesh");
-        ICON_CHECK_ARG(C % 2 == 0 && C / 2 + 7 == c0, "icon_query: icon prior expects c0 = C/2 + 7 (C=%d c0=%d)", C, c0);
+        ICON_CHECK_ARG((smpl_feats & ~ICON_FEAT_ALL) == 0, "icon_query: smpl_feats mask %d has bits outside ICON_FEAT_ALL",
+                       smpl_feats);
+        const int cm = smpl_feats & ICON_FEAT_CMAP ? 1 : 0, nm = smpl_feats & ICON_FEAT_NORM ? 1 : 0;
+        const bool vs = smpl_feats & ICON_FEAT_VIS;   // with vis, feat_select keeps half of the C image channels
+        const int tail = 1 + 3 * cm + 3 * nm;          // sdf [, cmap xyz] [, norm xyz]
+        ICON_CHECK_ARG((!vs || C % 2 == 0) && c0 == (vs ? C / 2 : C) + tail,
+                       "icon_query: icon prior with smpl_feats mask %d expects c0 = %s + %d (C=%d c0=%d)", smpl_feats,
+                       vs ? "C/2" : "C", tail, C, c0);
+        q.feats = smpl_feats;
         MeshView m = mesh_view(mesh_ws, V, F);
         float4 *xyz4 = nullptr;
         int rc = run_sdf(points, stride_c, stride_n, N, h_calib, m, w.rec, nullptr, w.sdf_ws, &xyz4, stream);
         if (rc) return rc;
-        unsigned nb = (unsigned)((N + 255) / 256);
-        k_outlier_flag<<<nb, 256, 0, stream>>>(w.rec, N, sdf_clip, w.krank);
-        ICON_LAUNCHED();
-        rc = scan_exclusive_i32(w.krank, w.krank, N, w.d_K, w.scan_ws, stream);
-        if (rc) return rc;
-        k_outlier_signs<<<nb, 256, 0, stream>>>(w.rec, N, sdf_clip, w.krank, w.signs);
-        ICON_LAUNCHED();
-        q.xyz4 = xyz4; q.rec = w.rec; q.krank = w.krank; q.signs = w.signs; q.d_K = w.d_K;
+        if (cm) {
+            // the cmap overwrite needs each outlier's rank over the whole call; without cmap the query is point-local
+            unsigned nb = (unsigned)((N + 255) / 256);
+            k_outlier_flag<<<nb, 256, 0, stream>>>(w.rec, N, sdf_clip, w.krank);
+            ICON_LAUNCHED();
+            rc = scan_exclusive_i32(w.krank, w.krank, N, w.d_K, w.scan_ws, stream);
+            if (rc) return rc;
+            k_outlier_signs<<<nb, 256, 0, stream>>>(w.rec, N, sdf_clip, w.krank, w.signs);
+            ICON_LAUNCHED();
+            q.krank = w.krank; q.signs = w.signs; q.d_K = w.d_K;
+        }
+        q.xyz4 = xyz4; q.rec = w.rec;
         profile_mark(3, stream);
         rc = launch_any<0>(q, mlp_tc, stream);
         profile_mark(4, stream);

@@ -108,31 +108,40 @@ __device__ __forceinline__ void gather_point(const QueryParams &q, int64_t pi, f
             const float4 xyz = q.xyz4[pi];
             in_cube = xyz.w;
             if (MODE == 0) {
-                const int d = q.C / 2;
+                // d image channels, then sdf [, cmap xyz] [, norm xyz] (include/icon_b200.h icon_query_feats); the host
+                // checked c0 = d + 1 + 3 cmap + 3 norm <= 15, so every column written here is below 15
+                const bool has_vis = q.feats & ICON_FEAT_VIS;
+                const int d = has_vis ? q.C / 2 : q.C;
                 const float4 *rp = (const float4 *)(q.rec + 8 * pi);
                 const float4 r0 = rp[0], r1 = rp[1];
-                const int fb = r1.w != 0.f ? 0 : d;          // feat_select: vis=1 front, vis=0 back
-                float sdf = r0.x, cx = r0.y, cy = r0.z, cz = r0.w;
-                if (fabsf(sdf) >= q.clip) {                  // HGPIFuNet.py:299-304
-                    sdf = sdf > 0.f ? 1.f : -1.f;
-                    const long long K = *q.d_K, k3 = 3ll * (long long)q.krank[pi];
-                    cx = (float)q.signs[k3 % K];
-                    cy = (float)q.signs[(k3 + 1) % K];
-                    cz = (float)q.signs[(k3 + 2) % K];
+                const int fb = has_vis && r1.w == 0.f ? d : 0;   // feat_select: vis=1 front, vis=0 back; no vis: all C
+                float sdf = r0.x;
+                const bool outlier = fabsf(sdf) >= q.clip;
+                if (outlier) sdf = sdf > 0.f ? 1.f : -1.f;       // HGPIFuNet.py:299-302
+                float *col = xf + d * TC_M;                      // next SMPL column
+                col[0] = sdf;
+                col += TC_M;
+                if (q.feats & ICON_FEAT_CMAP) {
+                    float cx = r0.y, cy = r0.z, cz = r0.w;
+                    if (outlier) {                               // HGPIFuNet.py:303-304
+                        const long long K = *q.d_K, k3 = 3ll * (long long)q.krank[pi];
+                        cx = (float)q.signs[k3 % K];
+                        cy = (float)q.signs[(k3 + 1) % K];
+                        cz = (float)q.signs[(k3 + 2) % K];
+                    }
+                    col[0] = cx; col[TC_M] = cy; col[2 * TC_M] = cz;
+                    col += 3 * TC_M;
                 }
-                if (d == 6) {
+                if (q.feats & ICON_FEAT_NORM) { col[0] = r1.x; col[TC_M] = r1.y; col[2 * TC_M] = r1.z; }
+                if (d == 6) {                                    // icon-filter (C = 12, vis) and icon-mvp (C = 6)
 #pragma unroll
                     for (int ch = 0; ch < 6; ++ch)
                         xf[ch * TC_M] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
-                } else {                                     // any d in 1..8 (c0 = d + 7 <= 15)
+                } else {                                     // any d in 1..14 (c0 >= d + 1)
 #pragma unroll
-                    for (int ch = 0; ch < 8; ++ch)
+                    for (int ch = 0; ch < 14; ++ch)
                         if (ch < d) xf[ch * TC_M] = bilinear(q.feat + (size_t)(fb + ch) * q.H * q.W, q.H, q.W, xyz.x, xyz.y);
                 }
-                const float smpl[7] = {sdf, cx, cy, cz, r1.x, r1.y, r1.z};
-#pragma unroll
-                for (int t = 0; t < 7; ++t)
-                    if (d + t < 15) xf[(d + t) * TC_M] = smpl[t];
             } else if (MODE == 1) {
                 if (q.C == 12) {
 #pragma unroll

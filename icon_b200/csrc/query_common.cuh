@@ -9,8 +9,9 @@ struct QueryParams {
     const float4 *xyz4;      // [N] transformed xyz + in_cube
     const float *rec;        // [N][8] icon prior
     const int32_t *krank;    // [N] exclusive outlier rank (icon)
-    const int8_t *signs;     // [K] sign of the k-th outlier (icon)
-    const int64_t *d_K;      // number of outliers (icon)
+    const int8_t *signs;     // [K] sign of the k-th outlier (icon, with cmap)
+    const int64_t *d_K;      // number of outliers (icon, with cmap)
+    int feats;               // icon: ICON_FEAT_* mask of the smpl_feats subset (include/icon_b200.h icon_query_feats)
     const float *feat;       // [C][H][W]
     int C, H, W;
     const float *vol;        // [7][VD][VD][VD] (pamir)

@@ -313,8 +313,17 @@ class HGPIFuNet(BasePIFuNet):
         regressor = regressor if regressor is not None else self.if_regressor
         if regressor.last_op is not None:
             raise NotImplementedError("query(): last_op (sigmoid) is the training path; test_mode=True at inference")
-        if self.prior_type == "icon" and set(self.smpl_feats) != {"sdf", "cmap", "norm", "vis"}:
-            raise NotImplementedError("fused query kernel implements smpl_feats = sdf, cmap, norm, vis")
+        if self.prior_type == "icon":
+            # HGPIFuNet.py:97-104 sized the MLP from smpl_dim; the columns come from smpl_feats (the reference fails
+            # inside conv1d when the two disagree)
+            tail = ops.icon_c0(self.smpl_feats, 0)
+            for im_feat in features:
+                want = ops.icon_c0(self.smpl_feats, im_feat.shape[1])
+                if regressor.c0 != want:
+                    raise RuntimeError(
+                        f"icon prior: smpl_feats {self.smpl_feats} give {tail} SMPL columns (sdf 1, cmap 3, norm 3) and, "
+                        f"with {im_feat.shape[1]} feature channels, an MLP input width c0 = {want}; the MLP has "
+                        f"c0 = {regressor.c0} (smpl_dim = {self.smpl_dim})")
         preds_list = []
         body = self._prepared_body() if self.prior_type == "icon" else None
         vol = None
@@ -327,7 +336,7 @@ class HGPIFuNet(BasePIFuNet):
         with torch.no_grad():
             for im_feat in features:
                 preds = ops.query(self.prior_type, points, calibs, im_feat, regressor.packed(),
-                                  body=body, vol_feat=vol, sdf_clip=self.sdf_clip)
+                                  body=body, vol_feat=vol, sdf_clip=self.sdf_clip, smpl_feats=self.smpl_feats)
                 preds_list.append(preds)
         return preds_list
 

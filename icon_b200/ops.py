@@ -215,8 +215,34 @@ def _point_strides(points):
     return points, points.stride(1), points.stride(2), points.shape[2]
 
 
-def query(prior, points, calib, feat, mlp, c0=None, body=None, vol_feat=None, sdf_clip=0.05, out=None):
-    """Fused HGPIFuNet.query for one feature stack, B=1.  points [1,3,N] -> preds [1,1,N]."""
+SMPL_FEATS_ALL = ("sdf", "cmap", "norm", "vis")
+FEAT_CMAP, FEAT_NORM, FEAT_VIS = 1, 2, 4                         # include/icon_b200.h ICON_FEAT_*
+_FEAT_BIT = {"sdf": 0, "cmap": FEAT_CMAP, "norm": FEAT_NORM, "vis": FEAT_VIS}
+
+
+def smpl_feats_mask(smpl_feats):
+    """`smpl_feats` names -> the ICON_FEAT_* mask of icon_query_feats.  `sdf` is always a column and the order does not
+    matter: the reference concatenates sdf, cmap, norm, vis in that order whatever the list says."""
+    unknown = set(smpl_feats) - set(_FEAT_BIT)
+    if unknown:
+        raise _C.IconError(f"smpl_feats: unknown feature(s) {sorted(unknown)}; the icon prior knows {list(SMPL_FEATS_ALL)}")
+    mask = 0
+    for name in set(smpl_feats):
+        mask |= _FEAT_BIT[name]
+    return mask
+
+
+def icon_c0(smpl_feats, C):
+    """MLP input width of the icon prior for C image-feature channels: C/2 with `vis` (feat_select), C without, plus
+    sdf and 3 each for cmap / norm (the check icon_query_feats makes)."""
+    mask = smpl_feats_mask(smpl_feats)
+    return (C // 2 if mask & FEAT_VIS else C) + 1 + 3 * bool(mask & FEAT_CMAP) + 3 * bool(mask & FEAT_NORM)
+
+
+def query(prior, points, calib, feat, mlp, c0=None, body=None, vol_feat=None, sdf_clip=0.05, out=None,
+          smpl_feats=SMPL_FEATS_ALL):
+    """Fused HGPIFuNet.query for one feature stack, B=1.  points [1,3,N] -> preds [1,1,N].
+    smpl_feats: the icon prior's SMPL feature subset (include/icon_b200.h icon_query_feats); other priors ignore it."""
     _need_cuda(points, feat, mlp.f32, mlp.tc, vol_feat)
     c0 = mlp.c0
     pts, sc, sn, N = _point_strides(points)
@@ -225,6 +251,7 @@ def query(prior, points, calib, feat, mlp, c0=None, body=None, vol_feat=None, sd
         raise _C.IconError(f"feature map must be [1,C,H,W], got {tuple(feat.shape)}")
     feat = feat.float().contiguous()
     C, H, W = feat.shape[1:]
+    mask = smpl_feats_mask(smpl_feats) if prior == "icon" else 0
     pid = PRIOR_ID[prior]
     if out is None:
         out = torch.empty(1, 1, N, dtype=torch.float32, device=pts.device)
@@ -243,8 +270,9 @@ def query(prior, points, calib, feat, mlp, c0=None, body=None, vol_feat=None, sd
         VD = vol_feat.shape[2]
     nbytes = lib.icon_query_workspace_bytes(N, F, pid)
     ws = torch.empty(max(nbytes, 256), dtype=torch.uint8, device=pts.device)
-    check(lib.icon_query(pid, _p(pts), sc, sn, N, _calib_rows(calib), _p(feat), C, H, W, _p(vol_feat), VD,
-                         _p(mesh), V, F, _p(mlp.f32), _p(mlp.tc), c0, float(sdf_clip), _p(out), _p(ws), nbytes, _stream()),
+    check(lib.icon_query_feats(pid, _p(pts), sc, sn, N, _calib_rows(calib), _p(feat), C, H, W, _p(vol_feat), VD,
+                               _p(mesh), V, F, _p(mlp.f32), _p(mlp.tc), c0, float(sdf_clip), mask, _p(out), _p(ws),
+                               nbytes, _stream()),
           "icon_query")
     return out
 

@@ -45,7 +45,7 @@ int64_t icon_launch_count(void);
 /* Measurement hook (bench.py roofline): when enabled, icon_query records CUDA events on its
  * stream around its stages; icon_profile_last_query synchronises on the last one and returns
  * the stage durations of the most recent icon_query in milliseconds:
- * h_ms[0] binning+sort, [1] SDF brick kernel, [2] outlier rank, [3] gather+MLP kernel. */
+ * h_ms[0] binning+sort, [1] SDF brick kernel, [2] outlier rank (empty without cmap), [3] gather+MLP kernel. */
 int icon_profile_enable(int on);
 int icon_profile_last_query(float *h_ms);
 
@@ -97,7 +97,7 @@ int icon_get_mlp_impl(void);
  *   mesh_ws     : icon only: workspace filled by icon_smpl_prepare (same V,F); else NULL
  *   mlp_packed  : ICON_MLP_PACKED_FLOATS floats
  *   mlp_tc      : ICON_MLP_TC_BYTES bytes (16-byte aligned) or NULL (-> FP32 kernel)
- *   c0          : MLP input channels (13 or 10)
+ *   c0          : MLP input channels (13 or 10 for the icon prior's full smpl_feats; see icon_query_feats)
  *   sdf_clip    : cfg.sdf_clip/100 (icon)
  *   out         : [N] f32 occupancy (preds[0,0,:])
  *   ws          : scratch, icon_query_workspace_bytes(N, F) bytes
@@ -108,6 +108,26 @@ int icon_query(int prior, const float *points, int64_t stride_c, int64_t stride_
                const float *vol_feat, int VD, const void *mesh_ws, int V, int F,
                const float *mlp_packed, const void *mlp_tc, int c0, float sdf_clip, float *out,
                void *ws, size_t ws_bytes, icon_stream_t stream);
+
+/* icon_query for any `smpl_feats` subset of the icon prior (HGPIFuNet.py:97-104, 298-346).  smpl_feats is a bitmask
+ * of the ICON_FEAT_* bits below; `sdf` is always a column.  The MLP input columns are, in order:
+ *   image features   with VIS: the C/2 channels feat_select picks (vis = 1: [0, C/2), vis = 0: [C/2, C));
+ *                    without:  all C channels in order
+ *   sdf              |sdf| >= sdf_clip becomes sign(sdf)
+ *   cmap xyz         if CMAP, with the call-level outlier overwrite (HGPIFuNet.py:303-304)
+ *   norm xyz         if NORM
+ * so c0 = C/2 + 1 + 3 cmap + 3 norm with VIS (C even) and C + 1 + 3 cmap + 3 norm without.  Without CMAP the query
+ * is point-local (no outlier rank: a call split into pieces gives the same values).  The mask is ignored for pifu /
+ * pamir.  icon_query is this function with all three bits set. */
+#define ICON_FEAT_CMAP 1
+#define ICON_FEAT_NORM 2
+#define ICON_FEAT_VIS 4
+#define ICON_FEAT_ALL (ICON_FEAT_CMAP | ICON_FEAT_NORM | ICON_FEAT_VIS)
+int icon_query_feats(int prior, const float *points, int64_t stride_c, int64_t stride_n, int64_t N,
+                     const float *h_calib, const float *feat, int C, int H, int W,
+                     const float *vol_feat, int VD, const void *mesh_ws, int V, int F,
+                     const float *mlp_packed, const void *mlp_tc, int c0, float sdf_clip, int smpl_feats,
+                     float *out, void *ws, size_t ws_bytes, icon_stream_t stream);
 
 /* Points-per-warp policy of the SDF kernel: force_ppw in {1, 8, 32} pins it (0 = automatic: 1 below ppw8_from
  * points per call, 8 below ppw32_from, else 32; negative thresholds keep the current value).  Results are
