@@ -152,6 +152,30 @@ int icon_sdf_only(const float *points, int64_t stride_c, int64_t stride_n, int64
 int icon_sdf_bruteforce(const float *points, int64_t stride_c, int64_t stride_n, int64_t N,
                         const float *h_calib, const void *mesh_ws, int V, int F, float *rec,
                         int32_t *face, icon_stream_t stream);
+/* ------------------------------------------------------------------ any triangle mesh: distance and sampling
+ * The two trimesh calls of the benchmark's Chamfer / P2S metric (lib/dataset/Evaluator.py:200-230,
+ * calculate_chamfer_p2s): trimesh.proximity.closest_point and trimesh.sample.sample_surface_even.
+ *
+ * icon_mesh_prepare: distance-only workspace for verts [V,3] f32, faces [F,3] i64 (no cmap, vis or normals; F is
+ * bounded by memory only): per-face records, Morton-sorted 4-ary AABB tree with 32-bit ids, and the cumulative
+ * area weights the sampler draws from.  The workspace stays valid while verts / faces are unchanged. */
+size_t icon_mesh_workspace_bytes(int V, int F);
+int icon_mesh_prepare(const float *verts, const int64_t *faces, int V, int F, void *mesh_ws, size_t mesh_ws_bytes,
+                      icon_stream_t stream);
+/* Unsigned nearest face of points [N,3] f32 (contiguous): out_sqdist [N] f32 exact squared distance, out_face [N] i32
+ * (may be NULL) the nearest face, lowest index on ties.  Bit-identical to brute force over all faces
+ * (oracle_mesh_distance).  Needs no scratch. */
+int icon_mesh_distance(const float *points, int64_t N, const void *mesh_ws, int V, int F, float *out_sqdist,
+                       int32_t *out_face, icon_stream_t stream);
+/* sample_surface_even(mesh, count) (trimesh 3.9.35 semantics, seeded): 3 count area-weighted uniform candidates, then
+ * greedy removal in candidate order of every candidate within radius sqrt(area / (3 count)) of a kept one, keeping at
+ * most count (<= 8192).  out_points [count,3] f32, out_face [count] i32, *out_count (device i32) = samples kept.
+ * verts / faces are the arrays the workspace was prepared from; ws: icon_mesh_sample_workspace_bytes(count). */
+size_t icon_mesh_sample_workspace_bytes(int count);
+int icon_mesh_sample(const float *verts, const int64_t *faces, int V, int F, const void *mesh_ws, int count,
+                     uint64_t seed, float *out_points, int32_t *out_face, int32_t *out_count, void *ws,
+                     size_t ws_bytes, icon_stream_t stream);
+
 /* MLP alone on a ready [c0,N] feature matrix (parity tap for lib/net/MLP.py:49-72). */
 int icon_mlp_only(const float *feature, int c0, int64_t N, const float *mlp_packed,
                   const void *mlp_tc, float *out, icon_stream_t stream);
