@@ -110,7 +110,7 @@ struct Carver {
 };
 
 // ---------------------------------------------------------------- mesh workspace layout
-constexpr int BVH_MAX_LEVELS = 10;   // 4-ary implicit tree over leaves of 4 Morton-sorted faces
+constexpr int TREE_MAX_LEVELS = 17;  // 4-ary implicit tree over leaves of 4 Morton-sorted faces: 4^16 leaves > 2^31 faces
 constexpr int RAY_GRID = 256;        // yz cell grid for the +x ray parity
 constexpr int RAY_LIST_PER_FACE = 64;
 
@@ -133,18 +133,25 @@ struct MeshHeader {                  // device-resident, written by icon_smpl_pr
     int pad;
 };
 
-struct MeshView {
+// Morton-sorted per-face records and the implicit 4-ary AABB tree over them (face_tree.cuh builds and walks it)
+struct FaceTree {
+    float4 *tri_s;        // [F][3] per-face records (a.xyz, ab.x) (ab.yz, ac.xy) (ac.z, -, -, -), sorted
+    float4 *sph_s;        // [F] bounding spheres (centre xyz, radius), conservative, sorted
+    int32_t *order;       // [F] sorted position -> original face id
+    float4 *nodes;        // [total_nodes][2]: (min.xyz, -) (max.xyz, -), level 0 (leaves) first
+    int F;
+    int nlevels;
+    int lvl_cnt[TREE_MAX_LEVELS];
+    int lvl_off[TREE_MAX_LEVELS];
+};
+
+struct MeshView : FaceTree {
     const float4 *tri;    // [F][3]: (a.xyz, ab.x) (ab.yz, ac.xy) (ac.z, -, -, -), original face order
     const float4 *sph;    // [F]: bounding sphere (centre xyz, radius), conservative
     const float4 *attr;   // [F][6]: normals 9, cmap 9, vis 3, pad 3
     const float4 *rbox;   // [F][2]: (ymin, ymax, zmin, zmax) (xmax, xmin, -, -)
     float *vnormals;      // [V][3] scratch
-    // Morton-sorted copy + implicit AABB tree
-    unsigned long long *keys;   // [F] morton << 32 | face
-    int32_t *order;       // [F] sorted position -> face id
-    float4 *tri_s;        // [F][3] sorted
-    float4 *sph_s;        // [F] sorted
-    float4 *nodes;        // [total_nodes][2]: (min.xyz, -) (max.xyz, -), level 0 (leaves) first
+    unsigned long long *keys;   // [F] morton << 32 | face: the sort keys of the tree
     // ray grid
     int32_t *rcount;      // [RAY_GRID^2 + 1]
     int32_t *roff;        // [RAY_GRID^2 + 1]
@@ -160,10 +167,7 @@ struct MeshView {
     int32_t *boff;        // [NBRICK + 1] list offsets
     unsigned short *blist;   // [brick_cap] leaf ids, ascending box distance to the brick per list
     int64_t brick_cap;
-    int V, F;
-    int nlevels;
-    int lvl_cnt[BVH_MAX_LEVELS];
-    int lvl_off[BVH_MAX_LEVELS];
+    int V;
 };
 size_t mesh_ws_bytes(int V, int F);
 MeshView mesh_view(const void *ws, int V, int F);

@@ -5,28 +5,27 @@
 //   trimesh.proximity.closest_point  -> icon_mesh_distance: exact squared distance + lowest-index nearest face
 //   trimesh.sample.sample_surface_even -> icon_mesh_sample: area-weighted candidates, greedy radius removal
 //
-// Any triangle mesh (no cmap / vis / normals, no sign): icon_mesh_prepare builds the same per-face records (a, ab, ac,
-// bounding sphere) and Morton-sorted implicit 4-ary AABB tree as icon_smpl_prepare, but with 32-bit leaf and node ids
-// and as many levels as F needs, so F is bounded by memory only.  The Morton code is taken over the mesh's own
-// bounding cube (the SMPL tree uses the fixed [-1.5, 1.5]^3 of a body in the query frame).
+// Any triangle mesh (no cmap / vis / normals, no sign): icon_mesh_prepare builds the same per-face records and
+// Morton-sorted 4-ary AABB tree as icon_smpl_prepare (face_tree.cuh), but with 32-bit ids, so F is bounded by memory
+// only.  The Morton code is taken over the mesh's own bounding cube (the SMPL tree uses the fixed [-1.5, 1.5]^3 of a
+// body in the query frame), its sort is a bucket sort and rank.
 //
-// k_mesh_dist is the tree walk of k_sdf_warp (sdf.cu, DESIGN.md 4.2) at one query point per warp (PPW = 1): the query
-// sets are sparse (1000 samples on a mesh), so the warp box is the point and the 32 lanes split the candidate faces.
-// Phases A (greedy descent), B (breadth-first cull, 32-bit frontier in shared memory), C (sphere cull, support-function
-// bound, exact Ericson distance) and the tie rule are k_sdf_warp's; a frontier overflow falls back to all faces.
-// Results equal the brute-force scan (oracle_mesh_distance in oracle/mesh_oracle.c) bit for bit.
+// k_mesh_dist runs face_tree.cuh's walk at one query point per warp (PPW = 1): the query sets are sparse (1000 samples
+// on a mesh), so the warp box is the point and the 32 lanes split the candidate faces.  The frontier holds 1024
+// 32-bit ids; the slacks scale with the largest coordinate in play.  Results equal the brute-force scan
+// (oracle_mesh_distance in oracle/mesh_oracle.c) bit for bit.
 //
-// Resources (nvcc 12.9 -Xptxas -v, sm_90a): k_mesh_dist 58 registers, 41472 bytes static shared memory per 128-thread
-// block (4 warps x (2 x 1024 frontier ids + 32 staged faces)), no spills; shared memory
-// bounds residency at 5 blocks = 20 warps per SM.  k_gm_select 32 registers, no spills.
+// Resources (nvcc 12.9 -Xptxas -v, sm_90a): k_mesh_dist 56 registers, 41472 bytes static shared memory per
+// 128-thread block (4 warps x (2 x 1024 frontier ids + 32 staged faces)), no spills; shared memory bounds residency at
+// 5 blocks = 20 warps per SM.  k_gm_select 32 registers, no spills.
 #include <float.h>
 
 #include "common.cuh"
+#include "face_tree.cuh"
 #include "geom.cuh"
 
 namespace icon {
 
-constexpr int GM_MAX_LEVELS = 17;            // 4^16 leaves of 4 faces > 2^31 faces
 constexpr int GM_BUCKET_BITS = 18;           // sort buckets: the top 18 of the 30 Morton bits
 constexpr int GM_NBUCKET = 1 << GM_BUCKET_BITS;
 constexpr int GM_T = 128;                    // 4 warps per block, one query point per warp
@@ -42,11 +41,7 @@ struct GMeshHeader {                         // device-resident, written by icon
     float absmax;                            // largest |coordinate| of the mesh (scale of the bounds' slack)
 };
 
-struct GMesh {
-    float4 *tri_s;                           // [F][3] per-face records (geom.cuh layout), Morton-sorted
-    float4 *sph_s;                           // [F] bounding spheres, sorted
-    int32_t *order;                          // [F] sorted position -> original face id
-    float4 *nodes;                           // [total_nodes][2] (min.xyz, -) (max.xyz, -), leaves first
+struct GMesh : FaceTree {
     unsigned long long *wcum;                // [F] inclusive prefix sum of the face weights, original face order
     GMeshHeader *hdr;
     // prepare scratch
@@ -55,10 +50,7 @@ struct GMesh {
     int32_t *bcount, *boff;                  // [GM_NBUCKET + 1]
     void *scan_ws;                           // int32 bucket scan
     unsigned long long *s64_ws;              // block totals of the uint64 scan
-    int V, F;
-    int nlevels;
-    int lvl_cnt[GM_MAX_LEVELS];
-    int lvl_off[GM_MAX_LEVELS];
+    int V;
 };
 
 static size_t s64_ws_elems(int64_t n) {
@@ -72,19 +64,12 @@ static size_t s64_ws_elems(int64_t n) {
 
 static GMesh carve_gmesh(Carver &c, int V, int F) {
     GMesh m{};
-    m.V = V; m.F = F;
-    int64_t n = (F + 3) / 4, o = 0;
-    int l = 0;
-    while (true) {
-        m.lvl_cnt[l] = (int)n; m.lvl_off[l] = (int)o; o += n; ++l;
-        if (n == 1) break;
-        n = (n + 3) / 4;
-    }
-    m.nlevels = l;
+    m.V = V;
+    const size_t total_nodes = tree_levels(m, F);
     m.tri_s = c.take<float4>((size_t)F * 3);
     m.sph_s = c.take<float4>((size_t)F);
     m.order = c.take<int32_t>((size_t)F);
-    m.nodes = c.take<float4>((size_t)o * 2);
+    m.nodes = c.take<float4>(total_nodes * 2);
     m.wcum = c.take<unsigned long long>((size_t)F);
     m.hdr = c.take<GMeshHeader>(1);
     m.keys = c.take<unsigned long long>((size_t)F);
@@ -157,14 +142,6 @@ __global__ void __launch_bounds__(256) k_gm_bounds(const float *__restrict__ ver
     }
 }
 
-__device__ __forceinline__ unsigned expand10_gm(unsigned v) {
-    v = (v * 0x00010001u) & 0xFF0000FFu;
-    v = (v * 0x00000101u) & 0x0F00F00Fu;
-    v = (v * 0x00000011u) & 0xC30C30C3u;
-    v = (v * 0x00000005u) & 0x49249249u;
-    return v;
-}
-
 __device__ __forceinline__ V3 centroid(V3 a, V3 b, V3 c) {
     return mk3((a.x + b.x + c.x) / 3.f, (a.y + b.y + c.y) / 3.f, (a.z + b.z + c.z) / 3.f);
 }
@@ -184,9 +161,7 @@ __global__ void __launch_bounds__(256) k_gm_keys(const float *__restrict__ verts
     if (f == 0)
         m.hdr->absmax = fmaxf(fmaxf(fmaxf(fabsf(lx), fabsf(ly)), fabsf(lz)),
                               fmaxf(fmaxf(fabsf(ord2f(h->hi[0])), fabsf(ord2f(h->hi[1]))), fabsf(ord2f(h->hi[2]))));
-    const V3 sc = centroid(a, b, c);
-    auto qz = [s](float v, float l) { return (unsigned)fminf(fmaxf((v - l) * s, 0.f), 1023.f); };
-    const unsigned code = (expand10_gm(qz(sc.x, lx)) << 2) | (expand10_gm(qz(sc.y, ly)) << 1) | expand10_gm(qz(sc.z, lz));
+    const unsigned code = morton30(centroid(a, b, c), mk3(lx, ly, lz), s);
     m.keys[f] = ((unsigned long long)code << 32) | (unsigned)f;
     atomicAdd(&m.bcount[code >> (30 - GM_BUCKET_BITS)], 1);
     // weight: the same fp64 area as k_gm_bounds, relative to the largest, in wbits fixed-point bits
@@ -225,50 +200,19 @@ __global__ void __launch_bounds__(256) k_gm_records(const float *__restrict__ ve
                                                     GMesh m) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= m.F) return;
-    const float sc1 = fmaxf(1.f, m.hdr->absmax);
     V3 a, b, c;
     load_face(verts, faces, m.order[p], a, b, c);
-    const V3 ab = sub3(b, a), ac = sub3(c, a);
-    const V3 sc = centroid(a, b, c);
-    const float ra = dot3(sub3(a, sc), sub3(a, sc)), rb = dot3(sub3(b, sc), sub3(b, sc)),
-                rc = dot3(sub3(c, sc), sub3(c, sc));
-    const float sr = sqrtf(fmaxf(ra, fmaxf(rb, rc))) * 1.0001f + 1e-7f * sc1;
-    m.tri_s[3 * (size_t)p + 0] = make_float4(a.x, a.y, a.z, ab.x);
-    m.tri_s[3 * (size_t)p + 1] = make_float4(ab.y, ab.z, ac.x, ac.y);
-    m.tri_s[3 * (size_t)p + 2] = make_float4(ac.z, 0.f, 0.f, 0.f);
-    m.sph_s[p] = make_float4(sc.x, sc.y, sc.z, sr);
+    write_face_record(a, b, c, 1e-7f * fmaxf(1.f, m.hdr->absmax), m.tri_s + 3 * (size_t)p, m.sph_s + p);
 }
 
 __global__ void __launch_bounds__(256) k_gm_leaves(GMesh m) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= m.lvl_cnt[0]) return;
-    float4 lo = make_float4(FLT_MAX, FLT_MAX, FLT_MAX, 0.f), hi = make_float4(-FLT_MAX, -FLT_MAX, -FLT_MAX, 0.f);
-    for (int t = 4 * n; t < min(4 * n + 4, m.F); ++t) {
-        const Tri tr = load_tri(m.tri_s + 3 * (size_t)t);
-        const V3 vs[3] = {tr.a, mk3(tr.a.x + tr.ab.x, tr.a.y + tr.ab.y, tr.a.z + tr.ab.z),
-                          mk3(tr.a.x + tr.ac.x, tr.a.y + tr.ac.y, tr.a.z + tr.ac.z)};
-        for (int k = 0; k < 3; ++k) {
-            lo.x = fminf(lo.x, vs[k].x); hi.x = fmaxf(hi.x, vs[k].x);
-            lo.y = fminf(lo.y, vs[k].y); hi.y = fmaxf(hi.y, vs[k].y);
-            lo.z = fminf(lo.z, vs[k].z); hi.z = fmaxf(hi.z, vs[k].z);
-        }
-    }
-    m.nodes[2 * (size_t)n] = lo;
-    m.nodes[2 * (size_t)n + 1] = hi;
+    if (n < m.lvl_cnt[0]) write_leaf_box(m, n);
 }
 
 __global__ void __launch_bounds__(256) k_gm_level(GMesh m, int l) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n >= m.lvl_cnt[l]) return;
-    const float4 *child = m.nodes + 2 * (size_t)m.lvl_off[l - 1];
-    float4 lo = make_float4(FLT_MAX, FLT_MAX, FLT_MAX, 0.f), hi = make_float4(-FLT_MAX, -FLT_MAX, -FLT_MAX, 0.f);
-    for (int c = 4 * n; c < min(4 * n + 4, m.lvl_cnt[l - 1]); ++c) {
-        const float4 a = child[2 * (size_t)c], b = child[2 * (size_t)c + 1];
-        lo.x = fminf(lo.x, a.x); lo.y = fminf(lo.y, a.y); lo.z = fminf(lo.z, a.z);
-        hi.x = fmaxf(hi.x, b.x); hi.y = fmaxf(hi.y, b.y); hi.z = fmaxf(hi.z, b.z);
-    }
-    m.nodes[2 * ((size_t)m.lvl_off[l] + n)] = lo;
-    m.nodes[2 * ((size_t)m.lvl_off[l] + n) + 1] = hi;
+    if (n < m.lvl_cnt[l]) write_parent_box(m, l, n);
 }
 
 // ---- inclusive uint64 prefix sum (the weights' cumulative sum): integer, so exact and independent of block order
@@ -320,189 +264,26 @@ static int scan64_inclusive(unsigned long long *x, int64_t n, unsigned long long
 __global__ void k_gm_total(GMesh m) { m.hdr->total = m.wcum[m.F - 1]; }
 
 // ---------------------------------------------------------------- nearest face, one point per warp
-__device__ __forceinline__ float gm_box_dist2(V3 p, float4 lo, float4 hi) {
-    const float dx = fmaxf(fmaxf(lo.x - p.x, p.x - hi.x), 0.f);
-    const float dy = fmaxf(fmaxf(lo.y - p.y, p.y - hi.y), 0.f);
-    const float dz = fmaxf(fmaxf(lo.z - p.z, p.z - hi.z), 0.f);
-    return fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-}
-__device__ __forceinline__ float gm_box_far2(V3 p, float4 lo, float4 hi) {
-    const float dx = fmaxf(fabsf(lo.x - p.x), fabsf(hi.x - p.x));
-    const float dy = fmaxf(fabsf(lo.y - p.y), fabsf(hi.y - p.y));
-    const float dz = fmaxf(fabsf(lo.z - p.z), fabsf(hi.z - p.z));
-    return fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-}
-__device__ __forceinline__ float gm_warp_min(float v) {
-    for (int o = 16; o; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ float gm_warp_max(float v) {
-    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
-struct GmWarpSmem {
-    float4 sph[32];                          // bounding spheres of the surviving faces of the current chunk
-    float4 tri[32][3];                       // their (a, ab, ac) records
-    int kk[32];                              // their sorted positions
-    int32_t fr[2][GM_FR_CAP];                // node / leaf ids
-};
+using MeshDistSmem = WalkSmem<int32_t, GM_FR_CAP>;
 
 __global__ void __launch_bounds__(GM_T) k_mesh_dist(const float *__restrict__ pts, int64_t N, GMesh m,
                                                     float *__restrict__ out_d, int32_t *__restrict__ out_f) {
-    __shared__ GmWarpSmem smem[GM_T / 32];
-    GmWarpSmem &S = smem[threadIdx.x >> 5];
-    const int lane = threadIdx.x & 31;
+    __shared__ MeshDistSmem smem[GM_T / 32];
     const int64_t i = (int64_t)blockIdx.x * (GM_T / 32) + (threadIdx.x >> 5);
     if (i >= N) return;                                          // whole warp
     const V3 p = mk3(pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]);
-    // k_sdf_warp's additive slacks (1e-6 on lengths, 1e-7 on the support bound) are sized for coordinates of
+    // the SMPL path's additive slacks (1e-6 on lengths, 1e-7 on the support bound) are sized for coordinates of
     // magnitude <= 1; a general mesh may be in any unit, so they scale with the largest coordinate in play (the leaf
     // boxes are built from a + ab, which may sit an ulp of that magnitude away from the vertex)
     const float sc = fmaxf(fmaxf(1.f, m.hdr->absmax), fmaxf(fmaxf(fabsf(p.x), fabsf(p.y)), fabsf(p.z)));
-    const float tol = 1e-6f * sc, tol_sup = 1e-7f * sc * sc;
-    const float4 wlo = make_float4(p.x - tol, p.y - tol, p.z - tol, 0.f);
-    const float4 whi = make_float4(p.x + tol, p.y + tol, p.z + tol, 0.f);
-    const float rw = tol;                                        // k_sdf_warp's warp radius for one point
-
-    float best = FLT_MAX;
-    int bi = 0x7fffffff;
-    auto try_face = [&](int k) {
-        const Tri tr = load_tri(m.tri_s + 3 * (size_t)k);
-        const float d = tri_sqdist(p, tr.a, tr.ab, tr.ac);
-        const int f = __ldg(m.order + k);
-        if (d < best || (d == best && f < bi)) { best = d; bi = f; }
-    };
-    // ---- phase A: greedy descent towards the point -> a first bound
-    {
-        int node = 0;
-        for (int lvl = m.nlevels - 1; lvl > 0; --lvl) {
-            const int ch = 4 * node + (lane & 3);
-            float a = FLT_MAX;
-            int ai = ch;
-            if (ch < m.lvl_cnt[lvl - 1]) {
-                const float4 *nb = m.nodes + 2 * ((size_t)m.lvl_off[lvl - 1] + ch);
-                a = gm_box_dist2(p, __ldg(nb), __ldg(nb + 1));
-            }
-            for (int o = 1; o <= 2; o <<= 1) {
-                const float ob = __shfl_xor_sync(0xffffffffu, a, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, ai, o);
-                if (ob < a || (ob == a && oi < ai)) { a = ob; ai = oi; }
-            }
-            node = __shfl_sync(0xffffffffu, ai, 0);
-        }
-        for (int k = 4 * node; k < min(4 * node + 4, m.F); ++k) try_face(k);
-    }
-    float ubw2 = sqrtf(best);
-    float ub2 = (ubw2 * 1.00001f + tol) * (ubw2 * 1.00001f + tol);
-
-    // ---- phase B: breadth-first cull, 32 child boxes per step; the bound tightens with the nearest far corner
-    int cur = 0, n = 1;
-    bool overflow = false;
-    if (lane == 0) S.fr[0][0] = 0;
-    __syncwarp();
-    for (int lvl = m.nlevels - 1; lvl > 0 && !overflow; --lvl) {
-        int nn = 0;
-        float far2 = FLT_MAX;
-        const int ccnt = m.lvl_cnt[lvl - 1];
-        const float4 *nodes = m.nodes + 2 * (size_t)m.lvl_off[lvl - 1];
-        for (int base = 0; base < n; base += 8) {
-            const int slot = base + (lane >> 2);
-            bool pass = false;
-            int ch = 0;
-            if (slot < n) {
-                ch = 4 * S.fr[cur][slot] + (lane & 3);
-                if (ch < ccnt) {
-                    const float4 lo = __ldg(nodes + 2 * (size_t)ch), hi = __ldg(nodes + 2 * (size_t)ch + 1);
-                    const float gx = fmaxf(fmaxf(lo.x - whi.x, wlo.x - hi.x), 0.f);
-                    const float gy = fmaxf(fmaxf(lo.y - whi.y, wlo.y - hi.y), 0.f);
-                    const float gz = fmaxf(fmaxf(lo.z - whi.z, wlo.z - hi.z), 0.f);
-                    pass = fmaf(gz, gz, fmaf(gy, gy, gx * gx)) <= ub2;
-                    far2 = fminf(far2, gm_box_far2(p, lo, hi));
-                }
-            }
-            const unsigned mask = __ballot_sync(0xffffffffu, pass);
-            const int at = nn + __popc(mask & ((1u << lane) - 1u));
-            if (pass && at < GM_FR_CAP) S.fr[cur ^ 1][at] = ch;
-            nn += __popc(mask);
-        }
-        if (nn > GM_FR_CAP) overflow = true;
-        n = nn;
-        cur ^= 1;
-        const float l2 = sqrtf(gm_warp_min(far2)) + rw;
-        if (l2 < ubw2) { ubw2 = l2; ub2 = (ubw2 * 1.00001f + tol) * (ubw2 * 1.00001f + tol); }
-        __syncwarp();
-    }
-
-    // ---- phase C: 32 faces (8 leaves) at a time, sphere-culled against the loosest bound, then split over the lanes
-    //      with the per-lane sphere and support-function bounds before the exact distance
-    float sbA = best > 0.f ? best * rsqrtf(best) * 1.00001f + tol : tol;
-    float ubA = ubw2 * 1.00001f + tol;
-    auto lane_test = [&](int k, float4 s, const float4 *tr) {
-        const float dx = p.x - s.x, dy = p.y - s.y, dz = p.z - s.z;
-        const float dd = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-        const float l = sbA + s.w;
-        if (dd > l * l) return;
-        const float4 r0 = tr[0], r1 = tr[1], r2 = tr[2];
-        const V3 ab = mk3(r0.w, r1.x, r1.y), ac = mk3(r1.z, r1.w, r2.x);
-        const float S1 = fmaf(dz, ab.z, fmaf(dy, ab.y, dx * ab.x));
-        const float T1 = fmaf(dz, ac.z, fmaf(dy, ac.y, dx * ac.x));
-        const float M = fmaxf(fmaxf(-(S1 + T1), fmaf(2.f, S1, -T1)), fmaf(2.f, T1, -S1)) * (1.f / 3.f);
-        const float g = dd - M - tol_sup;
-        if (g > 0.f && g * g > best * dd * 1.0001f) return;
-        const float d = tri_sqdist(p, mk3(r0.x, r0.y, r0.z), ab, ac);
-        if (!(d <= best)) return;                                // also drops NaN, as the brute-force scan does
-        const int f = __ldg(m.order + k);
-        if (d < best || f < bi) {
-            best = d; bi = f;
-            sbA = d > 0.f ? d * rsqrtf(d) * 1.00001f + tol : tol;
-        }
-    };
-    auto merge = [&]() {                                         // lowest distance, then lowest face id
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-        }
-    };
-    if (!overflow) {
-        for (int base = 0; base < n; base += 8) {
-            const int slot = base + (lane >> 2);
-            bool pass = false;
-            int k = 0;
-            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (slot < n) {
-                k = 4 * S.fr[cur][slot] + (lane & 3);
-                if (k < m.F) {
-                    s = __ldg(m.sph_s + k);
-                    const float l2 = ubA + s.w;
-                    pass = gm_box_dist2(mk3(s.x, s.y, s.z), wlo, whi) <= l2 * l2;
-                }
-            }
-            const unsigned mask = __ballot_sync(0xffffffffu, pass);
-            const int cnt = __popc(mask);
-            if (pass) {
-                const int at = __popc(mask & ((1u << lane) - 1u));
-                const float4 *tp = m.tri_s + 3 * (size_t)k;
-                S.sph[at] = s;
-                S.kk[at] = k;
-                S.tri[at][0] = __ldg(tp); S.tri[at][1] = __ldg(tp + 1); S.tri[at][2] = __ldg(tp + 2);
-            }
-            __syncwarp();
-            if (lane < cnt) lane_test(S.kk[lane], S.sph[lane], &S.tri[lane][0]);
-            merge();
-            sbA = best > 0.f ? best * rsqrtf(best) * 1.00001f + tol : tol;
-            ubA = fminf(ubA, sbA);
-            __syncwarp();
-        }
-    } else {
-        for (int k = lane; k < m.F; k += 32) lane_test(k, __ldg(m.sph_s + k), m.tri_s + 3 * (size_t)k);
-        merge();
-    }
-    if (lane == 0) {
-        out_d[i] = best;
-        if (out_f) out_f[i] = bi;
+    const float tol = 1e-6f * sc;
+    NearestFace<1> nf(p, tol, 1e-7f * sc * sc);
+    // one point: the warp's box is the point inflated by tol, its radius tol
+    tree_nearest(m, smem[threadIdx.x >> 5], nf, p, tol, make_float4(p.x - tol, p.y - tol, p.z - tol, 0.f),
+                 make_float4(p.x + tol, p.y + tol, p.z + tol, 0.f));
+    if ((threadIdx.x & 31) == 0) {
+        out_d[i] = nf.best;
+        if (out_f) out_f[i] = nf.bi;
     }
 }
 

@@ -6,23 +6,17 @@
 //   barycentric_coordinates_of_projection + the four gathers -> cmap / normal / vis
 //
 // Design (DESIGN.md 4.2): one WARP per group of PPW query points (32 Morton-adjacent lattice points on the dense grid).
-//   nearest face  (A) greedy descent of the implicit 4-ary AABB tree over Morton-sorted faces (icon_smpl_prepare) to
-//                 the leaf nearest the warp centre: a first bound for every lane; (B) breadth-first cull of the
-//                 tree, 32 child boxes per step, ballot-compacted into a 16-bit frontier in shared memory, against
-//                 the warp's bound; (C) the surviving leaves' faces are culled 32 at a time by bounding sphere, and
-//                 every lane tests the survivors against ITS OWN best through two cheap lower bounds (sphere,
-//                 support function) before the exact Ericson distance.  A subtree / face is skipped only when its
-//                 bound is strictly farther than the current best (float slack on every bound); ties resolve to
-//                 the lowest ORIGINAL face index, exactly like the brute-force scan.
-//                 Dense lattices (PPW = 32) replace A and B by a per-body leaf list of the warp's brick (32^3 bricks
-//                 over [-1,1]^3, built by the body's first dense call), sorted by distance, so C can stop early.
+//   nearest face  the tree walk of face_tree.cuh over the body's tree (icon_smpl_prepare), descending towards the
+//                 warp centre, with a 16-bit frontier and the fixed slacks of coordinates of magnitude ~1.
+//                 Dense lattices (PPW = 32) replace its phases A and B by a per-body leaf list of the warp's brick
+//                 (32^3 bricks over [-1,1]^3, built by the body's first dense call), sorted by distance, so phase C
+//                 can stop early.
 //   sign          the faces listed in the point's yz cell (256 x 256 grid over the mesh's yz
 //                 box) are the only ones a +x ray can hit; each is tested with the same
 //                 Moller-Trumbore code as the brute-force scan, so the hit COUNT is identical.
 // Results are identical to brute force over all faces (icon_sdf_bruteforce, the CPU oracle):
 // the pruning is conservative and the per-face arithmetic is the same code (geom.cuh).
 #include <float.h>
-#include <stdlib.h>
 
 #include <algorithm>
 #include <mutex>
@@ -30,6 +24,7 @@
 #include <unordered_set>
 
 #include "common.cuh"
+#include "face_tree.cuh"
 #include "geom.cuh"
 
 namespace icon {
@@ -92,13 +87,6 @@ constexpr int NBIN = NBIN_AX * NBIN_AX * NBIN_AX;
 // lists, and the smaller footprint lets more warps be resident to hide the tree walk's dependent loads
 __host__ __device__ constexpr int fr_cap(int ppw) { return ppw >= 16 ? 1024 : (ppw >= 4 ? 768 : 384); }
 
-__device__ __forceinline__ float box_dist2(V3 p, float4 lo, float4 hi) {
-    float dx = fmaxf(fmaxf(lo.x - p.x, p.x - hi.x), 0.f);
-    float dy = fmaxf(fmaxf(lo.y - p.y, p.y - hi.y), 0.f);
-    float dz = fmaxf(fmaxf(lo.z - p.z, p.z - hi.z), 0.f);
-    return fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-}
-
 __device__ __forceinline__ unsigned spread7(unsigned v) {      // <= 10 bits -> every third bit
     v = (v | (v << 16)) & 0x030000FFu;
     v = (v | (v << 8)) & 0x0300F00Fu;
@@ -153,15 +141,6 @@ __global__ void k_points_scatter(const int32_t *__restrict__ bid, int64_t N, con
     }
 }
 
-__device__ __forceinline__ float warp_max(float v) {
-    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ float warp_min(float v) {
-    for (int o = 16; o; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-
 #ifdef ICON_SDF_STATS
 __device__ unsigned long long g_stats[8];   // warps, overflow warps, sum leaves, sum faces, sum exact tests, sum ray tests
 #define STAT(i, v) do { if (lane == 0) atomicAdd(&g_stats[i], (unsigned long long)(v)); } while (0)
@@ -169,19 +148,11 @@ __device__ unsigned long long g_stats[8];   // warps, overflow warps, sum leaves
 #define STAT(i, v) do { } while (0)
 #endif
 
-struct ChunkSmem {
-    float4 sph[32];                    // bounding spheres of the surviving faces of the current chunk (compacted)
-    float4 tri[32][3];                 // their (a, ab, ac) records
-    int kk[32];                        // their sorted positions
-};
-template <int FR_CAP>
-struct WarpSmem : ChunkSmem {
-    unsigned short fr[2][FR_CAP];      // node / leaf ids (leaf count <= 65535 is checked by the host)
-};
-// the brick path reads its leaf list from global memory and needs no frontier (a third of the shared memory; at 64
-// registers per thread, registers then bound residency at 32 warps per SM)
+// 16-bit frontier ids: icon_smpl_prepare checks that the leaf count is <= 65535.  The brick path reads its leaf list
+// from global memory and needs no frontier (a third of the shared memory; at 64 registers per thread, registers then
+// bound residency at 32 warps per SM)
 template <int PPW, bool BRICK>
-using SdfSmem = typename std::conditional<BRICK, ChunkSmem, WarpSmem<fr_cap(PPW)>>::type;
+using SdfSmem = typename std::conditional<BRICK, ChunkSmem, WalkSmem<unsigned short, fr_cap(PPW)>>::type;
 template <int PPW, bool BRICK>
 constexpr size_t sdf_smem_bytes() { return sizeof(SdfSmem<PPW, BRICK>) * (SW_T / 32); }
 
@@ -204,13 +175,6 @@ __device__ __forceinline__ float leaf_key(const MeshView &m, int l, float4 lo, f
     return fmaf(gz, gz, fmaf(gy, gy, gx * gx));
 }
 
-__device__ __forceinline__ float box_far2(V3 p, float4 lo, float4 hi) {   // squared distance to the farthest corner
-    float dx = fmaxf(fabsf(lo.x - p.x), fabsf(hi.x - p.x));
-    float dy = fmaxf(fabsf(lo.y - p.y), fabsf(hi.y - p.y));
-    float dz = fmaxf(fabsf(lo.z - p.z), fabsf(hi.z - p.z));
-    return fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-}
-
 // PPW = query points per warp; each point is replicated on REP = 32/PPW lanes which split the candidate faces
 // (and the ray list) between them and merge by shuffle.  32: one point per lane, for dense sets where 32 Morton-
 // consecutive points fill a small box.  8 / 1: for the engine's sparse refinement sets, where 32 consecutive points
@@ -222,10 +186,9 @@ __device__ __forceinline__ float box_far2(V3 p, float4 lo, float4 hi) {   // squ
 template <int PPW, bool BRICK>
 __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, const float4 *__restrict__ xyz4,
                                          const int32_t *__restrict__ perm, int64_t N, const MeshView &m,
-                                         float *__restrict__ rec, int32_t *__restrict__ face, int order,
+                                         float *__restrict__ rec, int32_t *__restrict__ face,
                                          int32_t *__restrict__ defer, int32_t *__restrict__ ndefer) {
     constexpr int REP = 32 / PPW;
-    constexpr int FR_CAP = fr_cap(PPW);
     const int lane = threadIdx.x & 31;
     const int sub = lane % PPW, rep_id = lane / PPW;           // which point of the warp, which replica
     const int64_t pos0 = wid * PPW;
@@ -244,16 +207,13 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
     const float4 whi = make_float4(warp_max(p.x) + 1e-6f, warp_max(p.y) + 1e-6f, warp_max(p.z) + 1e-6f, 0.f);
     const MeshHeader h = *m.hdr;
 
-    float best = FLT_MAX;
-    int bi = 0x7fffffff;
-    float ubw2;                                               // bound on d(lane, its nearest face), all lanes
-    int cur = 0, n = 1;                                       // tree path: frontier buffer and length
-    bool overflow = false;
-    int b = 0;                                                // brick path: the warp's brick and its box
-    float4 blo, bhi;
+    // the body lies in [-1.5, 1.5]^3 and the points that matter in [-1, 1]^3: the walk's fixed slacks
+    NearestFace<PPW> nf(p, 1e-6f, 1e-7f);
     if constexpr (BRICK) {
         bool ok = h.brick_built && !h.brick_overflow && c.x >= -1.f && c.x < 1.f && c.y >= -1.f && c.y < 1.f &&
                   c.z >= -1.f && c.z < 1.f;
+        int b = 0;
+        float4 blo, bhi;
         if (ok) {
             const int bx = min(BRICK_AX - 1, (int)((c.x + 1.f) * (BRICK_AX * 0.5f)));
             const int by = min(BRICK_AX - 1, (int)((c.y + 1.f) * (BRICK_AX * 0.5f)));
@@ -267,214 +227,27 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
             return;
         }
         const int f = __ldg(m.bface + b);
-        const Tri tr = load_tri(m.tri + 3 * (size_t)f);
-        best = tri_sqdist(p, tr.a, tr.ab, tr.ac);
-        bi = f;
-        ubw2 = fminf(warp_max(sqrtf(best)), __ldg(m.bub + b));
+        nf.try_face(m.tri + 3 * (size_t)f, f);                // not taken if NaN here; the brick's bound still holds
+        nf.start_scan(fminf(warp_max(sqrtf(nf.best)), __ldg(m.bub + b)));
         STAT(0, 1);
+        // the list is sorted by box distance to the brick, which bounds from below every lane's distance to the
+        // leaf's faces: once a step's first leaf is farther than the loosest lane bound, so is the rest of the list
+        const int o1 = __ldg(m.boff + b + 1);
+        for (int base = __ldg(m.boff + b); base < o1; base += 8) {
+            const int slot = base + (lane >> 2);
+            const int leaf = slot < o1 ? (int)__ldg(m.blist + slot) : -1;
+            float key = 0.f;
+            if (lane == 0) key = leaf_key(m, leaf, blo, bhi);
+            if (__shfl_sync(0xffffffffu, key, 0) > nf.ub * nf.ub) break;
+            STAT(2, min(8, o1 - base));
+            nf.chunk(m, S, leaf, wlo, whi);
+        }
+        nf.merge();
     } else {
-        auto try_face = [&](int k) {                             // exact test of sorted face k for this lane
-            const Tri tr = load_tri(m.tri_s + 3 * (size_t)k);
-            const float d = tri_sqdist(p, tr.a, tr.ab, tr.ac);
-            const int f = __ldg(m.order + k);
-            if (d < best || (d == best && f < bi)) { best = d; bi = f; }
-        };
-
-        // ---- phase A: greedy descent towards the warp centre -> a first bound for every lane
-        {
-            int node = 0;
-            for (int lvl = m.nlevels - 1; lvl > 0; --lvl) {
-                const int ch = 4 * node + (lane & 3);
-                float a = FLT_MAX;
-                int ai = ch;
-                if (ch < m.lvl_cnt[lvl - 1]) {
-                    const float4 *nb = m.nodes + 2 * ((size_t)m.lvl_off[lvl - 1] + ch);
-                    a = box_dist2(c, __ldg(nb), __ldg(nb + 1));
-                }
-                for (int o = 1; o <= 2; o <<= 1) {               // min over the 4 children (lanes 4j..4j+3)
-                    const float ob = __shfl_xor_sync(0xffffffffu, a, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, ai, o);
-                    if (ob < a || (ob == a && oi < ai)) { a = ob; ai = oi; }
-                }
-                node = __shfl_sync(0xffffffffu, ai, 0);
-            }
-            for (int k = 4 * node; k < min(4 * node + 4, m.F); ++k) try_face(k);
-        }
-        const float ubw = warp_max(sqrtf(best));                  // every lane's nearest is within ubw
-        ubw2 = ubw;
-        float ub2 = (ubw2 * 1.00001f + 1e-6f) * (ubw2 * 1.00001f + 1e-6f);
-
-        // ---- phase B: breadth-first cull of the tree, 32 child boxes per step.  The bound also
-        //      tightens on the way down: some face lies within the nearest far-corner distance of c,
-        //      so every lane's nearest face is within that + 2 rw of c.
-        if (lane == 0) S.fr[0][0] = 0;
-        __syncwarp();
-        for (int lvl = m.nlevels - 1; lvl > 0 && !overflow; --lvl) {
-            int nn = 0;
-            float far2 = FLT_MAX;
-            const int ccnt = m.lvl_cnt[lvl - 1];
-            const float4 *nodes = m.nodes + 2 * (size_t)m.lvl_off[lvl - 1];
-            for (int base = 0; base < n; base += 8) {
-                const int slot = base + (lane >> 2);
-                bool pass = false;
-                int ch = 0;
-                if (slot < n) {
-                    ch = 4 * (int)S.fr[cur][slot] + (lane & 3);
-                    if (ch < ccnt) {
-                        const float4 lo = __ldg(nodes + 2 * (size_t)ch), hi = __ldg(nodes + 2 * (size_t)ch + 1);
-                        // distance between the node's box and the warp's box bounds every lane's distance to the node
-                        const float gx = fmaxf(fmaxf(lo.x - whi.x, wlo.x - hi.x), 0.f);
-                        const float gy = fmaxf(fmaxf(lo.y - whi.y, wlo.y - hi.y), 0.f);
-                        const float gz = fmaxf(fmaxf(lo.z - whi.z, wlo.z - hi.z), 0.f);
-                        pass = fmaf(gz, gz, fmaf(gy, gy, gx * gx)) <= ub2;
-                        far2 = fminf(far2, box_far2(c, lo, hi));
-                    }
-                }
-                const unsigned mask = __ballot_sync(0xffffffffu, pass);
-                const int at = nn + __popc(mask & ((1u << lane) - 1u));
-                if (pass && at < FR_CAP) S.fr[cur ^ 1][at] = (unsigned short)ch;
-                nn += __popc(mask);
-            }
-            if (nn > FR_CAP) overflow = true;
-            n = nn;
-            cur ^= 1;
-            // some face lies within the nearest far-corner distance of c -> within that + rw of every lane
-            const float l2 = sqrtf(warp_min(far2)) + rw;
-            if (l2 < ubw2) { ubw2 = l2; ub2 = (ubw2 * 1.00001f + 1e-6f) * (ubw2 * 1.00001f + 1e-6f); }
-            __syncwarp();
-        }
-        // ---- near-first order of the surviving leaves.  The lanes' bounds only tighten while faces are tested, and the
-        //      warp-level cull of a chunk uses the LOOSEST lane bound: leaves that can beat even the tightest current
-        //      bound (box distance <= min over lanes of sqrt(best)) go first, so that the bounds are (nearly) final
-        //      before the long tail of barely-surviving leaves is looked at -- most of the tail then fails the one
-        //      warp-level test instead of 32 per-lane tests.  Order does not affect results (ties: lowest face index).
-        if (order && !overflow && n > 8) {
-            const float ubmin = warp_min(best * rsqrtf(fmaxf(best, 1e-30f))) * 1.00001f + 1e-6f;
-            const float t2 = ubmin * ubmin;
-            int n1 = 0, n2 = 0;
-            for (int base = 0; base < n; base += 32) {
-                const int slot = base + lane;
-                const bool valid = slot < n;
-                int leaf = 0;
-                bool near = false;
-                if (valid) {
-                    leaf = (int)S.fr[cur][slot];
-                    const float4 lo = __ldg(m.nodes + 2 * (size_t)leaf), hi = __ldg(m.nodes + 2 * (size_t)leaf + 1);
-                    const float gx = fmaxf(fmaxf(lo.x - whi.x, wlo.x - hi.x), 0.f);
-                    const float gy = fmaxf(fmaxf(lo.y - whi.y, wlo.y - hi.y), 0.f);
-                    const float gz = fmaxf(fmaxf(lo.z - whi.z, wlo.z - hi.z), 0.f);
-                    near = fmaf(gz, gz, fmaf(gy, gy, gx * gx)) <= t2;
-                }
-                const unsigned mn = __ballot_sync(0xffffffffu, valid && near), mf = __ballot_sync(0xffffffffu, valid && !near);
-                const unsigned lt = (1u << lane) - 1u;
-                if (valid && near) S.fr[cur ^ 1][n1 + __popc(mn & lt)] = (unsigned short)leaf;
-                if (valid && !near) S.fr[cur ^ 1][n - 1 - (n2 + __popc(mf & lt))] = (unsigned short)leaf;
-                n1 += __popc(mn); n2 += __popc(mf);
-            }
-            cur ^= 1;
-            __syncwarp();
-        }
-        STAT(0, 1); STAT(1, overflow ? 1 : 0); STAT(2, n);
+        const int n = tree_nearest(m, S, nf, c, rw, wlo, whi);
+        STAT(0, 1); STAT(1, n > fr_cap(PPW) ? 1 : 0); STAT(2, n);
     }
-    // ---- phases C+D: 32 faces (8 leaves) at a time: cull by bounding sphere against the warp's box and bound,
-    //      stage the survivors (sphere + triangle) compacted in shared memory, then every lane tests them against
-    //      its own best through two cheap lower bounds (bounding sphere, then the support-function bound
-    //      d >= |w| - max_k u.(v_k - c_f), u = w/|w|, w = p - c_f, nearly exact for faces seen head-on) before
-    //      the exact distance.
-    {
-        float sbA = best * rsqrtf(best) * 1.00001f + 1e-6f;    // ~sqrt(best), inflated; bounds only
-        float ubA = ubw2 * 1.00001f + 1e-6f;
-        // `tr` points at the face's three float4 (a, ab, ac); it is only dereferenced once the sphere test passes
-        auto lane_test = [&](int k, float4 s, const float4 *tr) {
-            const float dx = p.x - s.x, dy = p.y - s.y, dz = p.z - s.z;
-            const float dd = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-            const float l = sbA + s.w;
-            if (dd > l * l) return;                            // sphere bound beats this lane's best
-            const float4 r0 = tr[0], r1 = tr[1], r2 = tr[2];
-            const V3 ab = mk3(r0.w, r1.x, r1.y), ac = mk3(r1.z, r1.w, r2.x);
-            const float S1 = fmaf(dz, ab.z, fmaf(dy, ab.y, dx * ab.x));
-            const float T1 = fmaf(dz, ac.z, fmaf(dy, ac.y, dx * ac.x));
-            const float M = fmaxf(fmaxf(-(S1 + T1), fmaf(2.f, S1, -T1)), fmaf(2.f, T1, -S1)) * (1.f / 3.f);
-            const float g = dd - M - 1e-7f;                    // |w|^2 - |w| h(u)
-            if (g > 0.f && g * g > best * dd * 1.0001f) return;   // support bound beats this lane's best
-            const float d = tri_sqdist(p, mk3(r0.x, r0.y, r0.z), ab, ac);
-            if (d > best) return;
-            const int f = __ldg(m.order + k);
-            if (d < best || f < bi) {
-                best = d; bi = f;
-                sbA = d * rsqrtf(d) * 1.00001f + 1e-6f;
-                if (!(d > 0.f)) sbA = 1e-6f;
-            }
-        };
-        // one step: this lane's slot holds `leaf` (-1: none), 4 lanes per leaf, 8 leaves = 32 faces
-        auto chunk = [&](int leaf) {
-            bool pass = false;
-            int k = 0;
-            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (leaf >= 0) {
-                k = 4 * leaf + (lane & 3);
-                if (k < m.F) {
-                    s = __ldg(m.sph_s + k);
-                    const float l2 = ubA + s.w;                // sphere vs the warp's box: some lane may be that close
-                    pass = box_dist2(mk3(s.x, s.y, s.z), wlo, whi) <= l2 * l2;
-                }
-            }
-            const unsigned mask = __ballot_sync(0xffffffffu, pass);
-            const int cnt = __popc(mask);
-            STAT(3, cnt);
-            if (pass) {
-                const int at = __popc(mask & ((1u << lane) - 1u));
-                const float4 *tp = m.tri_s + 3 * (size_t)k;
-                S.sph[at] = s;
-                S.kk[at] = k;
-                S.tri[at][0] = __ldg(tp); S.tri[at][1] = __ldg(tp + 1); S.tri[at][2] = __ldg(tp + 2);
-            }
-            __syncwarp();
-            for (int j = rep_id; j < cnt; j += REP) lane_test(S.kk[j], S.sph[j], &S.tri[j][0]);
-            if (REP > 1) {                                      // replicas of a point share their best
-#pragma unroll
-                for (int o = PPW; o < 32; o <<= 1) {
-                    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                    if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-                }
-                sbA = best > 0.f ? best * rsqrtf(best) * 1.00001f + 1e-6f : 1e-6f;
-            }
-            ubA = fminf(ubA, warp_max(sbA));                   // the lanes' bounds only shrink: cull the next chunk harder
-            __syncwarp();
-        };
-        if constexpr (BRICK) {
-            // the list is sorted by box distance to the brick, which bounds from below every lane's distance to the
-            // leaf's faces: once a step's first leaf is farther than the loosest lane bound, so is the rest of the list
-            const int o1 = __ldg(m.boff + b + 1);
-            for (int base = __ldg(m.boff + b); base < o1; base += 8) {
-                const int slot = base + (lane >> 2);
-                const int leaf = slot < o1 ? (int)__ldg(m.blist + slot) : -1;
-                float key = 0.f;
-                if (lane == 0) key = leaf_key(m, leaf, blo, bhi);
-                if (__shfl_sync(0xffffffffu, key, 0) > ubA * ubA) break;
-                STAT(2, min(8, o1 - base));
-                chunk(leaf);
-            }
-        } else if (!overflow) {
-            for (int base = 0; base < n; base += 8) {
-                const int slot = base + (lane >> 2);
-                chunk(slot < n ? (int)S.fr[cur][slot] : -1);
-            }
-        } else {
-            for (int k = rep_id; k < m.F; k += REP) {
-                lane_test(k, __ldg(m.sph_s + k), m.tri_s + 3 * (size_t)k);
-            }
-        }
-        if (REP > 1) {                                          // final merge over the replicas (ties: lowest face id)
-#pragma unroll
-            for (int o = PPW; o < 32; o <<= 1) {
-                const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-            }
-        }
-    }
+    STAT(3, nf.staged);
     // ---- +x ray parity
     int hits = 0;
     if (!h.ray_overflow) {
@@ -499,7 +272,7 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
 #pragma unroll
         for (int o = PPW; o < 32; o <<= 1) hits += __shfl_xor_sync(0xffffffffu, hits, o);
     }
-    if (live && rep_id == 0) emit_record(p, bi, best, hits, m, rec, face, idx);
+    if (live && rep_id == 0) emit_record(p, nf.bi, nf.best, hits, m, rec, face, idx);
 }
 
 // Without `defer`, warp i of the grid takes the points of warp i.  BRICK appends the warps it leaves to the tree walk
@@ -507,7 +280,7 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
 template <int PPW, bool BRICK>
 __global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xyz4, const int32_t *__restrict__ perm,
                                                    int64_t N, MeshView m, float *__restrict__ rec,
-                                                   int32_t *__restrict__ face, int order, int32_t *__restrict__ defer,
+                                                   int32_t *__restrict__ face, int32_t *__restrict__ defer,
                                                    int32_t *__restrict__ ndefer) {
     static_assert(!BRICK || PPW == 32, "brick lists serve dense lattices: 32 points per warp");
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -515,7 +288,7 @@ __global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xy
     const bool listed = !BRICK && defer != nullptr;
     const int64_t nw = listed ? (int64_t)*ndefer : (N + PPW - 1) / PPW;
     for (int64_t i = (int64_t)blockIdx.x * (SW_T / 32) + (threadIdx.x >> 5); i < nw; i += (int64_t)gridDim.x * (SW_T / 32))
-        sdf_warp<PPW, BRICK>(listed ? (int64_t)defer[i] : i, S, xyz4, perm, N, m, rec, face, order, defer, ndefer);
+        sdf_warp<PPW, BRICK>(listed ? (int64_t)defer[i] : i, S, xyz4, perm, N, m, rec, face, defer, ndefer);
 }
 
 // ---------------------------------------------------------------- brick leaf lists (built once per body)
@@ -627,7 +400,6 @@ __global__ void __launch_bounds__(256) k_sdf_brute(const float *__restrict__ pts
 
 // points-per-warp policy of k_sdf_warp (see its header comment); icon_set_sdf_policy() overrides it for tuning
 static int64_t g_sdf_ppw32_from = 6000000, g_sdf_ppw8_from = 300000;
-static int g_sdf_order = -1;          // near-first leaf order: experimental, OFF unless ICON_B200_SDF_ORDER=1
 static int g_sdf_ppw_force = 0;
 static int g_sdf_bricks = 1;              // brick leaf lists on PPW = 32 calls (icon_set_sdf_bricks)
 static int64_t g_brick_max_entries = 0;   // > 0: a build may use at most this many list entries
@@ -671,7 +443,7 @@ static int build_bricks(const MeshView &m, cudaStream_t stream) {
     k_brick_centres<<<NBRICK / 256, 256, 0, stream>>>(m);
     ICON_LAUNCHED();
     k_sdf_warp<1, false><<<NBRICK / (SW_T / 32), SW_T, sdf_smem_bytes<1, false>(), stream>>>(
-        m.bxyz, m.bperm, NBRICK, m, m.brec, m.bface, 0, nullptr, nullptr);
+        m.bxyz, m.bperm, NBRICK, m, m.brec, m.bface, nullptr, nullptr);
     ICON_LAUNCHED();
     k_brick_count<<<NBRICK, 128, 0, stream>>>(m);
     ICON_LAUNCHED();
@@ -732,15 +504,11 @@ int run_sdf(const float *points, int64_t sc, int64_t sn, int64_t N, const float 
     // the point count alone cannot tell the two apart -- callers that know can pin it (icon_set_sdf_policy).
     int ppw = N >= g_sdf_ppw32_from ? 32 : (N >= g_sdf_ppw8_from ? 8 : 1);
     if (g_sdf_ppw_force) ppw = g_sdf_ppw_force;
-    if (g_sdf_order < 0) {
-        const char *e = getenv("ICON_B200_SDF_ORDER");
-        g_sdf_order = (e && e[0] == '1') ? 1 : 0;
-    }
     const int wpb = SW_T / 32;
     const int64_t nwarps = (N + ppw - 1) / ppw;
     const unsigned nblk_w = (unsigned)((nwarps + wpb - 1) / wpb);
 #define ICON_SDF_LAUNCH(P) k_sdf_warp<P, false><<<nblk_w, SW_T, sdf_smem_bytes<P, false>(), stream>>>( \
-        w.xyz4, w.perm, N, m, rec, face, g_sdf_order, nullptr, nullptr)
+        w.xyz4, w.perm, N, m, rec, face, nullptr, nullptr)
     if (ppw == 32 && g_sdf_bricks) {
         // dense call: the brick lists of this body, built by its first dense call, then the brick path and the tree
         // walk over the warps it leaves (those straddling bricks or outside the cube; all of them if the lists
@@ -758,11 +526,11 @@ int run_sdf(const float *points, int64_t sc, int64_t sn, int64_t N, const float 
         }
         ICON_CUDA(cudaMemsetAsync(w.ndefer, 0, sizeof(int32_t), stream));
         k_sdf_warp<32, true><<<nblk_w, SW_T, sdf_smem_bytes<32, true>(), stream>>>(
-            w.xyz4, w.perm, N, m, rec, face, g_sdf_order, w.defer, w.ndefer);
+            w.xyz4, w.perm, N, m, rec, face, w.defer, w.ndefer);
         ICON_LAUNCHED();
         const unsigned nblk_d = (unsigned)std::min<int64_t>(nblk_w, (int64_t)device_sm_count() * 16);
         k_sdf_warp<32, false><<<nblk_d, SW_T, sdf_smem_bytes<32, false>(), stream>>>(
-            w.xyz4, w.perm, N, m, rec, face, g_sdf_order, w.defer, w.ndefer);
+            w.xyz4, w.perm, N, m, rec, face, w.defer, w.ndefer);
     } else {
         switch (ppw) {
             case 32: ICON_SDF_LAUNCH(32); break;

@@ -10,25 +10,15 @@
 #include <float.h>
 
 #include "common.cuh"
+#include "face_tree.cuh"
 #include "geom.cuh"
 
 namespace icon {
 
-static void bvh_levels(int F, int &nlevels, int *cnt, int *off) {
-    int n = (F + 3) / 4, l = 0, o = 0;
-    while (true) {
-        cnt[l] = n; off[l] = o; o += n; ++l;
-        if (n == 1 || l == BVH_MAX_LEVELS) break;
-        n = (n + 3) / 4;
-    }
-    nlevels = l;
-}
-
 static MeshView carve_mesh(Carver &c, int V, int F) {
     MeshView m{};
-    m.V = V; m.F = F;
-    bvh_levels(F, m.nlevels, m.lvl_cnt, m.lvl_off);
-    const size_t total_nodes = (size_t)m.lvl_off[m.nlevels - 1] + m.lvl_cnt[m.nlevels - 1];
+    m.V = V;
+    const size_t total_nodes = tree_levels(m, F);
     m.tri = c.take<float4>((size_t)F * 3);
     m.sph = c.take<float4>((size_t)F);
     m.attr = c.take<float4>((size_t)F * 6);
@@ -105,14 +95,6 @@ __global__ void __launch_bounds__(128) k_vertex_normals(const float *__restrict_
     out[3 * v + 2] = sz / nrm;
 }
 
-__device__ __forceinline__ unsigned expand10(unsigned v) {
-    v = (v * 0x00010001u) & 0xFF0000FFu;
-    v = (v * 0x00000101u) & 0x0F00F00Fu;
-    v = (v * 0x00000011u) & 0xC30C30C3u;
-    v = (v * 0x00000005u) & 0x49249249u;
-    return v;
-}
-
 __global__ void k_face_records(const float *__restrict__ verts, const int64_t *__restrict__ faces,
                                const float *__restrict__ vnormals, const float *__restrict__ cmap,
                                const float *__restrict__ vis, int F, float4 *__restrict__ tri,
@@ -124,17 +106,7 @@ __global__ void k_face_records(const float *__restrict__ verts, const int64_t *_
     V3 a = mk3(verts[3 * i0], verts[3 * i0 + 1], verts[3 * i0 + 2]);
     V3 b = mk3(verts[3 * i1], verts[3 * i1 + 1], verts[3 * i1 + 2]);
     V3 c = mk3(verts[3 * i2], verts[3 * i2 + 1], verts[3 * i2 + 2]);
-    V3 ab = sub3(b, a), ac = sub3(c, a);
-    // bounding sphere (centroid, max corner distance, inflated): only a conservative lower bound
-    // for pruning, never the reported distance
-    V3 sc = mk3((a.x + b.x + c.x) / 3.f, (a.y + b.y + c.y) / 3.f, (a.z + b.z + c.z) / 3.f);
-    float ra = dot3(sub3(a, sc), sub3(a, sc)), rb = dot3(sub3(b, sc), sub3(b, sc)),
-          rc = dot3(sub3(c, sc), sub3(c, sc));
-    float sr = sqrtf(fmaxf(ra, fmaxf(rb, rc))) * 1.0001f + 1e-7f;
-    tri[3 * f + 0] = make_float4(a.x, a.y, a.z, ab.x);
-    tri[3 * f + 1] = make_float4(ab.y, ab.z, ac.x, ac.y);
-    tri[3 * f + 2] = make_float4(ac.z, 0.f, 0.f, 0.f);
-    sph[f] = make_float4(sc.x, sc.y, sc.z, sr);
+    const V3 sc = write_face_record(a, b, c, 1e-7f, tri + 3 * f, sph + f);
     const float *n0 = vnormals + 3 * i0, *n1 = vnormals + 3 * i1, *n2 = vnormals + 3 * i2;
     const float *m0 = cmap + 3 * i0, *m1 = cmap + 3 * i1, *m2 = cmap + 3 * i2;
     attr[6 * f + 0] = make_float4(n0[0], n0[1], n0[2], n1[0]);
@@ -146,10 +118,8 @@ __global__ void k_face_records(const float *__restrict__ verts, const int64_t *_
     rbox[2 * f + 0] = make_float4(fminf(a.y, fminf(b.y, c.y)), fmaxf(a.y, fmaxf(b.y, c.y)),
                                   fminf(a.z, fminf(b.z, c.z)), fmaxf(a.z, fmaxf(b.z, c.z)));
     rbox[2 * f + 1] = make_float4(fmaxf(a.x, fmaxf(b.x, c.x)), fminf(a.x, fminf(b.x, c.x)), 0.f, 0.f);
-    // 30-bit Morton code of the centroid over [-1.5, 1.5]^3
-    auto qz = [](float v) { return (unsigned)fminf(fmaxf((v + 1.5f) * (1024.f / 3.f), 0.f), 1023.f); };
-    unsigned code = (expand10(qz(sc.x)) << 2) | (expand10(qz(sc.y)) << 1) | expand10(qz(sc.z));
-    keys[f] = ((unsigned long long)code << 32) | (unsigned)f;
+    // Morton code of the centroid over [-1.5, 1.5]^3
+    keys[f] = ((unsigned long long)morton30(sc, mk3(-1.5f, -1.5f, -1.5f), 1024.f / 3.f) << 32) | (unsigned)f;
 }
 
 // rank sort: F is ~1e4, so F^2 comparisons from shared memory are cheaper than a radix sort's passes
@@ -182,36 +152,12 @@ __global__ void k_sorted_copy(const int32_t *__restrict__ order, const float4 *_
     sph_s[p] = s;
 }
 
-__global__ void __launch_bounds__(1024) k_build_tree(const float4 *__restrict__ tri_s, MeshView m) {
-    // level 0: leaf = 4 consecutive sorted faces
-    for (int n = threadIdx.x; n < m.lvl_cnt[0]; n += blockDim.x) {
-        float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
-        for (int t = 4 * n; t < min(4 * n + 4, m.F); ++t) {
-            Tri tr = load_tri(tri_s + 3 * (size_t)t);
-            const V3 vs[3] = {tr.a, mk3(tr.a.x + tr.ab.x, tr.a.y + tr.ab.y, tr.a.z + tr.ab.z),
-                              mk3(tr.a.x + tr.ac.x, tr.a.y + tr.ac.y, tr.a.z + tr.ac.z)};
-            for (int k = 0; k < 3; ++k) {
-                lo[0] = fminf(lo[0], vs[k].x); hi[0] = fmaxf(hi[0], vs[k].x);
-                lo[1] = fminf(lo[1], vs[k].y); hi[1] = fmaxf(hi[1], vs[k].y);
-                lo[2] = fminf(lo[2], vs[k].z); hi[2] = fmaxf(hi[2], vs[k].z);
-            }
-        }
-        m.nodes[2 * (size_t)n] = make_float4(lo[0], lo[1], lo[2], 0.f);
-        m.nodes[2 * (size_t)n + 1] = make_float4(hi[0], hi[1], hi[2], 0.f);
-    }
+__global__ void __launch_bounds__(1024) k_build_tree(MeshView m) {
+    for (int n = threadIdx.x; n < m.lvl_cnt[0]; n += blockDim.x) write_leaf_box(m, n);
     for (int l = 1; l < m.nlevels; ++l) {
         __threadfence_block();
         __syncthreads();
-        for (int n = threadIdx.x; n < m.lvl_cnt[l]; n += blockDim.x) {
-            float4 lo = make_float4(FLT_MAX, FLT_MAX, FLT_MAX, 0.f), hi = make_float4(-FLT_MAX, -FLT_MAX, -FLT_MAX, 0.f);
-            for (int c = 4 * n; c < min(4 * n + 4, m.lvl_cnt[l - 1]); ++c) {
-                float4 a = m.nodes[2 * ((size_t)m.lvl_off[l - 1] + c)], b = m.nodes[2 * ((size_t)m.lvl_off[l - 1] + c) + 1];
-                lo.x = fminf(lo.x, a.x); lo.y = fminf(lo.y, a.y); lo.z = fminf(lo.z, a.z);
-                hi.x = fmaxf(hi.x, b.x); hi.y = fmaxf(hi.y, b.y); hi.z = fmaxf(hi.z, b.z);
-            }
-            m.nodes[2 * ((size_t)m.lvl_off[l] + n)] = lo;
-            m.nodes[2 * ((size_t)m.lvl_off[l] + n) + 1] = hi;
-        }
+        for (int n = threadIdx.x; n < m.lvl_cnt[l]; n += blockDim.x) write_parent_box(m, l, n);
     }
     // ray grid frame from the root box
     __syncthreads();
@@ -294,7 +240,7 @@ extern "C" int icon_smpl_prepare(const float *verts, const int64_t *faces, const
     ICON_LAUNCHED();
     k_sorted_copy<<<(F + 127) / 128, 128, 0, stream>>>(m.order, m.tri, m.sph, F, m.tri_s, m.sph_s);
     ICON_LAUNCHED();
-    k_build_tree<<<1, 1024, 0, stream>>>(m.tri_s, m);
+    k_build_tree<<<1, 1024, 0, stream>>>(m);
     ICON_LAUNCHED();
     ICON_CUDA(cudaMemsetAsync(m.rcount, 0, sizeof(int32_t) * (RAY_GRID * RAY_GRID + 1), stream));
     k_ray_count<<<(F + 127) / 128, 128, 0, stream>>>(m);

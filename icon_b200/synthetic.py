@@ -79,6 +79,17 @@ def body_attributes(verts, seed=0):
     return cmap, vis
 
 
+def collapse_faces(faces, n=16, seed=0):
+    """A copy of `faces` with faces 0..3 and n - 4 random others collapsed to a segment (corner 1 moved onto corner 0).
+    The exact point-triangle distance to such a face is NaN (0/0) wherever (c - a).(p - a) > 0, which a nearest-face
+    search must never take; faces 0..3 have the lowest ids, so they would win the tie rule if it did."""
+    rng = np.random.RandomState(seed)
+    k = np.concatenate([np.arange(4), 4 + rng.choice(len(faces) - 4, n - 4, replace=False)])
+    out = faces.copy()
+    out[k, 1] = out[k, 0]
+    return out
+
+
 def lattice_points(res, device="cpu"):
     """Cell-centre lattice p = -1 + 2 (i + 0.5) / res per axis, x fastest; [1, res^3, 3]."""
     a = (-1.0 + 2.0 * (torch.arange(res, dtype=torch.float64) + 0.5) / res).float()

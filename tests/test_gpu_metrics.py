@@ -1,8 +1,8 @@
 """The Chamfer / P2S metric on the device (icon_b200/metrics.py, csrc/mesh_dist.cu).
 
 icon_mesh_distance against the brute-force CPU scan (oracle_mesh_distance), bit for bit in squared distance and face
-id, on a synthetic body, a decimated scan, a mesh past the SMPL path's 16-bit leaf ids and a marching-cubes surface,
-with points on and off the surface and equidistant ties; the device sampler against its NumPy restatement
+id, on a synthetic body, the same body with collapsed faces, a decimated scan, a mesh past the SMPL path's 16-bit leaf
+ids and a marching-cubes surface, with points on and off the surface and equidistant ties; the device sampler against its NumPy restatement
 (oracle/sample.py), bit for bit; chamfer_p2s against the same arithmetic in fp64 on the CPU, and on concentric
 spheres against |r1 - r2| 100.
 """
@@ -85,6 +85,9 @@ def _mc_surface(dev, R=129):
 def _mesh(name, dev):
     if name == "body":
         return S.body_mesh(rings=40, segs=44, seed=3)
+    if name == "collapsed":
+        v, f = S.body_mesh(rings=40, segs=44, seed=3)
+        return v, S.collapse_faces(f)
     if name == "scan":
         d = np.load(os.path.join(GOLDEN, "scan_body.npz"))
         return d["verts"], d["faces"].astype(np.int64)
@@ -97,7 +100,8 @@ def _mesh(name, dev):
     raise KeyError(name)
 
 
-@pytest.mark.parametrize("name,n_each", [("body", 200), ("scan", 150), ("sphere327k", 60), ("mc", 100), ("cube", 20)])
+@pytest.mark.parametrize("name,n_each", [("body", 200), ("scan", 150), ("sphere327k", 60), ("mc", 100), ("cube", 20),
+                                         ("collapsed", 100)])
 def test_mesh_distance_equals_brute_force(name, n_each):
     dev = _cuda()
     from icon_b200 import metrics
@@ -107,6 +111,8 @@ def test_mesh_distance_equals_brute_force(name, n_each):
     pts = _points(v, f, n_each, seed=7, spread=1.5)
     if name == "cube":                                                 # the centre: all 12 faces at 0.25
         pts = np.concatenate([pts, np.zeros((1, 3), np.float32), np.array([[0.0, 0.0, 0.3]], np.float32)])
+    if name == "collapsed":                                            # on and around the faces of NaN distance
+        pts = np.concatenate([pts, _points(v, f[f[:, 0] == f[:, 1]], n_each, seed=8, spread=1.5)])
     m = metrics.Mesh(v, f, device=dev)
     d, fi = m.distance(torch.from_numpy(pts).to(dev))
     rd, rf = _brute(pts, v, f)

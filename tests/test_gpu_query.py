@@ -61,7 +61,7 @@ def sdf_policy():
 
 
 @pytest.mark.parametrize("ppw", [0, 1, 2, 4, 8, 16, 32])
-@pytest.mark.parametrize("kind", ["random", "lattice", "faces_and_outside"])
+@pytest.mark.parametrize("kind", ["random", "lattice", "faces_and_outside", "collapsed"])
 def test_sdf_block_bit_exact_vs_oracle(kind, ppw, sdf_policy, mlp_impl):
     if mlp_impl != "tcgen05":
         pytest.skip("SDF block does not depend on the MLP implementation")
@@ -75,6 +75,17 @@ def test_sdf_block_bit_exact_vs_oracle(kind, ppw, sdf_policy, mlp_impl):
         a = torch.linspace(-1, 1, 21)
         z, y, x = torch.meshgrid(a, a, a, indexing="ij")
         pts = torch.stack([x, y, z], -1).reshape(1, -1, 3)       # includes the +-1 cube faces
+    elif kind == "collapsed":
+        # faces with two coincident corners (NaN distance at half the points): points on and around them, random
+        # points, and a dense 16^3 patch of 256^3-lattice spacing around face 0, whose warps take the brick lists
+        f = S.collapse_faces(faces[0].numpy())
+        faces = torch.from_numpy(f)[None]
+        k = np.nonzero(f[:, 0] == f[:, 1])[0]
+        a = torch.arange(16, dtype=torch.float32) * (2.0 / 255.0)
+        z, y, x = torch.meshgrid(a, a, a, indexing="ij")
+        patch = torch.stack([x, y, z], -1).reshape(1, -1, 3) + (verts[0, f[0, 0]] - 15.0 / 255.0)
+        pts = torch.cat([S.adversarial_points(verts[0].numpy(), f[k], n_each=200, seed=3), _points(3000, seed=3),
+                         patch], 1)
     else:
         pts = _points(3000, seed=2, spread=1.6)                   # about half outside the cube
         pts[0, :200, 0] = 1.0
