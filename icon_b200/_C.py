@@ -73,6 +73,10 @@ _SIGS = {
     "icon_voxelize": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _f, _vp, _vp, _sz, _vp]),
     "icon_visibility_workspace_bytes": (_sz, [_i]),
     "icon_visibility": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
+    "icon_vertex_normals_workspace_bytes": (_sz, [_i, _i]),
+    "icon_vertex_normals": (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "icon_normal_render_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "icon_normal_render": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "icon_mc_workspace_bytes": (_sz, [_i, _i]),
     "icon_mc_count": (_i, [_vp, _i, _f, _i, _vp, _sz, _vp, _vp]),
     "icon_mc_emit": (_i, [_vp, _i, _f, _i, _vp, _vp, _vp, _i64, _i64, _vp]),

@@ -5,6 +5,8 @@
                 samples of each mesh, proximity.closest_point (an rtree walk) measures them against the other mesh.
                 Here both meshes are prepared once (icon_mesh_prepare), sampled (icon_mesh_sample) and queried
                 (icon_mesh_distance: exact nearest face, bit-identical to brute force) by this library's kernels.
+  NC            lib/dataset/Evaluator.py:125-177 (calculate_normal_consist) stays the reference's; the overlay patch
+                (make_Evaluator) gives it a GL-free _render_normal drawn by icon_b200/normal_render.py.
 
 The arithmetic after the distances is the reference's: NaN -> 0, chamfer = 0.5 (mean pred->gt + mean gt->pred) 100,
 p2s = mean pred->gt 100, a distance being the square root of the exact squared distance (in fp64).  The samples are
@@ -111,13 +113,32 @@ def chamfer_p2s(verts_pr, faces_pr, verts_gt, faces_gt, sampled_points=1000, see
 
 
 def make_Evaluator(reference_evaluator):
-    """Overlay patch of lib.dataset.Evaluator: the reference's Evaluator class with calculate_chamfer_p2s computed
-    here from the arrays set_mesh / space_transfer hold (verts_pr / faces_pr in the SDF frame, verts_gt / faces_gt
-    projected); every other method is the reference's."""
+    """Overlay patch of lib.dataset.Evaluator: the reference's Evaluator class with three names rebound.
+
+    * calculate_chamfer_p2s: computed here from the arrays set_mesh / space_transfer hold (verts_pr / faces_pr in the
+      SDF frame, verts_gt / faces_gt projected).
+    * init_gl: stores an icon_b200.normal_render.NormalRenderer(512, 512) in Evaluator._normal_render; it opens no GL
+      context and never imports lib.renderer.
+    * _render_normal(mesh, deg, norms=None): the normal image of any object with `vertices` / `faces` (a trimesh or a
+      namespace), drawn by icon_normal_render and returned as get_color returns it (numpy float32 [H,W,4]).
+
+    Every other method is the reference's; render_normal, calculate_normal_consist, render_mesh_list and
+    _get_reproj_normal_error run unchanged on top of the patched _render_normal."""
+    from . import normal_render
+
     def calculate_chamfer_p2s(self, sampled_points=1000):
         return chamfer_p2s(self.verts_pr, self.faces_pr, self.verts_gt, self.faces_gt, sampled_points)
+
+    def init_gl():
+        reference_evaluator._normal_render = normal_render.NormalRenderer(width=512, height=512)
+
+    def _render_normal(self, mesh, deg, norms=None):
+        """Evaluator._render_normal on the device (icon_b200.normal_render.normal_image), numpy float32 [H,W,4]."""
+        return self._normal_render.render(mesh.vertices, mesh.faces, deg, self.offset, self.scale_factor, norms)
 
     calculate_chamfer_p2s.__doc__ = chamfer_p2s.__doc__
     if reference_evaluator is not None:
         reference_evaluator.calculate_chamfer_p2s = calculate_chamfer_p2s
+        reference_evaluator.init_gl = staticmethod(init_gl)
+        reference_evaluator._render_normal = _render_normal
     return reference_evaluator

@@ -5,7 +5,8 @@
     # or, with no code change at all:  ICON_B200_OVERLAY=/path/to/ICON python -m icon_b200.overlay -m apps.infer ...
 
 The reference's `lib` package stays the reference's: every module, helper and constant that is not part of the
-accelerated path (`lib.common.render`, `lib.dataset.Evaluator` but for `calculate_chamfer_p2s`, `lib.smplx`, `lib.common.config`, the rest of
+accelerated path (`lib.common.render`, `lib.dataset.Evaluator` but for `calculate_chamfer_p2s`, `init_gl` and
+`_render_normal`, `lib.smplx`, `lib.common.config`, the rest of
 `train_util` / `mesh_util` / `net_util` ...) is imported from the checkout unchanged.  An import hook on
 `sys.meta_path` then does two things, only for the modules listed below:
 
@@ -16,11 +17,14 @@ accelerated path (`lib.common.render`, `lib.dataset.Evaluator` but for `calculat
 * PATCH    -- the reference module is executed normally, then the accelerated names are rebound in its namespace
               (`query_func` in `lib/common/train_util.py`, `get_visibility` in `lib/dataset/mesh_util.py`, the
               encoder classes in `lib/net/{NormalNet,MLP,HGFilters,VE}.py`, `define_G` in `lib/net/FBNet.py`,
-              `Evaluator.calculate_chamfer_p2s` in `lib/dataset/Evaluator.py`), so
+              `Evaluator.calculate_chamfer_p2s`, `Evaluator.init_gl` and `Evaluator._render_normal` in
+              `lib/dataset/Evaluator.py`), so
               `from lib.common.train_util import *` (apps/ICON.py:20) still finds everything else it uses.
 
 Callers and call sites this serves: apps/ICON.py:17-22, 52-90 (HGPIFuNet, Seg3dLossless, query_func, get_visibility),
-apps/infer.py:22-31, apps/ICON.py:634-640 (calculate_chamfer_p2s), lib/dataset/mesh_util.py:187-237 (load_checkpoint:
+apps/infer.py:22-31, apps/ICON.py:634-640 (calculate_chamfer_p2s), apps/ICON.py:527-528, 555-558, 641-643 (init_gl,
+render_normal and calculate_normal_consist through _render_normal: no OpenGL context),
+lib/dataset/mesh_util.py:187-237 (load_checkpoint:
 identical state_dict keys),
 lib/dataset/TestDataset.py:137 (get_visibility).
 """
@@ -73,7 +77,7 @@ def _patches():
         "lib.net.HGFilters": {"HGFilter": encoders.HGFilter, "HourGlass": encoders.HourGlass},
         "lib.net.FBNet": {"define_G": make_define_G},          # callable(old value) -> new value
         "lib.net.VE": {"VolumeEncoder": encoders.VolumeEncoder, "Residual3D": encoders.Residual3D},
-        "lib.dataset.Evaluator": {"Evaluator": metrics.make_Evaluator},     # calculate_chamfer_p2s only
+        "lib.dataset.Evaluator": {"Evaluator": metrics.make_Evaluator},     # chamfer_p2s, init_gl, _render_normal
     }
 
 

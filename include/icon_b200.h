@@ -251,6 +251,24 @@ size_t icon_visibility_workspace_bytes(int image_size);
 int icon_visibility(const float *xyz, int V, const int64_t *faces, int F, int image_size, float *vis,
                     void *ws, size_t ws_bytes, icon_stream_t stream);
 
+/* ------------------------------------------------------------------ normal images of the evaluation
+ * Replace the OpenGL NormalRender behind Evaluator._render_normal (lib/dataset/Evaluator.py:58-73) and trimesh's
+ * vertex_normals it draws by default.  Rules (parity unpinned): csrc/normal_render.cu header.
+ *
+ * icon_vertex_normals: trimesh's angle-weighted vertex normals of verts [V,3] f64, faces [F,3] i64, computed in fp64
+ * and written as out [V,3] f32; bitwise reproducible (no float atomics).  Unreferenced vertices get zero. */
+size_t icon_vertex_normals_workspace_bytes(int V, int F);
+int icon_vertex_normals(const double *verts, int V, const int64_t *faces, int F, float *out, void *ws,
+                        size_t ws_bytes, icon_stream_t stream);
+/* icon_normal_render: one orthographic normal image at width x height (each <= 16384).
+ * verts [V,3] f32 (already scale_factor * vertices), norms [V,3] f32, faces [F,3] i64, h_model: HOST pointer to the
+ * 12 floats of the model matrix's first three rows.  out_rgba [height,width,4] f32 (16-byte aligned) in get_color's
+ * row order, background (1,1,1,0); out_face [height,width] i32 the drawn face (-1 background) or NULL. */
+size_t icon_normal_render_workspace_bytes(int V, int F, int width, int height);
+int icon_normal_render(const float *verts, const float *norms, int V, const int64_t *faces, int F,
+                       const float *h_model, int width, int height, float *out_rgba, int32_t *out_face,
+                       void *ws, size_t ws_bytes, icon_stream_t stream);
+
 /* ------------------------------------------------------------------ encoder operators
  * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
  * two take NCHW fp32 tensors; every 2-D convolution and normalisation runs on the NHWC path after them. */
