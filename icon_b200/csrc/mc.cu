@@ -63,8 +63,10 @@ __device__ __forceinline__ const float *mc_row(const McGrid &g, int i, int j) {
     return in ? g.occ + ((size_t)(i + g.shift) * g.R + (j + g.shift)) * g.R + g.shift : nullptr;
 }
 
-// classification of the 4 voxels (i, j, k0 .. k0+3): fl = edge-ownership bits (i, j, k axis), cs = cube case
-__device__ __forceinline__ void mc_classify4(const McGrid &g, float iso, int i, int j, int k0, unsigned fl[4], int cs[4]) {
+// classification of the 4 voxels (i, j, k0 .. k0+3): fl = edge-ownership bits (i, j, k axis), cs = cube case.
+// CT = the branch's precision (float padded, double plain): a node is below iso iff (CT)f < iso, so NaN never is
+template <typename CT>
+__device__ __forceinline__ void mc_classify4(const McGrid &g, CT iso, int i, int j, int k0, unsigned fl[4], int cs[4]) {
     const int G = g.G;
     const float *rows[4] = {mc_row(g, i, j), i + 1 < G ? mc_row(g, i + 1, j) : nullptr,
                             (i + 1 < G && j + 1 < G) ? mc_row(g, i + 1, j + 1) : nullptr,
@@ -76,7 +78,7 @@ __device__ __forceinline__ void mc_classify4(const McGrid &g, float iso, int i, 
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
 #pragma unroll
-            for (int m = 0; m < 5; ++m) nib[m] |= (__ldg(rows[r] + k0 + m) < iso) ? (1u << r) : 0u;
+            for (int m = 0; m < 5; ++m) nib[m] |= ((CT)__ldg(rows[r] + k0 + m) < iso) ? (1u << r) : 0u;
         }
     } else {
 #pragma unroll
@@ -86,7 +88,7 @@ __device__ __forceinline__ void mc_classify4(const McGrid &g, float iso, int i, 
             for (int m = 0; m < 5; ++m) {
                 const int k = k0 + m;
                 const float f = (p != nullptr && k >= g.lo && k <= g.hi) ? __ldg(p + k) : 0.f;
-                nib[m] |= (f < iso) ? (1u << r) : 0u;
+                nib[m] |= ((CT)f < iso) ? (1u << r) : 0u;
             }
         }
     }
@@ -144,7 +146,8 @@ __device__ __forceinline__ int mc_block_scan(int x, int *total) {
     return s_w[w] + inc - x;
 }
 
-__global__ void __launch_bounds__(MC_T) k_mc_count(McGrid g, McGeom q, float iso, int32_t *__restrict__ blk_v,
+template <typename CT>
+__global__ void __launch_bounds__(MC_T) k_mc_count(McGrid g, McGeom q, CT iso, int32_t *__restrict__ blk_v,
                                                    int32_t *__restrict__ blk_t, uint8_t *__restrict__ vflags,
                                                    uint8_t *__restrict__ vcase) {
     const int64_t u = (int64_t)blockIdx.x * MC_T + threadIdx.x;
@@ -180,8 +183,9 @@ __global__ void __launch_bounds__(MC_T) k_mc_count(McGrid g, McGeom q, float iso
         if (k0 + m < g.G) { vflags[v0 + m] = (uint8_t)fl[m]; vcase[v0 + m] = (uint8_t)cs[m]; }
 }
 
+// MC_T threads per block; the register cap replaces __launch_bounds__, under which ptxas spilled the fp32 variant
 template <typename VT>
-__global__ void __launch_bounds__(MC_T) k_mc_verts(McGrid g, McGeom q, float iso, const int32_t *__restrict__ blk_v,
+__global__ void __maxnreg__(64) k_mc_verts(McGrid g, McGeom q, VT iso, const int32_t *__restrict__ blk_v,
                                                    const int32_t *__restrict__ base_v,
                                                    const uint8_t *__restrict__ vflags, int32_t *__restrict__ voff,
                                                    VT *__restrict__ verts) {
@@ -211,7 +215,7 @@ __global__ void __launch_bounds__(MC_T) k_mc_verts(McGrid g, McGeom q, float iso
         for (int a = 0; a < 3; ++a) {
             if (!(fl[m] & (1u << a))) continue;
             const VT f1 = (VT)g.at(i + (a == 0), j + (a == 1), k + (a == 2));
-            const VT t = ((VT)iso - f0) / (f1 - f0);
+            const VT t = (iso - f0) / (f1 - f0);
             VT pi = (VT)i, pj = (VT)j, pk = (VT)k;
             if (a == 0) pi += t; else if (a == 1) pj += t; else pk += t;
             verts[3 * id + 0] = pk;   // x
@@ -298,7 +302,7 @@ extern "C" size_t icon_mc_workspace_bytes(int R, int padded) {
     return c.total();
 }
 
-extern "C" int icon_mc_count(const float *occ, int R, float iso, int padded, void *ws, size_t ws_bytes,
+extern "C" int icon_mc_count(const float *occ, int R, double iso, int padded, void *ws, size_t ws_bytes,
                              int64_t *d_counts, icon_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     ICON_CHECK_ARG(occ && ws && d_counts && R >= 3 && R <= 1290, "icon_mc_count: bad argument (R=%d)", R);
@@ -311,14 +315,17 @@ extern "C" int icon_mc_count(const float *occ, int R, float iso, int padded, voi
     Carver c(ws);
     McWs w = carve_mc(c, g.G);
     const McGeom q = make_geom(g.G);
-    k_mc_count<<<(unsigned)w.nblocks, MC_T, 0, stream>>>(g, q, iso, w.blk_v, w.blk_t, w.vflags, w.vcase);
+    if (padded)
+        k_mc_count<float><<<(unsigned)w.nblocks, MC_T, 0, stream>>>(g, q, (float)iso, w.blk_v, w.blk_t, w.vflags, w.vcase);
+    else
+        k_mc_count<double><<<(unsigned)w.nblocks, MC_T, 0, stream>>>(g, q, iso, w.blk_v, w.blk_t, w.vflags, w.vcase);
     ICON_LAUNCHED();
     int rc = scan_exclusive_i32(w.blk_v, w.base_v, w.nblocks, d_counts, w.scan_ws, stream);
     if (rc) return rc;
     return scan_exclusive_i32(w.blk_t, w.base_t, w.nblocks, d_counts + 1, w.scan_ws, stream);
 }
 
-extern "C" int icon_mc_emit(const float *occ, int R, float iso, int padded, const void *ws, void *verts,
+extern "C" int icon_mc_emit(const float *occ, int R, double iso, int padded, const void *ws, void *verts,
                             int64_t *faces, int64_t n_verts, int64_t n_tris, icon_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     if (n_verts == 0 && n_tris == 0) return ICON_OK;
@@ -329,7 +336,7 @@ extern "C" int icon_mc_emit(const float *occ, int R, float iso, int padded, cons
     const McGeom q = make_geom(g.G);
     if (n_verts > 0) {
         if (padded)
-            k_mc_verts<float><<<(unsigned)w.nblocks, MC_T, 0, stream>>>(g, q, iso, w.blk_v, w.base_v, w.vflags, w.voff,
+            k_mc_verts<float><<<(unsigned)w.nblocks, MC_T, 0, stream>>>(g, q, (float)iso, w.blk_v, w.base_v, w.vflags, w.voff,
                                                                         (float *)verts);
         else
             k_mc_verts<double><<<(unsigned)w.nblocks, MC_T, 0, stream>>>(g, q, iso, w.blk_v, w.base_v, w.vflags, w.voff,

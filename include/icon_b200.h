@@ -223,13 +223,14 @@ int icon_grid_count_above(const float *occ, int64_t n, float balance, int64_t *d
  * occupancys[1:,1:,1:] crop and the [:, [2,1,0]] / [:, [0,2,1]] permutations.  Indexing
  * contract: DESIGN.md "marching cubes" (oracle/mcubes.py restates it).
  *   occ [R,R,R]; padded=1 -> kaolin branch (zero pad, padded-frame coords, f32 verts),
- *   padded=0 -> PyMCubes branch (f64 verts).
+ *   padded=0 -> PyMCubes branch (f64 verts).  Each branch classifies and interpolates in its vertex precision:
+ *   f < (float)iso and fp32 t padded, (double)f < iso and fp64 t plain (PyMCubes takes the iso value as a double).
  * icon_mc_count fills ws and writes {n_verts, n_tris} to d_counts (device int64[2]);
  * icon_mc_emit writes verts [n_verts,3] (f32 or f64) and faces [n_tris,3] i64. */
 size_t icon_mc_workspace_bytes(int R, int padded);
-int icon_mc_count(const float *occ, int R, float iso, int padded, void *ws, size_t ws_bytes,
+int icon_mc_count(const float *occ, int R, double iso, int padded, void *ws, size_t ws_bytes,
                   int64_t *d_counts, icon_stream_t stream);
-int icon_mc_emit(const float *occ, int R, float iso, int padded, const void *ws, void *verts,
+int icon_mc_emit(const float *occ, int R, double iso, int padded, const void *ws, void *verts,
                  int64_t *faces, int64_t n_verts, int64_t n_tris, icon_stream_t stream);
 
 /* ------------------------------------------------------------------ PaMIR semantic voxelisation
@@ -342,9 +343,10 @@ int icon_nhwc_to_nchw(const float *x, float *y, int N, int C, int Cs, int c_off,
 int icon_stem_pack(const float *x, void *hi, void *lo, int N, int Cin, int H, int W, int Cp8, int Wp, int Hrows, int sy,
                    int reflect, icon_stream_t stream);
 /* ---- clean_mesh (csrc/clean.cu; reference lib/dataset/mesh_util.py:778-791: trimesh split + largest component).
- * faces int64 [nf][3] indexing nv vertices.  _count: union-find over the vertices, picks the component with the most
- * vertices (ties: the one containing the smallest vertex id), leaves the kept counts in d_counts[0..1] and the
- * re-index tables in `ws`; _emit writes the compacted float32 vertices / int32 faces (ascending original order). */
+ * faces int64 [nf][3] indexing nv vertices (nf < 2^28).  _count: trimesh's components (faces joined across edges used
+ * by exactly two faces), picks the one with the most distinct vertices (ties: the one with the smallest face index),
+ * leaves the kept counts in d_counts[0..1] and the re-index tables in `ws`; _emit writes the compacted float32
+ * vertices / int32 faces (ascending original order).  Deterministic: the result does not depend on block order. */
 size_t icon_clean_mesh_workspace_bytes(int64_t nv, int64_t nf);
 int icon_clean_mesh_count(const int64_t *faces, int64_t nv, int64_t nf, void *ws, size_t ws_bytes, int64_t *d_counts,
                           icon_stream_t stream);

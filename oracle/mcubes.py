@@ -22,7 +22,9 @@ contract that the CUDA kernels reproduce bit for bit:
       fastest) + axis;
     - triangles are emitted cell by cell in linear cell order (last dim fastest), and within a
       cell in triangle-table order.
-  contract "plain" (PyMCubes branch): same, without padding, fp64 coordinates.
+  contract "plain" (PyMCubes branch): same, without padding, fp64 coordinates; the iso value stays a double
+    (PyMCubes' `isovalue`), so the cube test is float64(f) < iso and t is computed in fp64 from it.
+  In both, NaN is never below iso; ±inf compare as themselves; t follows IEEE arithmetic (NaN for inf / inf).
 
 `export_mesh` then applies the reference's own `[:, [2,1,0]]` / `[:, [0,2,1]]` permutations.
 
@@ -57,17 +59,30 @@ def _edge_owner():
 _OWNER = _edge_owner()
 
 
-def marching_cubes(vol, iso=0.5, pad=True, dtype=np.float32):
-    """vol [X,Y,Z] -> (verts [Nv,3] in vol's index frame (+1 if padded), faces [Nf,3] int64)."""
+def _grid(vol, pad):
     g = np.asarray(vol, dtype=np.float32)
-    if pad:
-        g = np.pad(g, 1)
-    X, Y, Z = g.shape
-    cx, cy, cz = X - 1, Y - 1, Z - 1
-    below = g < np.float32(iso)
+    return np.pad(g, 1) if pad else g
+
+
+def cube_cases(vol, iso=0.5, pad=True, dtype=np.float32):
+    """Cube case (bit c set when corner c is below iso) of every cell of the working grid [X-1, Y-1, Z-1].  The
+    comparison runs in the output precision: fp64 iso in the PyMCubes branch, which takes it as a double; NaN is
+    never below iso."""
+    g = _grid(vol, pad)
+    cx, cy, cz = (n - 1 for n in g.shape)
+    below = g.astype(dtype) < dtype(iso)
     cube = np.zeros((cx, cy, cz), np.int32)
     for c, (dx, dy, dz) in enumerate(CORNERS):
         cube |= below[dx:dx + cx, dy:dy + cy, dz:dz + cz].astype(np.int32) << c
+    return cube
+
+
+def marching_cubes(vol, iso=0.5, pad=True, dtype=np.float32):
+    """vol [X,Y,Z] -> (verts [Nv,3] in vol's index frame (+1 if padded), faces [Nf,3] int64)."""
+    g = _grid(vol, pad)
+    X, Y, Z = g.shape
+    cx, cy, cz = X - 1, Y - 1, Z - 1
+    cube = cube_cases(vol, iso, pad, dtype)
     nv = np.asarray(NUM_VERTS, np.int32)[cube]
     act = np.flatnonzero(nv.reshape(-1))           # linear cell order, last dim fastest
     if act.size == 0:
