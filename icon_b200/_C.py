@@ -77,6 +77,10 @@ _SIGS = {
     "icon_vertex_normals": (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "icon_normal_render_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "icon_normal_render": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "icon_area_vertex_normals_workspace_bytes": (_sz, [_i, _i]),
+    "icon_area_vertex_normals": (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "icon_mesh_views_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "icon_mesh_views": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "icon_mc_workspace_bytes": (_sz, [_i, _i]),
     "icon_mc_count": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _sz, _vp, _vp]),
     "icon_mc_emit": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _vp, _vp, _i64, _i64, _vp]),

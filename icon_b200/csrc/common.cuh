@@ -109,6 +109,26 @@ struct Carver {
     size_t total() const { return align_up(off, 256); }
 };
 
+// in-place ascending heapsort of one thread's list: O(n log n) whatever its length
+__device__ __forceinline__ void heap_sift(int32_t *a, int root, int n) {
+    const int32_t x = a[root];
+    for (int c = 2 * root + 1; c < n; c = 2 * root + 1) {
+        if (c + 1 < n && a[c + 1] > a[c]) ++c;
+        if (a[c] <= x) break;
+        a[root] = a[c];
+        root = c;
+    }
+    a[root] = x;
+}
+
+__device__ __forceinline__ void heap_sort_i32(int32_t *a, int n) {
+    for (int i = n / 2 - 1; i >= 0; --i) heap_sift(a, i, n);
+    for (int m = n - 1; m > 0; --m) {
+        const int32_t t = a[0]; a[0] = a[m]; a[m] = t;
+        heap_sift(a, 0, m);
+    }
+}
+
 // ---------------------------------------------------------------- mesh workspace layout
 constexpr int TREE_MAX_LEVELS = 17;  // 4-ary implicit tree over leaves of 4 Morton-sorted faces: 4^16 leaves > 2^31 faces
 constexpr int RAY_GRID = 256;        // yz cell grid for the +x ray parity

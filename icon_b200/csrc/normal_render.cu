@@ -102,17 +102,6 @@ __global__ void k_vn_fill(const int64_t *__restrict__ faces, int F, int V, const
     for (int k = 0; k < 3; ++k) corners[off[id[k]] + atomicAdd(&cursor[id[k]], 1)] = 3 * f + k;
 }
 
-__device__ void heap_sift(int32_t *a, int root, int n) {
-    const int32_t x = a[root];
-    for (int c = 2 * root + 1; c < n; c = 2 * root + 1) {
-        if (c + 1 < n && a[c + 1] > a[c]) ++c;
-        if (a[c] <= x) break;
-        a[root] = a[c];
-        root = c;
-    }
-    a[root] = x;
-}
-
 // per vertex: sort its corner list (heapsort: O(n log n) whatever the valence), sum a_k n_f in corner order, unit
 __global__ void k_vn_sum(const int32_t *__restrict__ off, int32_t *__restrict__ corners,
                          const double *__restrict__ fdata, int V, float *__restrict__ out) {
@@ -120,11 +109,7 @@ __global__ void k_vn_sum(const int32_t *__restrict__ off, int32_t *__restrict__ 
     if (v >= V) return;
     int32_t *a = corners + off[v];
     const int n = off[v + 1] - off[v];
-    for (int i = n / 2 - 1; i >= 0; --i) heap_sift(a, i, n);
-    for (int m = n - 1; m > 0; --m) {
-        const int32_t t = a[0]; a[0] = a[m]; a[m] = t;
-        heap_sift(a, 0, m);
-    }
+    heap_sort_i32(a, n);
     double3 s = make_double3(0.0, 0.0, 0.0);
     for (int i = 0; i < n; ++i) {
         const int c = a[i];

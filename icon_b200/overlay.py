@@ -5,8 +5,8 @@
     # or, with no code change at all:  ICON_B200_OVERLAY=/path/to/ICON python -m icon_b200.overlay -m apps.infer ...
 
 The reference's `lib` package stays the reference's: every module, helper and constant that is not part of the
-accelerated path (`lib.common.render`, `lib.dataset.Evaluator` but for `calculate_chamfer_p2s`, `init_gl` and
-`_render_normal`, `lib.smplx`, `lib.common.config`, the rest of
+accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.dataset.Evaluator` but for
+`calculate_chamfer_p2s`, `init_gl` and `_render_normal`, `lib.smplx`, `lib.common.config`, the rest of
 `train_util` / `mesh_util` / `net_util` ...) is imported from the checkout unchanged.  An import hook on
 `sys.meta_path` then does two things, only for the modules listed below:
 
@@ -18,12 +18,13 @@ accelerated path (`lib.common.render`, `lib.dataset.Evaluator` but for `calculat
               (`query_func` in `lib/common/train_util.py`, `get_visibility` in `lib/dataset/mesh_util.py`, the
               encoder classes in `lib/net/{NormalNet,MLP,HGFilters,VE}.py`, `define_G` in `lib/net/FBNet.py`,
               `Evaluator.calculate_chamfer_p2s`, `Evaluator.init_gl` and `Evaluator._render_normal` in
-              `lib/dataset/Evaluator.py`), so
+              `lib/dataset/Evaluator.py`, `Render.get_rendered_video` in `lib/common/render.py`), so
               `from lib.common.train_util import *` (apps/ICON.py:20) still finds everything else it uses.
 
 Callers and call sites this serves: apps/ICON.py:17-22, 52-90 (HGPIFuNet, Seg3dLossless, query_func, get_visibility),
 apps/infer.py:22-31, apps/ICON.py:634-640 (calculate_chamfer_p2s), apps/ICON.py:527-528, 555-558, 641-643 (init_gl,
 render_normal and calculate_normal_consist through _render_normal: no OpenGL context),
+apps/infer.py:548-562 (`-export_video`: get_rendered_video's 360 views per mesh, a chunk of views per kernel call),
 lib/dataset/mesh_util.py:187-237 (load_checkpoint:
 identical state_dict keys),
 lib/dataset/TestDataset.py:137 (get_visibility).
@@ -51,7 +52,7 @@ def _replacements():
 
 
 def _patches():
-    from . import encoders, mesh, metrics, net, visibility, voxelize
+    from . import encoders, mesh, mesh_views, metrics, net, visibility, voxelize
 
     def make_define_G(reference_define_G):
         import torch.nn as nn
@@ -78,6 +79,7 @@ def _patches():
         "lib.net.FBNet": {"define_G": make_define_G},          # callable(old value) -> new value
         "lib.net.VE": {"VolumeEncoder": encoders.VolumeEncoder, "Residual3D": encoders.Residual3D},
         "lib.dataset.Evaluator": {"Evaluator": metrics.make_Evaluator},     # chamfer_p2s, init_gl, _render_normal
+        "lib.common.render": {"Render": mesh_views.make_Render},            # get_rendered_video
     }
 
 

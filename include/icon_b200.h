@@ -270,6 +270,26 @@ int icon_normal_render(const float *verts, const float *norms, int V, const int6
                        const float *h_model, int width, int height, float *out_rgba, int32_t *out_face,
                        void *ws, size_t ws_bytes, icon_stream_t stream);
 
+/* ------------------------------------------------------------------ self-rotation video of the demo
+ * Replace the pytorch3d renders of Render.get_rendered_video (lib/common/render.py:327-374; MeshRasterizer +
+ * cleanShader at get_camera / init_renderer(camera, "clean_mesh", "gray")) and the colours VF2Mesh gives a mesh.
+ * Rules (parity unpinned): csrc/mesh_views.cu header.
+ *
+ * icon_area_vertex_normals: pytorch3d's verts_normals_packed of verts [V,3] f32, faces [F,3] i64 -> out [V,3] f32;
+ * bitwise reproducible (no float atomics). */
+size_t icon_area_vertex_normals_workspace_bytes(int V, int F);
+int icon_area_vertex_normals(const float *verts, int V, const int64_t *faces, int F, float *out, void *ws,
+                             size_t ws_bytes, icon_stream_t stream);
+/* icon_mesh_views: A orthographic views at S x S (S <= 4096, A F < 2^31) in one call.  verts [V,3] f32, colors
+ * [V,3] f32 (per-vertex RGB), faces [F,3] i64, h_view_mats: HOST pointer to A x 12 floats (each view's 3 x 4 matrix,
+ * rows; icon_b200/mesh_views.py view_matrices).  out [A,S,S,3] u8 RGB, row 0 at the top; face_out [A,S,S] i32 the
+ * nearest fragment's face (-1 background) or NULL; rgb_out [A,S,S,3] f32 the blended colour before the uint8
+ * conversion, or NULL.  ws: icon_mesh_views_workspace_bytes(V, F, S, A) bytes (about 250 A S^2 + 16 A V + 8 A F). */
+size_t icon_mesh_views_workspace_bytes(int V, int F, int S, int A);
+int icon_mesh_views(const float *verts, const float *colors, int V, const int64_t *faces, int F,
+                    const float *h_view_mats, int A, int S, uint8_t *out, int32_t *face_out, float *rgb_out,
+                    void *ws, size_t ws_bytes, icon_stream_t stream);
+
 /* ------------------------------------------------------------------ encoder operators
  * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
  * two take NCHW fp32 tensors; every 2-D convolution and normalisation runs on the NHWC path after them. */
