@@ -81,6 +81,11 @@ _SIGS = {
     "icon_area_vertex_normals": (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "icon_mesh_views_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "icon_mesh_views": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_mesh_render_state_bytes": (_sz, [_i, _i, _i]),
+    "icon_mesh_render_workspace_bytes": (_sz, [_i, _i, _i, _i, _i, _i]),
+    "icon_mesh_render_forward": (_i, [_i, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "icon_mesh_render_backward": (_i, [_i, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp, _vp, _vp, _sz,
+                                       _vp]),
     "icon_mc_workspace_bytes": (_sz, [_i, _i]),
     "icon_mc_count": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _sz, _vp, _vp]),
     "icon_mc_emit": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _vp, _vp, _i64, _i64, _vp]),

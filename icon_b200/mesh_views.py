@@ -11,7 +11,9 @@ header.  `view_matrices` builds each view's matrix in float64 and rounds it to f
 (verts_normals_padded + 1) / 2 from icon_area_vertex_normals.  `make_Render` is the overlay patch of
 lib.common.render: it rebinds Render.get_rendered_video only.
 """
+import functools
 import math
+import types
 
 import numpy as np
 import torch
@@ -47,10 +49,17 @@ def view_matrices(angles, y_center=0.0, scale=100.0):
     """The camera of each angle (degrees) as get_rendered_video / get_camera set it up: eye (100 cos, y_center,
     100 sin), looking at (0, y_center, 0), up +y, orthographic over +-100 with scale_xyz = scale.  -> float32
     [A,3,4], rows x_ndc, y_ndc, z_view = M [p; 1]; built in float64 and rounded once."""
-    out = np.empty((len(angles), 3, 4), np.float64)
+    return eye_matrices([(100.0 * math.cos(np.pi / 180 * angle), float(y_center), 100.0 * math.sin(np.pi / 180 * angle))
+                         for angle in angles], y_center, scale)
+
+
+def eye_matrices(eyes, y_center=0.0, scale=100.0):
+    """get_camera's matrix for each eye tuple of Render.cam_pos: looking at (0, y_center, 0), up +y, orthographic
+    over +-100 with scale_xyz = scale.  -> float32 [A,3,4] (as view_matrices)."""
+    out = np.empty((len(eyes), 3, 4), np.float64)
     at, up = np.array([0.0, float(y_center), 0.0]), np.array([0.0, 1.0, 0.0])
-    for k, angle in enumerate(angles):
-        eye = np.array([100.0 * math.cos(np.pi / 180 * angle), float(y_center), 100.0 * math.sin(np.pi / 180 * angle)])
+    for k, e in enumerate(eyes):
+        eye = np.array([float(x) for x in e])
         z = _unit(at - eye)
         x = _unit(np.cross(up, z))
         y = _unit(np.cross(z, x))
@@ -158,3 +167,177 @@ def make_Render(reference_render):
 def render_chunk(verts, faces, colors, mats, size):
     """One chunk of get_rendered_video's frames of one mesh: uint8 [n,size,size,3] on the device."""
     return views_from_matrices(verts, faces, mats, size, colors, chunk=len(mats))
+
+
+# ---------------------------------------------------------------- differentiable renders of the fitting loops
+
+NORMAL, SILHOUETTE = 0, 1            # icon_mesh_render_* modes (ICON_RENDER_NORMAL / _SILHOUETTE)
+
+
+def _mesh_tensors(verts, faces, colors):
+    dev = _device(verts, faces, colors)
+    v = verts.detach().to(dev, torch.float32).contiguous()
+    f = faces.detach().to(dev, torch.int64).contiguous()
+    c = colors.detach().to(dev, torch.float32).contiguous() if colors is not None else None
+    if v.dim() != 2 or v.shape[1] != 3 or f.dim() != 2 or f.shape[1] != 3 or v.shape[0] == 0 or f.shape[0] == 0:
+        raise _C.IconError(f"fit render: verts {tuple(v.shape)} / faces {tuple(f.shape)} must be non-empty [n,3]")
+    if c is not None and tuple(c.shape) != tuple(v.shape):
+        raise _C.IconError(f"fit render: colours {tuple(c.shape)} for verts {tuple(v.shape)}")
+    return dev, v, f, c
+
+
+def _render_forward(mode, v, f, c, mats, S, keep_state):
+    """One icon_mesh_render_forward call -> (out, state or None)."""
+    A, V, F = mats.shape[0] // 12, v.shape[0], f.shape[0]
+    shape = (A, S, S, 3) if mode == NORMAL else (A, S, S)
+    out = torch.empty(shape, dtype=torch.float32, device=v.device)
+    with torch.cuda.device(v.device):
+        sbytes = lib.icon_mesh_render_state_bytes(mode, S, A)
+        state = torch.empty(sbytes, dtype=torch.uint8, device=v.device)
+        nbytes = lib.icon_mesh_render_workspace_bytes(mode, 0, V, F, S, A)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=v.device)
+        check(lib.icon_mesh_render_forward(mode, _p(v), _p(c), V, _p(f), F, _hf(mats), A, S, _p(out), _p(state),
+                                           sbytes, _p(ws), nbytes, _stream()), "icon_mesh_render_forward")
+    return out, (state if keep_state else None)
+
+
+def _render_backward(mode, v, f, c, mats, S, state, grad_out):
+    """One icon_mesh_render_backward call -> (grad_verts, grad_colors or None)."""
+    A, V, F = mats.shape[0] // 12, v.shape[0], f.shape[0]
+    g = grad_out.detach().to(v.device, torch.float32).contiguous()
+    gv = torch.empty(V, 3, dtype=torch.float32, device=v.device)
+    gc = torch.empty(V, 3, dtype=torch.float32, device=v.device) if mode == NORMAL else None
+    with torch.cuda.device(v.device):
+        nbytes = lib.icon_mesh_render_workspace_bytes(mode, 1, V, F, S, A)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=v.device)
+        check(lib.icon_mesh_render_backward(mode, _p(v), _p(c), V, _p(f), F, _hf(mats), A, S, _p(g), _p(state),
+                                            state.numel(), _p(gv), _p(gc), _p(ws), nbytes, _stream()),
+              "icon_mesh_render_backward")
+    return gv, gc
+
+
+class NormalImage(torch.autograd.Function):
+    """get_rgb_image's renders: verts [V,3], colors [V,3] (both may require grad), faces [F,3], view matrices
+    float32 [A,3,4] -> rgb float32 [A,S,S,3] (softmax_rgb_blend before any rescaling)."""
+
+    @staticmethod
+    def forward(ctx, verts, colors, faces, mats, size, keep_state):
+        dev, v, f, c = _mesh_tensors(verts, faces, colors)
+        m = np.ascontiguousarray(np.asarray(mats, np.float32).reshape(-1))
+        out, state = _render_forward(NORMAL, v, f, c, m, int(size), keep_state)
+        if state is not None:
+            ctx.saved = (v, f, c, m, int(size), state, verts.dtype, colors.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        v, f, c, m, S, state, vdt, cdt = ctx.saved
+        gv, gc = _render_backward(NORMAL, v, f, c, m, S, state, grad)
+        return (gv.to(vdt) if ctx.needs_input_grad[0] else None, gc.to(cdt) if ctx.needs_input_grad[1] else None,
+                None, None, None, None)
+
+
+class SilhouetteImage(torch.autograd.Function):
+    """get_silhouette_image's renders: verts [V,3] (may require grad), faces [F,3], view matrices float32 [A,3,4]
+    -> alpha float32 [A,S,S] (sigmoid_alpha_blend)."""
+
+    @staticmethod
+    def forward(ctx, verts, faces, mats, size, keep_state):
+        dev, v, f, _ = _mesh_tensors(verts, faces, None)
+        m = np.ascontiguousarray(np.asarray(mats, np.float32).reshape(-1))
+        out, state = _render_forward(SILHOUETTE, v, f, None, m, int(size), keep_state)
+        if state is not None:
+            ctx.saved = (v, f, m, int(size), state, verts.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        v, f, m, S, state, vdt = ctx.saved
+        gv, _ = _render_backward(SILHOUETTE, v, f, None, m, S, state, grad)
+        return gv.to(vdt) if ctx.needs_input_grad[0] else None, None, None, None, None
+
+
+def normal_image(verts, faces, colors, mats, size=512):
+    """Differentiable get_rgb_image render of every view of mats -> float32 [A,size,size,3].  The state the
+    backward needs is kept only when grad mode is on and verts or colors require grad."""
+    keep = torch.is_grad_enabled() and (verts.requires_grad or colors.requires_grad)
+    return NormalImage.apply(verts, colors, faces, mats, size, keep)
+
+
+def silhouette_image(verts, faces, mats, size=512):
+    """Differentiable get_silhouette_image render of every view of mats -> float32 [A,size,size]."""
+    keep = torch.is_grad_enabled() and verts.requires_grad
+    return SilhouetteImage.apply(verts, faces, mats, size, keep)
+
+
+def fit_render(mode, verts, faces, colors, mats, size):
+    """The renders behind the patched get_rgb_image (NORMAL) / get_silhouette_image (SILHOUETTE)."""
+    if mode == NORMAL:
+        return normal_image(verts, faces, colors, mats, size)
+    return silhouette_image(verts, faces, mats, size)
+
+
+def _selected(render, cam_ids):
+    return [cam_id for cam_id in range(len(render.cam_pos)) if cam_id in cam_ids]
+
+
+def get_rgb_image(self, cam_ids=[0, 2]):
+    """render.py:296-325 for self.meshes[0]: one render per selected camera, in ascending cam id, each
+    ((rgb - 0.5) * 2) as [1,3,S,S]; cam 2 flipped along W when exactly two ids are given.  One kernel call renders
+    every selected view; gradients flow to the mesh's packed vertices and vertex colours."""
+    sel = _selected(self, cam_ids)
+    if not sel:
+        return []
+    mesh = self.meshes[0]
+    mats = eye_matrices([self.cam_pos[c] for c in sel], self.mesh_y_center, self.scale)
+    rgb = fit_render(NORMAL, mesh.verts_packed(), mesh.faces_packed(), mesh.textures.verts_features_packed(), mats,
+                     self.size)
+    images = []
+    for k, cam_id in enumerate(sel):
+        img = (rgb[k:k + 1].permute(0, 3, 1, 2) - 0.5) * 2.0
+        if cam_id == 2 and len(cam_ids) == 2:
+            img = torch.flip(img, dims=[3])
+        images.append(img)
+    return images
+
+
+def get_silhouette_image(self, cam_ids=[0, 2]):
+    """render.py:376-387 for self.meshes[0]: one [1,S,S] silhouette per selected camera, in ascending cam id; cam 2
+    flipped along W when exactly two ids are given.  One kernel call renders every selected view."""
+    sel = _selected(self, cam_ids)
+    if not sel:
+        return []
+    mesh = self.meshes[0]
+    mats = eye_matrices([self.cam_pos[c] for c in sel], self.mesh_y_center, self.scale)
+    alpha = fit_render(SILHOUETTE, mesh.verts_packed(), mesh.faces_packed(), None, mats, self.size)
+    images = []
+    for k, cam_id in enumerate(sel):
+        img = alpha[k:k + 1]
+        if cam_id == 2 and len(cam_ids) == 2:
+            img = torch.flip(img, dims=[2])
+        images.append(img)
+    return images
+
+
+def bind_fit_renders(render):
+    """Rebind get_rgb_image and get_silhouette_image on one Render instance (the class stays the reference's)."""
+    render.get_rgb_image = types.MethodType(get_rgb_image, render)
+    render.get_silhouette_image = types.MethodType(get_silhouette_image, render)
+    return render
+
+
+def make_TestDataset(reference_cls):
+    """Overlay patch of lib.dataset.TestDataset: after the reference __init__, the instance's `render` (the Render
+    both fitting loops of apps/infer.py draw through, via render_normal and render.get_silhouette_image) gets the
+    device get_rgb_image / get_silhouette_image."""
+    if reference_cls is None:
+        return None
+    reference_init = reference_cls.__init__
+
+    @functools.wraps(reference_init)
+    def __init__(self, *args, **kwargs):
+        reference_init(self, *args, **kwargs)
+        bind_fit_renders(self.render)
+
+    reference_cls.__init__ = __init__
+    return reference_cls

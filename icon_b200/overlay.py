@@ -18,12 +18,16 @@ accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.
               (`query_func` in `lib/common/train_util.py`, `get_visibility` in `lib/dataset/mesh_util.py`, the
               encoder classes in `lib/net/{NormalNet,MLP,HGFilters,VE}.py`, `define_G` in `lib/net/FBNet.py`,
               `Evaluator.calculate_chamfer_p2s`, `Evaluator.init_gl` and `Evaluator._render_normal` in
-              `lib/dataset/Evaluator.py`, `Render.get_rendered_video` in `lib/common/render.py`), so
+              `lib/dataset/Evaluator.py`, `Render.get_rendered_video` in `lib/common/render.py`, and in
+              `lib/dataset/TestDataset.py` an `__init__` that rebinds `get_rgb_image` / `get_silhouette_image` on
+              the instance's `self.render` only), so
               `from lib.common.train_util import *` (apps/ICON.py:20) still finds everything else it uses.
 
 Callers and call sites this serves: apps/ICON.py:17-22, 52-90 (HGPIFuNet, Seg3dLossless, query_func, get_visibility),
 apps/infer.py:22-31, apps/ICON.py:634-640 (calculate_chamfer_p2s), apps/ICON.py:527-528, 555-558, 641-643 (init_gl,
 render_normal and calculate_normal_consist through _render_normal: no OpenGL context),
+apps/infer.py:168-273, 431-505 (the body-fit and cloth loops: differentiable normal / silhouette renders through
+TestDataset.render_normal and render.get_silhouette_image),
 apps/infer.py:548-562 (`-export_video`: get_rendered_video's 360 views per mesh, a chunk of views per kernel call),
 lib/dataset/mesh_util.py:187-237 (load_checkpoint:
 identical state_dict keys),
@@ -80,6 +84,7 @@ def _patches():
         "lib.net.VE": {"VolumeEncoder": encoders.VolumeEncoder, "Residual3D": encoders.Residual3D},
         "lib.dataset.Evaluator": {"Evaluator": metrics.make_Evaluator},     # chamfer_p2s, init_gl, _render_normal
         "lib.common.render": {"Render": mesh_views.make_Render},            # get_rendered_video
+        "lib.dataset.TestDataset": {"TestDataset": mesh_views.make_TestDataset},  # self.render's fit renders
     }
 
 

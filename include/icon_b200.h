@@ -289,6 +289,27 @@ size_t icon_mesh_views_workspace_bytes(int V, int F, int S, int A);
 int icon_mesh_views(const float *verts, const float *colors, int V, const int64_t *faces, int F,
                     const float *h_view_mats, int A, int S, uint8_t *out, int32_t *face_out, float *rgb_out,
                     void *ws, size_t ws_bytes, icon_stream_t stream);
+/* Differentiable renders of the fitting loops: Render.get_rgb_image (mode ICON_RENDER_NORMAL, the rules of
+ * icon_mesh_views) and Render.get_silhouette_image (ICON_RENDER_SILHOUETTE), forward and backward; rules and
+ * gradient formulas (parity unpinned) in the csrc/mesh_views.cu header.  Arguments as icon_mesh_views (h_view_mats on
+ * the host; colors may be NULL for the silhouette).
+ * icon_mesh_render_forward: out [A,S,S,3] f32 rgb (NORMAL) or [A,S,S] f32 alpha (SILHOUETTE).  state: the K slot keys
+ *   of every pixel, [A][S][S][K] u64 (z bits << 32 | face, ascending, all ones when empty; K = 30 / 50), which the
+ *   backward reads: icon_mesh_render_state_bytes(mode, S, A) bytes.
+ * icon_mesh_render_backward: grad_out shaped as out -> grad_verts [V,3] f32 and (NORMAL, or NULL) grad_colors [V,3]
+ *   f32, overwritten; bitwise reproducible (no float atomics).
+ * ws: icon_mesh_render_workspace_bytes(mode, backward, V, F, S, A) bytes (backward = 0 forward, 1 backward). */
+#define ICON_RENDER_NORMAL 0
+#define ICON_RENDER_SILHOUETTE 1
+size_t icon_mesh_render_state_bytes(int mode, int S, int A);
+size_t icon_mesh_render_workspace_bytes(int mode, int backward, int V, int F, int S, int A);
+int icon_mesh_render_forward(int mode, const float *verts, const float *colors, int V, const int64_t *faces, int F,
+                             const float *h_view_mats, int A, int S, float *out, void *state, size_t state_bytes,
+                             void *ws, size_t ws_bytes, icon_stream_t stream);
+int icon_mesh_render_backward(int mode, const float *verts, const float *colors, int V, const int64_t *faces, int F,
+                              const float *h_view_mats, int A, int S, const float *grad_out, const void *state,
+                              size_t state_bytes, float *grad_verts, float *grad_colors, void *ws, size_t ws_bytes,
+                              icon_stream_t stream);
 
 /* ------------------------------------------------------------------ encoder operators
  * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
