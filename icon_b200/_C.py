@@ -79,6 +79,18 @@ _SIGS = {
     "icon_normal_render": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "icon_area_vertex_normals_workspace_bytes": (_sz, [_i, _i]),
     "icon_area_vertex_normals": (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    "icon_area_vertex_normals_backward_workspace_bytes": (_sz, [_i, _i]),
+    "icon_area_vertex_normals_backward": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "icon_mesh_topology_workspace_bytes": (_sz, [_i, _i]),
+    "icon_mesh_topology_count": (_i, [_vp, _i, _i, ctypes.POINTER(_i64), _vp, _sz, _vp]),
+    "icon_mesh_topology_build": (_i, [_vp, _vp, _sz, _vp]),
+    "icon_vertex_edges_workspace_bytes": (_sz, [_i, _i]),
+    "icon_vertex_edges": (_i, [_vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "icon_mesh_priors_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "icon_mesh_priors_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_mesh_priors_backward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_local_affine_forward": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp]),
+    "icon_local_affine_backward": (_i, [_vp, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "icon_mesh_views_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "icon_mesh_views": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "icon_mesh_render_state_bytes": (_sz, [_i, _i, _i]),
@@ -97,6 +109,13 @@ for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)          # AttributeError here = header / library mismatch
     _fn.restype = _res
     _fn.argtypes = _args
+
+
+class MeshTopology(ctypes.Structure):
+    """icon_mesh_topology (include/icon_b200.h): device pointers of one mesh's topology arrays."""
+    _fields_ = [("V", _i), ("F", _i), ("E", _i), ("faces", _vp), ("edges", _vp), ("face_to_edge", _vp),
+                ("vert_off", _vp), ("vert_edges", _vp), ("edge_off", _vp), ("edge_entries", _vp),
+                ("corner_off", _vp), ("vert_corners", _vp)]
 
 
 class IconError(RuntimeError):

@@ -12,6 +12,12 @@
 //   the next two corners of the face; then n / max(sqrt((x x + y y) + z z), 1e-6).  Each vertex's contributions are
 //   sorted by (pass, face) and summed in that order: no float atomics, bitwise reproducible.  Faces with an index
 //   outside [0, V) contribute nothing.
+//   Backward (icon_area_vertex_normals_backward; restated by oracle/mesh_priors.py with float64 autograd): the
+//   gradient of F.normalize(s, eps = 1e-6) with torch's semantics, from the fp32 s of the forward, in fp64:
+//   (g - n (n.g)) / |s| with n = s / |s| when the fp32 norm is >= 1e-6, else g / 1e-6 (clamp_min passes g there);
+//   then through each corner product n = u x w (u = p1 - p0, w = p2 - p0): p1 += w x G, p2 += G x u,
+//   p0 -= both.  Each vertex sums its contributions over the same sorted (pass, face) lists in fp64 (its own position
+//   in each listed face, all three products of that face) and rounds once.
 //
 // Views (icon_mesh_views).  Cameras: view a has eye = (100 cos t, y_c, 100 sin t), at = (0, y_c, 0), up = +y;
 //   look_at_view_transform's basis z = unit(at - eye), x = unit(up x z), y = unit(z x x), and FoVOrthographicCameras
@@ -175,6 +181,86 @@ __global__ void k_an_sum(const float *__restrict__ verts, const int64_t *__restr
     float nrm = sqrtf((sx * sx + sy * sy) + sz * sz);
     if (nrm < 1e-6f) nrm = 1e-6f;
     out[3 * (int64_t)v] = sx / nrm; out[3 * (int64_t)v + 1] = sy / nrm; out[3 * (int64_t)v + 2] = sz / nrm;
+}
+
+// backward, 1: sort the vertex's list, recompute s as k_an_sum does, then the normalize gradient (fp64) into gs
+__global__ void k_an_grad_s(const float *__restrict__ verts, const int64_t *__restrict__ faces, int F,
+                            const int32_t *__restrict__ off, int32_t *__restrict__ keys, int V,
+                            const float *__restrict__ gn, double *__restrict__ gs) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    int32_t *a = keys + off[v];
+    const int n = off[v + 1] - off[v];
+    heap_sort_i32(a, n);
+    float sx = 0.f, sy = 0.f, sz = 0.f;
+    for (int i = 0; i < n; ++i) {
+        const int pass = a[i] / F, f = a[i] % F;
+        const int c = pass == 0 ? 1 : (pass == 1 ? 2 : 0);
+        const int64_t i0 = faces[3 * (int64_t)f + c], i1 = faces[3 * (int64_t)f + (c + 1) % 3];
+        const int64_t i2 = faces[3 * (int64_t)f + (c + 2) % 3];
+        const float p0x = verts[3 * i0], p0y = verts[3 * i0 + 1], p0z = verts[3 * i0 + 2];
+        const float ux = verts[3 * i1] - p0x, uy = verts[3 * i1 + 1] - p0y, uz = verts[3 * i1 + 2] - p0z;
+        const float wx = verts[3 * i2] - p0x, wy = verts[3 * i2 + 1] - p0y, wz = verts[3 * i2 + 2] - p0z;
+        sx = sx + (uy * wz - uz * wy);
+        sy = sy + (uz * wx - ux * wz);
+        sz = sz + (ux * wy - uy * wx);
+    }
+    const double s[3] = {sx, sy, sz};
+    const double g[3] = {gn[3 * (int64_t)v], gn[3 * (int64_t)v + 1], gn[3 * (int64_t)v + 2]};
+    const double len = sqrt((s[0] * s[0] + s[1] * s[1]) + s[2] * s[2]);
+    const float nrm = sqrtf((sx * sx + sy * sy) + sz * sz);
+    if (nrm < 1e-6f) {                                    // the clamp: g / eps
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gs[3 * (int64_t)v + k] = g[k] / 1e-6;
+        return;
+    }
+    const double d = ((s[0] * g[0] + s[1] * g[1]) + s[2] * g[2]) / len;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) gs[3 * (int64_t)v + k] = (g[k] - (s[k] / len) * d) / len;
+}
+
+// backward, 2: per vertex, over its sorted (pass, face) entries, the derivative of the entry face's three corner
+// products n_k = (p_{k+1} - p_k) x (p_{k+2} - p_k) with respect to the vertex's own position in the face
+__global__ void k_an_grad_v(const float *__restrict__ verts, const int64_t *__restrict__ faces, int F,
+                            const int32_t *__restrict__ off, const int32_t *__restrict__ keys, int V,
+                            const double *__restrict__ gs, float *__restrict__ gv) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const int32_t *a = keys + off[v];
+    const int n = off[v + 1] - off[v];
+    double acc[3] = {0.0, 0.0, 0.0};
+    for (int i = 0; i < n; ++i) {
+        const int pass = a[i] / F, f = a[i] % F;
+        const int c = pass == 0 ? 1 : (pass == 1 ? 2 : 0);              // the vertex's corner in face f
+        double p[3][3];
+        int64_t id[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            id[k] = faces[3 * (int64_t)f + k];
+#pragma unroll
+            for (int q = 0; q < 3; ++q) p[k][q] = (double)verts[3 * id[k] + q];
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {                                   // corner k's product, added to vertex id[k]
+            const double *G = gs + 3 * id[k];
+            double u[3], w[3];
+#pragma unroll
+            for (int q = 0; q < 3; ++q) {
+                u[q] = p[(k + 1) % 3][q] - p[k][q];
+                w[q] = p[(k + 2) % 3][q] - p[k][q];
+            }
+            const double gu[3] = {w[1] * G[2] - w[2] * G[1], w[2] * G[0] - w[0] * G[2], w[0] * G[1] - w[1] * G[0]};
+            const double gw[3] = {G[1] * u[2] - G[2] * u[1], G[2] * u[0] - G[0] * u[2], G[0] * u[1] - G[1] * u[0]};
+#pragma unroll
+            for (int q = 0; q < 3; ++q) {
+                if (c == k) acc[q] -= gu[q] + gw[q];
+                else if (c == (k + 1) % 3) acc[q] += gu[q];
+                else acc[q] += gw[q];
+            }
+        }
+    }
+#pragma unroll
+    for (int q = 0; q < 3; ++q) gv[3 * (int64_t)v + q] = (float)acc[q];
 }
 
 struct AnWs {
@@ -910,6 +996,44 @@ extern "C" int icon_area_vertex_normals(const float *verts, int V, const int64_t
     k_an_fill<<<fb, 256, 0, stream>>>(faces, F, V, w.off, w.cursor, w.keys);
     ICON_LAUNCHED();
     k_an_sum<<<vb, 256, 0, stream>>>(verts, faces, F, w.off, w.keys, V, out);
+    ICON_LAUNCHED();
+    return ICON_OK;
+}
+
+extern "C" size_t icon_area_vertex_normals_backward_workspace_bytes(int V, int F) {
+    if (V <= 0 || F <= 0) return 0;
+    icon::Carver c(nullptr);
+    c.take<char>(icon::an_carve(nullptr, V, F, nullptr));
+    c.take<double>(3 * (size_t)V);
+    return c.total();
+}
+
+extern "C" int icon_area_vertex_normals_backward(const float *verts, int V, const int64_t *faces, int F,
+                                                 const float *grad_normals, float *grad_verts, void *ws,
+                                                 size_t ws_bytes, icon_stream_t stream_) {
+    using namespace icon;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    ICON_CHECK_ARG(verts && faces && grad_normals && grad_verts && ws, "icon_area_vertex_normals_backward: null pointer");
+    ICON_CHECK_ARG(V > 0 && F > 0 && F <= (INT32_MAX - 2) / 3, "icon_area_vertex_normals_backward: bad sizes V=%d F=%d",
+                   V, F);
+    ICON_CHECK_ARG(ws_bytes >= icon_area_vertex_normals_backward_workspace_bytes(V, F),
+                   "icon_area_vertex_normals_backward: workspace too small");
+    Carver c(ws);
+    AnWs w;
+    an_carve(c.take<char>(an_carve(nullptr, V, F, nullptr)), V, F, &w);
+    double *gs = c.take<double>(3 * (size_t)V);
+    ICON_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int32_t) * ((size_t)V + 1), stream));
+    ICON_CUDA(cudaMemsetAsync(w.cursor, 0, sizeof(int32_t) * (size_t)V, stream));
+    const unsigned fb = (unsigned)((F + 255) / 256), vb = (unsigned)((V + 255) / 256);
+    k_an_count<<<fb, 256, 0, stream>>>(faces, F, V, w.cnt);
+    ICON_LAUNCHED();
+    int rc = scan_exclusive_i32(w.cnt, w.off, (int64_t)V + 1, nullptr, w.scan_ws, stream);
+    if (rc) return rc;
+    k_an_fill<<<fb, 256, 0, stream>>>(faces, F, V, w.off, w.cursor, w.keys);
+    ICON_LAUNCHED();
+    k_an_grad_s<<<vb, 256, 0, stream>>>(verts, faces, F, w.off, w.keys, V, grad_normals, gs);
+    ICON_LAUNCHED();
+    k_an_grad_v<<<vb, 256, 0, stream>>>(verts, faces, F, w.off, w.keys, V, gs, grad_verts);
     ICON_LAUNCHED();
     return ICON_OK;
 }

@@ -13,6 +13,7 @@ lib.common.render: it rebinds Render.get_rendered_video only.
 """
 import functools
 import math
+import sys
 import types
 
 import numpy as np
@@ -82,6 +83,33 @@ def area_vertex_normals(verts, faces, device=None):
         check(lib.icon_area_vertex_normals(_p(v), v.shape[0], _p(f), f.shape[0], _p(out), _p(ws), nbytes,
                                            _stream()), "icon_area_vertex_normals")
     return out
+
+
+class VertexNormals(torch.autograd.Function):
+    """Differentiable area_vertex_normals: verts [V,3] (may require grad), faces [F,3] -> float32 [V,3].  The forward
+    is icon_area_vertex_normals, the backward icon_area_vertex_normals_backward (no float atomics)."""
+
+    @staticmethod
+    def forward(ctx, verts, faces):
+        dev = _device(verts, faces)
+        v = _as(verts, dev, torch.float32, "verts")
+        f = _as(faces, dev, torch.int64, "faces")
+        ctx.saved = (v, f, verts.dtype)
+        return area_vertex_normals(v, f, dev)
+
+    @staticmethod
+    def backward(ctx, grad):
+        v, f, dt = ctx.saved
+        if not ctx.needs_input_grad[0]:
+            return None, None
+        g = grad.detach().to(v.device, torch.float32).contiguous()
+        gv = torch.empty_like(v)
+        with torch.cuda.device(v.device):
+            nbytes = lib.icon_area_vertex_normals_backward_workspace_bytes(v.shape[0], f.shape[0])
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=v.device)
+            check(lib.icon_area_vertex_normals_backward(_p(v), v.shape[0], _p(f), f.shape[0], _p(g), _p(gv), _p(ws),
+                                                        nbytes, _stream()), "icon_area_vertex_normals_backward")
+        return gv.to(dt), None
 
 
 def vertex_colors(verts, faces, device=None):
@@ -319,17 +347,40 @@ def get_silhouette_image(self, cam_ids=[0, 2]):
     return images
 
 
+def VF2Mesh(self, verts, faces):
+    """render.py:237-258 with the vertex colours from VertexNormals: the reference's conversions (tensor, unsqueeze,
+    .float() / .long(), device) and its own Meshes / TexturesVertex (those of the Render class's module), with
+    verts_features = (VertexNormals(verts_packed, faces_packed) + 1) * 0.5, differentiable to the vertices."""
+    ref = sys.modules[type(self).__module__]
+    if not torch.is_tensor(verts):
+        verts = torch.tensor(verts)
+    if not torch.is_tensor(faces):
+        faces = torch.tensor(faces)
+    if verts.ndimension() == 2:
+        verts = verts.unsqueeze(0).float()
+    if faces.ndimension() == 2:
+        faces = faces.unsqueeze(0).long()
+    verts = verts.to(self.device)
+    faces = faces.to(self.device)
+    mesh = ref.Meshes(verts, faces).to(self.device)
+    colors = (VertexNormals.apply(mesh.verts_packed(), mesh.faces_packed()) + 1.0) * 0.5
+    mesh.textures = ref.TexturesVertex(verts_features=colors.unsqueeze(0))
+    return mesh
+
+
 def bind_fit_renders(render):
-    """Rebind get_rgb_image and get_silhouette_image on one Render instance (the class stays the reference's)."""
+    """Rebind get_rgb_image, get_silhouette_image and VF2Mesh on one Render instance (the class stays the
+    reference's)."""
     render.get_rgb_image = types.MethodType(get_rgb_image, render)
     render.get_silhouette_image = types.MethodType(get_silhouette_image, render)
+    render.VF2Mesh = types.MethodType(VF2Mesh, render)
     return render
 
 
 def make_TestDataset(reference_cls):
     """Overlay patch of lib.dataset.TestDataset: after the reference __init__, the instance's `render` (the Render
     both fitting loops of apps/infer.py draw through, via render_normal and render.get_silhouette_image) gets the
-    device get_rgb_image / get_silhouette_image."""
+    device get_rgb_image / get_silhouette_image and the VF2Mesh whose colours VertexNormals differentiates."""
     if reference_cls is None:
         return None
     reference_init = reference_cls.__init__

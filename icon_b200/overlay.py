@@ -19,8 +19,8 @@ accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.
               encoder classes in `lib/net/{NormalNet,MLP,HGFilters,VE}.py`, `define_G` in `lib/net/FBNet.py`,
               `Evaluator.calculate_chamfer_p2s`, `Evaluator.init_gl` and `Evaluator._render_normal` in
               `lib/dataset/Evaluator.py`, `Render.get_rendered_video` in `lib/common/render.py`, and in
-              `lib/dataset/TestDataset.py` an `__init__` that rebinds `get_rgb_image` / `get_silhouette_image` on
-              the instance's `self.render` only), so
+              `lib/dataset/TestDataset.py` an `__init__` that rebinds `get_rgb_image` / `get_silhouette_image` /
+              `VF2Mesh` on the instance's `self.render` only), so
               `from lib.common.train_util import *` (apps/ICON.py:20) still finds everything else it uses.
 
 Callers and call sites this serves: apps/ICON.py:17-22, 52-90 (HGPIFuNet, Seg3dLossless, query_func, get_visibility),
@@ -28,6 +28,8 @@ apps/infer.py:22-31, apps/ICON.py:634-640 (calculate_chamfer_p2s), apps/ICON.py:
 render_normal and calculate_normal_consist through _render_normal: no OpenGL context),
 apps/infer.py:168-273, 431-505 (the body-fit and cloth loops: differentiable normal / silhouette renders through
 TestDataset.render_normal and render.get_silhouette_image),
+apps/infer.py:405-476 and apps/ICON.py:483 (the cloth loop's LocalAffine and shape priors; VF2Mesh's differentiable
+vertex colours),
 apps/infer.py:548-562 (`-export_video`: get_rendered_video's 360 views per mesh, a chunk of views per kernel call),
 lib/dataset/mesh_util.py:187-237 (load_checkpoint:
 identical state_dict keys),
@@ -56,7 +58,7 @@ def _replacements():
 
 
 def _patches():
-    from . import encoders, mesh, mesh_views, metrics, net, visibility, voxelize
+    from . import encoders, mesh, mesh_priors, mesh_views, metrics, net, visibility, voxelize
 
     def make_define_G(reference_define_G):
         import torch.nn as nn
@@ -76,7 +78,9 @@ def _patches():
         "lib.common.train_util": {"query_func": net.query_func, "clean_mesh": mesh.clean_mesh,
                                   "get_visibility": visibility.get_visibility},      # duplicate at train_util.py:361
         "lib.dataset.mesh_util": {"get_visibility": visibility.get_visibility, "clean_mesh": mesh.clean_mesh,
-                                  "read_smpl_constants": voxelize.read_smpl_constants},
+                                  "read_smpl_constants": voxelize.read_smpl_constants,
+                                  "update_mesh_shape_prior_losses": mesh_priors.update_mesh_shape_prior_losses},
+        "lib.net.local_affine": {"LocalAffine": mesh_priors.LocalAffine},
         "lib.net.NormalNet": {"NormalNet": encoders.NormalNet},
         "lib.net.MLP": {"MLP": net.MLP},
         "lib.net.HGFilters": {"HGFilter": encoders.HGFilter, "HourGlass": encoders.HourGlass},
@@ -84,7 +88,7 @@ def _patches():
         "lib.net.VE": {"VolumeEncoder": encoders.VolumeEncoder, "Residual3D": encoders.Residual3D},
         "lib.dataset.Evaluator": {"Evaluator": metrics.make_Evaluator},     # chamfer_p2s, init_gl, _render_normal
         "lib.common.render": {"Render": mesh_views.make_Render},            # get_rendered_video
-        "lib.dataset.TestDataset": {"TestDataset": mesh_views.make_TestDataset},  # self.render's fit renders
+        "lib.dataset.TestDataset": {"TestDataset": mesh_views.make_TestDataset},  # self.render's fit renders, VF2Mesh
     }
 
 

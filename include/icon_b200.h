@@ -280,6 +280,13 @@ int icon_normal_render(const float *verts, const float *norms, int V, const int6
 size_t icon_area_vertex_normals_workspace_bytes(int V, int F);
 int icon_area_vertex_normals(const float *verts, int V, const int64_t *faces, int F, float *out, void *ws,
                              size_t ws_bytes, icon_stream_t stream);
+/* icon_area_vertex_normals_backward: grad_normals [V,3] f32 (the upstream gradient of out) -> grad_verts [V,3] f32,
+ * overwritten; fp64 sums in the forward's sorted incidence order, bitwise reproducible.  ws:
+ * icon_area_vertex_normals_backward_workspace_bytes(V, F) bytes. */
+size_t icon_area_vertex_normals_backward_workspace_bytes(int V, int F);
+int icon_area_vertex_normals_backward(const float *verts, int V, const int64_t *faces, int F,
+                                      const float *grad_normals, float *grad_verts, void *ws, size_t ws_bytes,
+                                      icon_stream_t stream);
 /* icon_mesh_views: A orthographic views at S x S (S <= 4096, A F < 2^31) in one call.  verts [V,3] f32, colors
  * [V,3] f32 (per-vertex RGB), faces [F,3] i64, h_view_mats: HOST pointer to A x 12 floats (each view's 3 x 4 matrix,
  * rows; icon_b200/mesh_views.py view_matrices).  out [A,S,S,3] u8 RGB, row 0 at the top; face_out [A,S,S] i32 the
@@ -310,6 +317,53 @@ int icon_mesh_render_backward(int mode, const float *verts, const float *colors,
                               const float *h_view_mats, int A, int S, const float *grad_out, const void *state,
                               size_t state_bytes, float *grad_verts, float *grad_colors, void *ws, size_t ws_bytes,
                               icon_stream_t stream);
+
+/* ------------------------------------------------------------------ cloth-refinement geometry
+ * The mesh topology, the three shape priors of update_mesh_shape_prior_losses (lib/dataset/mesh_util.py:168-176) and
+ * LocalAffine (lib/net/local_affine.py), forward and backward; rules and gradient formulas (parity unpinned) in the
+ * csrc/mesh_priors.cu header.  No float atomics: bitwise reproducible.  One mesh (B = 1).
+ *
+ * Topology: icon_mesh_topology_count(faces [F,3] i64) rejects an index outside [0, V) and returns the edge count E
+ *   to the host (it synchronises the stream); icon_mesh_topology_build, with the same unchanged ws, fills the arrays
+ *   of the struct (all device memory, caller-allocated to the sizes given). */
+typedef struct {
+    int V, F, E;
+    const int64_t *faces;      /* [F,3] */
+    int64_t *edges;            /* [E,2] (min, max), ascending */
+    int64_t *face_to_edge;     /* [F,3] columns e12, e20, e01 */
+    int32_t *vert_off;         /* [V+1] */
+    int32_t *vert_edges;       /* [2E] per vertex its edge ids, ascending (a self-loop twice); degree = row length */
+    int32_t *edge_off;         /* [E+1] */
+    int32_t *edge_entries;     /* [3F] per edge its face-corner entries 3 f + col, ascending */
+    int32_t *corner_off;       /* [V+1] */
+    int32_t *vert_corners;     /* [3F] per vertex its corners 3 f + c, ascending */
+} icon_mesh_topology;
+size_t icon_mesh_topology_workspace_bytes(int V, int F);
+int icon_mesh_topology_count(const int64_t *faces, int V, int F, int64_t *h_E, void *ws, size_t ws_bytes,
+                             icon_stream_t stream);
+int icon_mesh_topology_build(const icon_mesh_topology *t, void *ws, size_t ws_bytes, icon_stream_t stream);
+/* icon_vertex_edges: the vert_edges lists of caller edges [E,2] i64 (indices in [0, V), checked by the caller),
+ * built by the same code as the topology's. */
+size_t icon_vertex_edges_workspace_bytes(int V, int E);
+int icon_vertex_edges(const int64_t *edges, int E, int V, int32_t *vert_off, int32_t *vert_edges, void *ws,
+                      size_t ws_bytes, icon_stream_t stream);
+/* Priors of verts [V,3] f32: forward -> three f32 device scalars (edge, normal consistency, uniform laplacian);
+ * backward: the three upstream gradients as device scalars, NULL = absent (that term is skipped) -> grad_verts [V,3]
+ * f32, overwritten.  ws: icon_mesh_priors_workspace_bytes(V, F, E, backward) bytes. */
+size_t icon_mesh_priors_workspace_bytes(int V, int F, int E, int backward);
+int icon_mesh_priors_forward(const icon_mesh_topology *t, const float *verts, float *out_edge, float *out_nc,
+                             float *out_lap, void *ws, size_t ws_bytes, icon_stream_t stream);
+int icon_mesh_priors_backward(const icon_mesh_topology *t, const float *verts, const float *g_edge, const float *g_nc,
+                              const float *g_lap, float *grad_verts, void *ws, size_t ws_bytes, icon_stream_t stream);
+/* LocalAffine, B = 1: A [N,3,3], b [N,3], x [N,3], edges [E,2] i64 -> out [N,3], w_diff [E,3,4], w_rigid [N] (all
+ * f32).  Backward: g_out / g_diff / g_rigid shaped as those (NULL = absent), vert_off / vert_edges from
+ * icon_vertex_edges of the same edges -> grad_A, grad_b and (when not NULL) grad_x, overwritten. */
+int icon_local_affine_forward(const float *A, const float *b, const float *x, int N, const int64_t *edges, int E,
+                              float *out, float *w_diff, float *w_rigid, icon_stream_t stream);
+int icon_local_affine_backward(const float *A, const float *b, const float *x, int N, const int64_t *edges, int E,
+                               const int32_t *vert_off, const int32_t *vert_edges, const float *g_out,
+                               const float *g_diff, const float *g_rigid, float *grad_A, float *grad_b, float *grad_x,
+                               icon_stream_t stream);
 
 /* ------------------------------------------------------------------ encoder operators
  * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
