@@ -98,6 +98,12 @@ _SIGS = {
     "icon_mesh_render_forward": (_i, [_i, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp, _sz, _vp]),
     "icon_mesh_render_backward": (_i, [_i, _vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _sz, _vp, _vp, _vp, _sz,
                                        _vp]),
+    "icon_lbs_prepare_workspace_bytes": (_sz, [_i, _i, _i]),
+    "icon_lbs_prepare": (_i, [_vp, _vp, _i, _vp, _sz, _vp]),
+    "icon_lbs_state_bytes": (_sz, [_i, _i, _i, _i]),
+    "icon_lbs_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "icon_lbs_forward": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
+    "icon_lbs_backward": (_i, [_vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "icon_mc_workspace_bytes": (_sz, [_i, _i]),
     "icon_mc_count": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _sz, _vp, _vp]),
     "icon_mc_emit": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _vp, _vp, _i64, _i64, _vp]),
@@ -116,6 +122,12 @@ class MeshTopology(ctypes.Structure):
     _fields_ = [("V", _i), ("F", _i), ("E", _i), ("faces", _vp), ("edges", _vp), ("face_to_edge", _vp),
                 ("vert_off", _vp), ("vert_edges", _vp), ("edge_off", _vp), ("edge_entries", _vp),
                 ("corner_off", _vp), ("vert_corners", _vp)]
+
+
+class LbsModel(ctypes.Structure):
+    """icon_lbs_model (include/icon_b200.h): one body model's sizes, parents and device buffers."""
+    _fields_ = [("V", _i), ("J", _i), ("NB", _i), ("parents", _i * 64), ("v_template", _vp), ("shapedirs", _vp),
+                ("posedirs", _vp), ("J_regressor", _vp), ("lbs_weights", _vp), ("J_template", _vp), ("J_dirs", _vp)]
 
 
 class IconError(RuntimeError):

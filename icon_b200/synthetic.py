@@ -228,3 +228,64 @@ def adversarial_points(verts, faces, n_each=600, seed=0):
     near = (cen + 0.02 * rng.standard_normal(cen.shape)).astype(np.float32)
     pts = np.concatenate([on_vert, mid, cen, ray_v, ray_e, near], 0).astype(np.float32)
     return torch.from_numpy(pts)[None]
+
+
+SMPL_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21]
+
+
+def smplx_parents():
+    """A 55-joint tree shaped like SMPL-X's: SMPL's first 22 body joints, jaw and two eyes under the head (15), and
+    three-joint fingers under each wrist (20, 21), five per hand; the fingertips are at depth 10."""
+    par = SMPL_PARENTS[:22] + [15, 15, 15]
+    for wrist in (20, 21):
+        for _ in range(5):
+            n = len(par)
+            par += [wrist, n, n + 1]
+    return par
+
+
+def body_model(kind="smpl", seed=0, V=None):
+    """Seeded SMPL-family model arrays (float32; parents int64), for lbs (lib/smplx/lbs.py):
+    "smpl": v_template = body_mesh() (V 6890, its faces under "faces"), SMPL's 24-joint tree, NB 10;
+    "smplx": V 10475 points of an ellipsoidal cloud, smplx_parents() (55 joints, depth 10), NB 20;
+    "tiny": V points (default 31), J 2, NB 3.
+    J_regressor rows are 4 nearby vertices with positive weights summing to 1; lbs_weights rows are the at most 4
+    nearest joints (inverse-distance weights summing to 1); shapedirs [V,3,NB] and posedirs [9(J-1),3V] are small
+    Gaussians."""
+    rng = np.random.RandomState(seed)
+    out = {}
+    if kind == "smpl":
+        v, f = body_mesh(seed=seed)
+        out["faces"] = f
+        parents, NB = list(SMPL_PARENTS), 10
+    elif kind == "smplx":
+        v = (rng.standard_normal((10475, 3)) * np.array([0.25, 0.45, 0.12])).astype(np.float32)
+        parents, NB = smplx_parents(), 20
+    elif kind == "tiny":
+        v = (rng.standard_normal((31 if V is None else V, 3)) * 0.3).astype(np.float32)
+        parents, NB = [-1, 0], 3
+    else:
+        raise ValueError(f"body_model: unknown kind {kind!r}")
+    out.update(model_arrays(v, parents, NB, rng))
+    return out
+
+
+def model_arrays(v, parents, NB, rng):
+    """body_model()'s regressor, weights and blend shapes for points v [V,3] and a kinematic tree (see there)."""
+    nv, J = len(v), len(parents)
+    centres = rng.choice(nv, J, replace=nv < J)
+    jr = np.zeros((J, nv), np.float64)
+    for j, c in enumerate(centres):
+        near = np.argsort(((v - v[c]) ** 2).sum(1), kind="stable")[:min(4, nv)]
+        w = rng.uniform(0.5, 1.5, len(near))
+        jr[j, near] = w / w.sum()
+    joints = jr @ v.astype(np.float64)
+    d = np.sqrt(((v[:, None, :].astype(np.float64) - joints[None]) ** 2).sum(-1))
+    lw = np.zeros((nv, J), np.float64)
+    near = np.argsort(d, 1, kind="stable")[:, :min(4, J)]
+    w = 1.0 / (np.take_along_axis(d, near, 1) + 0.05)
+    np.put_along_axis(lw, near, w / w.sum(1, keepdims=True), 1)
+    return dict(v_template=v.astype(np.float32), J_regressor=jr.astype(np.float32), lbs_weights=lw.astype(np.float32),
+               shapedirs=(0.01 * rng.standard_normal((nv, 3, NB))).astype(np.float32),
+               posedirs=(0.01 * rng.standard_normal((9 * (J - 1), 3 * nv))).astype(np.float32),
+               parents=np.asarray(parents, np.int64))

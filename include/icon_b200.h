@@ -365,6 +365,40 @@ int icon_local_affine_backward(const float *A, const float *b, const float *x, i
                                const float *g_diff, const float *g_rigid, float *grad_A, float *grad_b, float *grad_x,
                                icon_stream_t stream);
 
+/* ------------------------------------------------------------------ body model (linear-blend skinning)
+ * lbs() of lib/smplx/lbs.py for an SMPL-family model, forward and backward; rules, layouts and reduction order in the
+ * csrc/body_model.cu header.  fp32 inputs and outputs, fp64 inside.  No float atomics: bitwise reproducible, and row b
+ * of a B-row call equals a one-row call on that row.
+ *
+ * icon_lbs_model: the caller fills V, J (2..64), NB (1..1024) and the buffer pointers (device, fp32, contiguous);
+ *   icon_lbs_prepare checks h_parents (host [J] i64: parents[0] = -1, parents[i] < i) and posedirs_rows = 9 (J - 1),
+ *   copies the parents into the struct and writes J_template / J_dirs (caller-allocated device fp64). */
+typedef struct {
+    int V, J, NB;
+    int parents[64];
+    const float *v_template;   /* [V,3] */
+    const float *shapedirs;    /* [V,3,NB] */
+    const float *posedirs;     /* [9(J-1), 3V] */
+    const float *J_regressor;  /* [J,V] */
+    const float *lbs_weights;  /* [V,J] */
+    double *J_template;        /* [J,3]    = J_regressor v_template */
+    double *J_dirs;            /* [J,3,NB] = J_regressor shapedirs */
+} icon_lbs_model;
+size_t icon_lbs_prepare_workspace_bytes(int V, int J, int NB);
+int icon_lbs_prepare(icon_lbs_model *m, const int64_t *h_parents, int posedirs_rows, void *ws, size_t ws_bytes,
+                     icon_stream_t stream);
+/* Forward: betas [B,NB], pose [B,J,3] (pose2rot = 1, axis-angle) or [B,J,3,3] (pose2rot = 0, used as given) ->
+ * verts [B,V,3], joints [B,J,3]; `state` (icon_lbs_state_bytes) keeps what the backward needs.  Backward:
+ * grad_verts [B,V,3] and / or grad_joints [B,J,3] (NULL = zero) -> grad_betas [B,NB] and grad_pose (the pose's
+ * shape), overwritten.  ws: icon_lbs_workspace_bytes(..., backward) bytes (the forward needs none). */
+size_t icon_lbs_state_bytes(int B, int V, int J, int NB);
+size_t icon_lbs_workspace_bytes(int B, int V, int J, int NB, int backward);
+int icon_lbs_forward(const icon_lbs_model *m, int B, const float *betas, const float *pose, int pose2rot, float *verts,
+                     float *joints, void *state, size_t state_bytes, void *ws, size_t ws_bytes, icon_stream_t stream);
+int icon_lbs_backward(const icon_lbs_model *m, int B, const void *state, size_t state_bytes, const float *grad_verts,
+                      const float *grad_joints, float *grad_betas, float *grad_pose, void *ws, size_t ws_bytes,
+                      icon_stream_t stream);
+
 /* ------------------------------------------------------------------ encoder operators
  * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
  * two take NCHW fp32 tensors; every 2-D convolution and normalisation runs on the NHWC path after them. */
