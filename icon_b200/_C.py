@@ -104,6 +104,11 @@ _SIGS = {
     "icon_lbs_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "icon_lbs_forward": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "icon_lbs_backward": (_i, [_vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_smplx_heads_prepare": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i,
+                                      _vp]),
+    "icon_smplx_heads_state_bytes": (_sz, [_i, _i, _i]),
+    "icon_smplx_heads_forward": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_smplx_heads_backward": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "icon_mc_workspace_bytes": (_sz, [_i, _i]),
     "icon_mc_count": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _sz, _vp, _vp]),
     "icon_mc_emit": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _vp, _vp, _i64, _i64, _vp]),
@@ -128,6 +133,13 @@ class LbsModel(ctypes.Structure):
     """icon_lbs_model (include/icon_b200.h): one body model's sizes, parents and device buffers."""
     _fields_ = [("V", _i), ("J", _i), ("NB", _i), ("parents", _i * 64), ("v_template", _vp), ("shapedirs", _vp),
                 ("posedirs", _vp), ("J_regressor", _vp), ("lbs_weights", _vp), ("J_template", _vp), ("J_dirs", _vp)]
+
+
+class SmplxHeads(ctypes.Structure):
+    """icon_smplx_heads (include/icon_b200.h): PIXIE's landmark / joint head tables of one SMPL-X model."""
+    _fields_ = [("V", _i), ("J", _i), ("R", _i), ("Ls", _i), ("Ld", _i), ("E", _i), ("nchain", _i),
+                ("chain", _i * 8), ("regressor", _vp), ("vid", _vp), ("bc", _vp), ("joint_reg", _vp),
+                ("reg_joint", _vp), ("inc_off", _vp), ("inc", _vp)]
 
 
 class IconError(RuntimeError):

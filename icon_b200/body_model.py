@@ -8,6 +8,10 @@
                   the overlay's binding of lib.smplx.body_models.lbs: fp32 CUDA calls on an unbatched v_template, with
                   no model buffer requiring grad and return_transformation=False, go to the kernels; every other call
                   (CPU, float64, a batched v_template, return_transformation=True) goes to the reference's own lbs.
+  make_pixie_SMPLX(reference_SMPLX)
+                  the overlay's patch of lib.pixielib.models.SMPLX.SMPLX: the same class, whose forward runs PIXIE's
+                  skinning on the same kernels and its landmark / joint heads on the heads kernels (_Heads, composed
+                  after _Lbs); calls that are not fp32 CUDA on one device go to the reference's forward.
 
 A model's prepared constants (J_template = J_regressor v_template, J_dirs = J_regressor shapedirs, the parents) are
 cached on the buffer tensors' identity and version, for several models at once: PyMAF's SMPL and the dataset's SMPL
@@ -213,3 +217,240 @@ def make_lbs(reference_lbs):
                              pose2rot=pose2rot, return_transformation=return_transformation)
     lbs_dispatch.reference = reference_lbs
     return lbs_dispatch
+
+
+# ---------------------------------------------------------------- PIXIE's SMPL-X: the skinning plus the heads
+
+LUT_ROWS = 79
+MAX_CHAIN = 8
+MAX_REG_ROWS = 64
+HEAD_BUFFERS = ("faces_tensor", "lmk_faces_idx", "lmk_bary_coords", "dynamic_lmk_faces_idx", "dynamic_lmk_bary_coords",
+                "head_kin_chain", "extra_joint_regressor", "source_idxs", "target_idxs")
+_NO_FACES = torch.empty(0, dtype=torch.long)          # the key's stand-ins when the model has no extra joints
+_NO_BCS = torch.empty(0, 3)
+
+
+def _host(t, dtype):
+    import numpy as np
+    return np.ascontiguousarray(t.detach().cpu().numpy(), dtype=dtype)
+
+
+def check_heads(V, J, faces, lmk_faces_idx, lmk_bary_coords, dynamic_lmk_faces_idx, dynamic_lmk_bary_coords,
+                head_kin_chain, face_ids, bcs, extra_joint_regressor, source_idxs, target_idxs):
+    """The host-side checks of PIXIE SMPLX's head buffers (shapes: ValueError; indices out of range: IconError, as the
+    kernels' prepare would raise); returns the host tables icon_smplx_heads_prepare takes."""
+    import numpy as np
+    pre = "pixie SMPLX:"
+
+    def shape(name, t, want):
+        if t.dim() != len(want) or any(w is not None and s != w for s, w in zip(t.shape, want)):
+            dims = ",".join("n" if w is None else str(w) for w in want)
+            raise ValueError(f"{pre} {name} {tuple(t.shape)} must be [{dims}]")
+    shape("faces_tensor", faces, (None, 3))
+    shape("lmk_faces_idx", lmk_faces_idx, (None,))
+    Ls = lmk_faces_idx.shape[0]
+    shape("lmk_bary_coords", lmk_bary_coords, (Ls, 3))
+    shape("dynamic_lmk_faces_idx", dynamic_lmk_faces_idx, (LUT_ROWS, None))
+    Ld = dynamic_lmk_faces_idx.shape[1]
+    shape("dynamic_lmk_bary_coords", dynamic_lmk_bary_coords, (LUT_ROWS, Ld, 3))
+    shape("extra_joint_selector.face_ids", face_ids, (None,))
+    shape("extra_joint_selector.bcs", bcs, (face_ids.shape[0], 3))
+    shape("extra_joint_regressor", extra_joint_regressor, (None, V))
+    R = extra_joint_regressor.shape[0]
+    if not 1 <= R <= MAX_REG_ROWS:
+        raise ValueError(f"{pre} extra_joint_regressor has {R} rows, the kernels take 1..{MAX_REG_ROWS}")
+    shape("source_idxs", source_idxs, (None,))
+    shape("target_idxs", target_idxs, (source_idxs.shape[0],))
+    shape("head_kin_chain", head_kin_chain, (None,))
+    if not 1 <= head_kin_chain.shape[0] <= MAX_CHAIN:
+        raise ValueError(f"{pre} head_kin_chain has {head_kin_chain.shape[0]} joints, the kernels take 1..{MAX_CHAIN}")
+    h = dict(faces=_host(faces, np.int64), lmk=_host(lmk_faces_idx, np.int64), lmk_bc=_host(lmk_bary_coords, np.float32),
+             dyn=_host(dynamic_lmk_faces_idx, np.int64), dyn_bc=_host(dynamic_lmk_bary_coords, np.float32),
+             ext=_host(face_ids, np.int64), ext_bc=_host(bcs, np.float32), src=_host(source_idxs, np.int64),
+             tgt=_host(target_idxs, np.int64), chain=_host(head_kin_chain, np.int64))
+    F = h["faces"].shape[0]
+    for name, ids in (("lmk_faces_idx", h["lmk"]), ("dynamic_lmk_faces_idx", h["dyn"]),
+                      ("extra_joint_selector.face_ids", h["ext"])):
+        bad = np.argwhere((ids < 0) | (ids >= F))
+        if len(bad):
+            i = tuple(int(x) for x in bad[0])
+            raise _C.IconError(f"{pre} {name}{list(i)} = {int(ids[i])}, a face id outside [0,{F}) "
+                               f"(faces_tensor {tuple(faces.shape)})")
+        used = h["faces"][ids.reshape(-1)]
+        bad = np.argwhere((used < 0) | (used >= V))
+        if len(bad):
+            f = int(ids.reshape(-1)[bad[0][0]])
+            raise _C.IconError(f"{pre} faces_tensor[{f}] = {h['faces'][f].tolist()} (used by {name}) has a vertex id "
+                               f"outside [0,{V}) (v_template ({V}, 3))")
+    for name, ids, n in (("head_kin_chain", h["chain"], J), ("source_idxs", h["src"], J), ("target_idxs", h["tgt"], R)):
+        bad = np.argwhere((ids < 0) | (ids >= n))
+        if len(bad):
+            i = int(bad[0][0])
+            what = f"extra_joint_regressor {tuple(extra_joint_regressor.shape)}" if name == "target_idxs" else \
+                f"{J} skinned joints"
+            raise _C.IconError(f"{pre} {name}[{i}] = {int(ids[i])} outside [0,{n}) ({what})")
+        if name != "head_kin_chain" and len(set(ids.tolist())) != len(ids):
+            raise _C.IconError(f"{pre} {name} {ids.tolist()} repeats an index")
+    return h
+
+
+class PreparedHeads:
+    """One SMPL-X model's head tables on the device (icon_smplx_heads), written by icon_smplx_heads_prepare."""
+
+    def __init__(self, V, J, regressor, h):
+        dev = regressor.device
+        Ls, Ld, E = h["lmk"].shape[0], h["dyn"].shape[1], h["ext"].shape[0]
+        N = 3 * (Ls + LUT_ROWS * Ld + E)
+        self.V, self.J, self.R, self.L, self.E = V, J, regressor.shape[0], Ls + Ld, E
+        self.regressor = regressor.detach().to(torch.float32).contiguous()
+        i32 = dict(dtype=torch.int32, device=dev)
+        self.arrays = dict(vid=torch.empty(max(N, 1), **i32), bc=torch.empty(max(N, 1), dtype=torch.float32, device=dev),
+                           joint_reg=torch.empty(J, **i32), reg_joint=torch.empty(self.R, **i32),
+                           inc_off=torch.empty(V + 1, **i32), inc=torch.empty(max(N, 1), **i32))
+        self.c = _C.SmplxHeads(V, J, self.R, 0, 0, 0, 0, (ctypes.c_int * 8)(), _p(self.regressor),
+                               *(_p(self.arrays[k]) for k in ("vid", "bc", "joint_reg", "reg_joint", "inc_off", "inc")))
+        S = h["src"].shape[0]
+        with torch.cuda.device(dev):
+            check(lib.icon_smplx_heads_prepare(
+                ctypes.byref(self.c), h["faces"].ctypes.data, h["faces"].shape[0], h["lmk"].ctypes.data,
+                h["lmk_bc"].ctypes.data, Ls, h["dyn"].ctypes.data, h["dyn_bc"].ctypes.data, Ld, h["ext"].ctypes.data,
+                h["ext_bc"].ctypes.data, E, h["src"].ctypes.data, h["tgt"].ctypes.data, S, h["chain"].ctypes.data,
+                h["chain"].shape[0], _stream()), "icon_smplx_heads_prepare")
+
+
+_HEADS = ModelCache()
+
+
+def _head_buffers(module):
+    sel = getattr(module, "extra_joint_selector", None)
+    face_ids, bcs = (sel.face_ids, sel.bcs) if sel is not None else (_NO_FACES, _NO_BCS)
+    return [getattr(module, k) for k in HEAD_BUFFERS[:6]] + [face_ids, bcs] + \
+        [getattr(module, k) for k in HEAD_BUFFERS[6:]]
+
+
+def prepared_heads(module):
+    """The cached PreparedHeads of a PIXIE SMPLX module's buffers (keyed on the tensors themselves, as the models)."""
+    key = tuple([module.v_template] + _head_buffers(module))
+    hit = _HEADS.get(key)
+    if hit is not None:
+        return hit
+    V, J = module.v_template.shape[0], module.J_regressor.shape[0]
+    h = check_heads(V, J, *key[1:])
+    return _HEADS.put(key, PreparedHeads(V, J, module.extra_joint_regressor, h))
+
+
+class _Heads(torch.autograd.Function):
+    """(verts [B,V,3], J_transformed [B,J,3], pose [B,J,3,3], PreparedHeads) -> (landmarks [B,Ls+Ld,3],
+    joints [B,J+Ls+Ld+E,3], rows [B] int32, not differentiable).  Composed after _Lbs; pose is not differentiated."""
+
+    @staticmethod
+    def forward(ctx, verts, jt, pose, heads):
+        B, dev = verts.shape[0], verts.device
+        v32, j32 = verts.detach().contiguous(), jt.detach().contiguous()
+        p32 = pose.detach().to(torch.float32).reshape(B, heads.J, 9).contiguous()
+        lm = torch.empty(B, heads.L, 3, dtype=torch.float32, device=dev)
+        joints = torch.empty(B, heads.J + heads.L + heads.E, 3, dtype=torch.float32, device=dev)
+        rows = torch.empty(B, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            sbytes = lib.icon_smplx_heads_state_bytes(B, heads.V, heads.R)
+            state = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+            check(lib.icon_smplx_heads_forward(ctypes.byref(heads.c), B, _p(v32), _p(j32), _p(p32), _p(lm),
+                                               _p(joints), _p(rows), _p(state), sbytes, _stream()),
+                  "icon_smplx_heads_forward")
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(rows)
+        ctx.saved = (heads, rows, B) if any(ctx.needs_input_grad[:2]) else None
+        return lm, joints, rows
+
+    @staticmethod
+    def backward(ctx, g_lm, g_joints, _g_rows):
+        if ctx.saved is None or (g_lm is None and g_joints is None):
+            return None, None, None, None
+        heads, rows, B = ctx.saved
+        dev = rows.device
+        gl, gj = (g.detach().to(dev, torch.float32).contiguous() if g is not None else None for g in (g_lm, g_joints))
+        gv = torch.empty(B, heads.V, 3, dtype=torch.float32, device=dev)
+        gjt = torch.empty(B, heads.J, 3, dtype=torch.float32, device=dev) if gj is not None else None
+        with torch.cuda.device(dev):
+            check(lib.icon_smplx_heads_backward(ctypes.byref(heads.c), B, _p(rows), _p(gl), _p(gj), _p(gv), _p(gjt),
+                                                _stream()), "icon_smplx_heads_backward")
+        return (gv if ctx.needs_input_grad[0] else None, gjt if ctx.needs_input_grad[1] else None, None, None)
+
+
+def pixie_smplx(module, shape_components, full_pose):
+    """PIXIE SMPLX.forward's body after its torch.cats, on the kernels: (vertices [B,V,3], landmarks [B,Ls+Ld,3],
+    joints [B,J+Ls+Ld+E,3], lookup-table rows [B] int32).  The model is the module's own v_template [V,3] and
+    buffers (never the per-call expand view, which would miss the cache)."""
+    bufs = (module.v_template, module.shapedirs, module.posedirs, module.J_regressor, module.parents,
+            module.lbs_weights)
+    model = prepared(*bufs, shape_components, full_pose, False)
+    check_inputs(shape_components, full_pose, model.V, model.J, model.NB, False)
+    heads = prepared_heads(module)
+    verts, jt = _Lbs.apply(shape_components, full_pose, model, False)
+    lm, joints, rows = _Heads.apply(verts, jt, full_pose, heads)
+    return verts, lm, joints, rows
+
+
+def _pixie_fill(module, shape_params, expression_params, global_pose, body_pose, jaw_pose, eye_pose, left_hand_pose,
+                right_hand_pose):
+    """SMPLX.forward's default-filling of None arguments (lib/pixielib/models/SMPLX.py:223-247)."""
+    if shape_params is None:
+        batch_size = global_pose.shape[0]
+        shape_params = module.shape_params.expand(batch_size, -1)
+    else:
+        batch_size = shape_params.shape[0]
+    if expression_params is None:
+        expression_params = module.expression_params.expand(batch_size, -1)
+    poses = []
+    for name, p in (("global_pose", global_pose), ("body_pose", body_pose), ("jaw_pose", jaw_pose),
+                    ("eye_pose", eye_pose), ("left_hand_pose", left_hand_pose), ("right_hand_pose", right_hand_pose)):
+        poses.append(getattr(module, name).unsqueeze(0).expand(batch_size, -1, -1, -1) if p is None else p)
+    return [shape_params, expression_params] + poses
+
+
+def pixie_on_kernels(module, filled):
+    """Whether make_pixie_SMPLX's forward sends a call (its filled arguments) to the kernels: every argument and
+    float buffer fp32 CUDA, every buffer on the arguments' device, no buffer requiring grad, the joint regressor on."""
+    if not getattr(module, "use_joint_regressor", False) or not all(torch.is_tensor(t) for t in filled):
+        return False
+    dev = filled[0].device
+    floats = list(filled) + [module.v_template, module.shapedirs, module.posedirs, module.J_regressor,
+                             module.lbs_weights, module.lmk_bary_coords, module.dynamic_lmk_bary_coords,
+                             module.extra_joint_regressor]
+    sel = getattr(module, "extra_joint_selector", None)
+    if sel is not None:
+        floats.append(sel.bcs)
+    if not all(t.is_cuda and t.dtype == torch.float32 and t.device == dev for t in floats):
+        return False
+    index = [module.parents, module.faces_tensor, module.lmk_faces_idx, module.dynamic_lmk_faces_idx,
+             module.head_kin_chain, module.source_idxs, module.target_idxs] + ([sel.face_ids] if sel is not None else [])
+    if not all(t.device == dev for t in index):
+        return False
+    return not any(t.requires_grad for t in floats[len(filled):])
+
+
+def make_pixie_SMPLX(reference_SMPLX):
+    """lib.pixielib.models.SMPLX's `SMPLX`: the reference's own class, with a `forward` that runs the skinning and the
+    heads on the kernels where pixie_on_kernels holds and calls the reference's forward, unchanged, for every other
+    call.  The class is patched in place, not subclassed: the reference's `__init__` calls `super(SMPLX, self)`
+    through the module's global name, which must stay the class itself.  Patching twice keeps the first original."""
+    reference_forward = reference_SMPLX.__dict__.get("_icon_b200_reference_forward", reference_SMPLX.forward)
+
+    def forward(self, shape_params=None, expression_params=None, global_pose=None, body_pose=None, jaw_pose=None,
+                eye_pose=None, left_hand_pose=None, right_hand_pose=None):
+        args = (shape_params, expression_params, global_pose, body_pose, jaw_pose, eye_pose, left_hand_pose,
+                right_hand_pose)
+        filled = _pixie_fill(self, *args)
+        if not pixie_on_kernels(self, filled):
+            return reference_forward(self, *args)
+        shape_components = torch.cat(filled[:2], dim=1)
+        full_pose = torch.cat(filled[2:], dim=1)
+        verts, landmarks, joints, _ = pixie_smplx(self, shape_components, full_pose)
+        return verts, landmarks, joints
+
+    forward.reference = reference_forward
+    forward.__doc__ = reference_forward.__doc__
+    forward.__qualname__ = reference_forward.__qualname__
+    reference_SMPLX.forward = forward
+    reference_SMPLX._icon_b200_reference_forward = reference_forward
+    return reference_SMPLX

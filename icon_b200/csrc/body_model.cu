@@ -34,7 +34,33 @@
 // Layout of a call's state (icon_lbs_state_bytes): a header (pose2rot), R [B,J,9], G [B,J,12], A [B,J,12],
 //   J [B,J,3], r [B,J,3] (pose2rot only), v_posed [B,V,3], all fp64.
 // -fmad=false, as the other geometry units.
+//
+// Heads: the landmark and joint heads of PIXIE's SMPLX.forward (lib/pixielib/models/SMPLX.py:261-293, lbs.py:38-145,
+// 427-434), read from the fp32 `verts` icon_lbs_forward wrote, as the reference reads its own.  Restated by the heads
+// part of oracle/body_model.py; pinned against the reference's class by tests/golden/pixie_body_model.npz.
+//   Prepared once per model (icon_smplx_heads_prepare, host-checked): corner vertex ids and barycentrics of the
+//   static landmarks [Ls,3], the lookup table [79,Ld,3] and the extra joints [E,3] ("slots", in that order), the
+//   regressor row written over each joint (source_idxs / target_idxs), the head chain, and per vertex the slots that
+//   read it, in (entry, table row, corner) order.
+//   Forward, per batch item b (fp64 from the fp32 inputs; each output rounded to fp32 once):
+//     row: rel = I, rel <- R[chain[i]] rel for i ascending (the pose as given; the reference detaches it, so the
+//       row is not differentiated); a = (-atan2(-rel[2,0], sqrt(rel00^2 + rel10^2)) 180) / pi;
+//       y = round_half_even(min(a, 39)); row = y >= 0 ? y : (y < -39 ? 78 : 39 - y).  The reference computes rel in
+//       fp32: the row equals the reference's wherever a is at least 1e-3 degrees from a half-integer (fp32 rounding
+//       of the six 3x3 products moves a by about 1e-4 degrees for matrices with entries of order 1).
+//     landmark / extra entry = (w0 v[i0] + w1 v[i1]) + w2 v[i2] (corner order); the dynamic entries use table row
+//       `row`.  reg[r] = sum over v of R[r,v] v[v]: per chunk of HEADS_CV vertices a warp's lanes sum their
+//       vertices in ascending order and a fixed xor-butterfly adds the lanes; the chunks are added in ascending
+//       order.  joints = cat[J_transformed, landmarks, extra] with joints[source_s] = reg[target_s] (the
+//       reference's `detach() * 0 + reg`, equal to reg for a finite J_transformed).
+//   Backward (NULL upstreams are zero; fp32 g_verts_heads, one thread per (b, vertex column)): u_e =
+//     g_landmarks[e] + g_joints[J + e]; g_v = sum over the slots reading v, in `inc` order, of w_slot u_e (the
+//     dynamic slots of other table rows skipped), then + sum over r ascending of R[r,v] g_joints[source of r].
+//     g_J_transformed = g_joints[:, :J] with zeros at the sources (the `detach() * 0`).  No float atomics.
+//   Launches: two forward (k_heads_reg_partial, k_heads_finish), one backward (k_heads_backward).
 #include <math.h>
+
+#include <vector>
 
 #include "common.cuh"
 
@@ -479,6 +505,147 @@ static bool lbs_model_ok(const icon_lbs_model *m) {
            (int64_t)m->V * 3 <= INT32_MAX;
 }
 
+// ---------------------------------------------------------------- SMPL-X heads (PIXIE)
+
+constexpr int HEADS_LUT = ICON_HEADS_LUT_ROWS;
+constexpr int HEADS_MAXR = 64;
+constexpr int HEADS_CV = 256;           // vertices per regressor chunk
+constexpr int HEADS_T = 256;
+
+static inline int heads_chunks(int V) { return (V + HEADS_CV - 1) / HEADS_CV; }
+
+// the table row of one batch item: rel <- R[chain[i]] rel for i ascending, the reference's Euler angle and rounding
+__device__ __forceinline__ int heads_lut_row(const icon_smplx_heads &h, const float *__restrict__ pose_b) {
+    double rel[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+#pragma unroll
+    for (int i = 0; i < ICON_HEADS_MAX_CHAIN; ++i) {     // static indices: the chain stays in the parameter space
+        if (i >= h.nchain) break;
+        const float *Rm = pose_b + 9 * h.chain[i];
+        double n[9];
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+                n[3 * r + c] = ((double)Rm[3 * r] * rel[c] + (double)Rm[3 * r + 1] * rel[3 + c]) +
+                               (double)Rm[3 * r + 2] * rel[6 + c];
+#pragma unroll
+        for (int e = 0; e < 9; ++e) rel[e] = n[e];
+    }
+    const double sy = sqrt(rel[0] * rel[0] + rel[3] * rel[3]);
+    const double a = (-atan2(-rel[6], sy) * 180.0) / 3.141592653589793;
+    const double y = rint(fmin(a, 39.0));          // round half to even, as torch.round
+    if (y >= 0.0) return (int)y;
+    return y < -39.0 ? 78 : 39 - (int)y;
+}
+
+// one CTA per (vertex chunk, batch item): a warp per output q = 3 r + c, each lane over its vertices in ascending
+// order, then the fixed butterfly
+__global__ void __launch_bounds__(HEADS_T) k_heads_reg_partial(icon_smplx_heads h, const float *__restrict__ verts,
+                                                               double *__restrict__ part) {
+    const int s = blockIdx.x, b = blockIdx.y, S = gridDim.x, Q = 3 * h.R;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int v0 = s * HEADS_CV, nv = min(HEADS_CV, h.V - v0);
+    const float *vb = verts + (size_t)b * h.V * 3;
+    for (int q = warp; q < Q; q += HEADS_T / 32) {
+        const int r = q / 3, c = q % 3;
+        const float *Rr = h.regressor + (size_t)r * h.V + v0;
+        double acc = 0.0;
+        for (int i = lane; i < nv; i += 32) acc = acc + (double)__ldg(Rr + i) * (double)vb[3 * (size_t)(v0 + i) + c];
+        acc = warp_sum_fixed(acc);
+        if (lane == 0) part[((size_t)b * S + s) * Q + q] = acc;
+    }
+}
+
+// one CTA per batch item: the table row, the chunk partials in ascending order, the landmarks, the extra joints and
+// the joint set
+__global__ void __launch_bounds__(HEADS_T) k_heads_finish(icon_smplx_heads h, int S, const double *__restrict__ part,
+                                                          const float *__restrict__ verts,
+                                                          const float *__restrict__ jl, const float *__restrict__ pose,
+                                                          float *__restrict__ landmarks, float *__restrict__ joints,
+                                                          int *__restrict__ rows) {
+    __shared__ double s_reg[3 * HEADS_MAXR];
+    __shared__ int s_row;
+    const int b = blockIdx.x, t = threadIdx.x, J = h.J, L = h.Ls + h.Ld, NJ = J + L + h.E, Q = 3 * h.R;
+    if (t == 0) {
+        s_row = heads_lut_row(h, pose + (size_t)b * J * 9);
+        rows[b] = s_row;
+    }
+    for (int q = t; q < Q; q += HEADS_T) {
+        double acc = 0.0;
+        for (int s = 0; s < S; ++s) acc = acc + part[((size_t)b * S + s) * Q + q];
+        s_reg[q] = acc;
+    }
+    __syncthreads();
+    const float *vb = verts + (size_t)b * h.V * 3;
+    for (int o = t; o < 3 * NJ; o += HEADS_T) {
+        const int e = o / 3, c = o % 3;
+        double val;
+        if (e < J) {
+            const int r = h.joint_reg[e];
+            val = r >= 0 ? s_reg[3 * r + c] : (double)jl[((size_t)b * J + e) * 3 + c];
+        } else {
+            const int k = e - J;
+            const int slot = 3 * (k < h.Ls ? k : k < L ? h.Ls + s_row * h.Ld + (k - h.Ls)
+                                                       : h.Ls + HEADS_LUT * h.Ld + (k - L));
+            val = ((double)h.bc[slot] * (double)vb[3 * h.vid[slot] + c] +
+                   (double)h.bc[slot + 1] * (double)vb[3 * h.vid[slot + 1] + c]) +
+                  (double)h.bc[slot + 2] * (double)vb[3 * h.vid[slot + 2] + c];
+            if (k < L) landmarks[((size_t)b * L + k) * 3 + c] = (float)val;
+        }
+        joints[((size_t)b * NJ + e) * 3 + c] = (float)val;
+    }
+}
+
+// a thread per (batch item, vertex column 3 v + c): the slots that read v in `inc` order, then the regressor rows
+// in ascending order; the threads past 3V write the skinned joints' gradient
+__global__ void __launch_bounds__(HEADS_T) k_heads_backward(icon_smplx_heads h, const int *__restrict__ rows,
+                                                            const float *__restrict__ gl,
+                                                            const float *__restrict__ gj, float *__restrict__ gv,
+                                                            float *__restrict__ gjl) {
+    const int b = blockIdx.y, J = h.J, L = h.Ls + h.Ld, NJ = J + L + h.E;
+    const int64_t V3 = 3 * (int64_t)h.V, col = (int64_t)blockIdx.x * HEADS_T + threadIdx.x;
+    if (col < V3) {
+        const int v = (int)(col / 3), c = (int)(col % 3), row = rows[b];
+        const int dyn0 = 3 * h.Ls, dyn1 = 3 * (h.Ls + HEADS_LUT * h.Ld);
+        double acc = 0.0;
+        for (int i = h.inc_off[v]; i < h.inc_off[v + 1]; ++i) {
+            const int slot = h.inc[i];
+            int k;
+            if (slot < dyn0) {
+                k = slot / 3;
+            } else if (slot < dyn1) {
+                const int d = slot / 3 - h.Ls;
+                if (d / h.Ld != row) continue;
+                k = h.Ls + d % h.Ld;
+            } else {
+                k = L + (slot - dyn1) / 3;
+            }
+            double u = 0.0;
+            if (gl && k < L) u = (double)gl[((size_t)b * L + k) * 3 + c];
+            if (gj) u = u + (double)gj[((size_t)b * NJ + J + k) * 3 + c];
+            acc = acc + (double)h.bc[slot] * u;
+        }
+        if (gj)
+            for (int r = 0; r < h.R; ++r) {
+                const int j = h.reg_joint[r];
+                if (j >= 0)
+                    acc = acc + (double)__ldg(h.regressor + (size_t)r * h.V + v) *
+                                    (double)gj[((size_t)b * NJ + j) * 3 + c];
+            }
+        gv[(size_t)b * V3 + col] = (float)acc;
+    } else if (gjl && col < V3 + 3 * J) {
+        const int o = (int)(col - V3), j = o / 3;
+        gjl[(size_t)b * 3 * J + o] = h.joint_reg[j] >= 0 ? 0.0f : gj[((size_t)b * NJ + j) * 3 + o % 3];
+    }
+}
+
+static bool heads_ok(const icon_smplx_heads *h) {
+    return h && h->V > 0 && (int64_t)h->V * 3 <= INT32_MAX && h->J >= 2 && h->J <= LBS_MAXJ && h->R >= 1 &&
+           h->R <= HEADS_MAXR && h->Ls >= 0 && h->Ld >= 0 && h->E >= 0 && h->nchain >= 1 &&
+           h->nchain <= ICON_HEADS_MAX_CHAIN && h->regressor && h->vid && h->bc && h->joint_reg && h->reg_joint &&
+           h->inc_off && h->inc;
+}
+
 }  // namespace icon
 
 // ---------------------------------------------------------------- C ABI
@@ -569,6 +736,138 @@ extern "C" int icon_lbs_backward(const icon_lbs_model *m, int B, const void *sta
     }
     k_lbs_chain_backward<<<(unsigned)B, LBS_CB_T, 0, stream>>>(*m, st, grad_verts ? (const double *)ws : nullptr,
                                                                tiles, grad_joints, grad_betas, grad_pose);
+    ICON_LAUNCHED();
+    return ICON_OK;
+}
+
+// ---------------------------------------------------------------- C ABI: SMPL-X heads
+
+extern "C" int icon_smplx_heads_prepare(icon_smplx_heads *h, const int64_t *h_faces, int F,
+                                        const int64_t *h_lmk_faces_idx, const float *h_lmk_bary, int Ls,
+                                        const int64_t *h_dyn_faces_idx, const float *h_dyn_bary, int Ld,
+                                        const int64_t *h_face_ids, const float *h_bcs, int E,
+                                        const int64_t *h_source, const int64_t *h_target, int S,
+                                        const int64_t *h_chain, int nchain, icon_stream_t stream_) {
+    using namespace icon;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    ICON_CHECK_ARG(h && h_faces && h_chain, "icon_smplx_heads_prepare: null pointer");
+    ICON_CHECK_ARG(F >= 1 && Ls >= 0 && Ld >= 0 && E >= 0 && S >= 0,
+                   "icon_smplx_heads_prepare: bad sizes F=%d Ls=%d Ld=%d E=%d S=%d", F, Ls, Ld, E, S);
+    ICON_CHECK_ARG((Ls == 0 || (h_lmk_faces_idx && h_lmk_bary)) && (Ld == 0 || (h_dyn_faces_idx && h_dyn_bary)) &&
+                   (E == 0 || (h_face_ids && h_bcs)) && (S == 0 || (h_source && h_target)),
+                   "icon_smplx_heads_prepare: null table");
+    ICON_CHECK_ARG(nchain >= 1 && nchain <= ICON_HEADS_MAX_CHAIN,
+                   "icon_smplx_heads_prepare: head chain of %d joints, the kernels take 1..%d", nchain,
+                   ICON_HEADS_MAX_CHAIN);
+    h->Ls = Ls;
+    h->Ld = Ld;
+    h->E = E;
+    h->nchain = nchain;
+    ICON_CHECK_ARG(heads_ok(h), "icon_smplx_heads_prepare: null buffer or bad sizes V=%d J=%d R=%d", h->V, h->J,
+                   h->R);
+    const int V = h->V, J = h->J, R = h->R;
+    for (int i = 0; i < nchain; ++i) {
+        ICON_CHECK_ARG(h_chain[i] >= 0 && h_chain[i] < J,
+                       "icon_smplx_heads_prepare: head_kin_chain[%d] = %lld outside [0,%d)", i,
+                       (long long)h_chain[i], J);
+        h->chain[i] = (int)h_chain[i];
+    }
+    for (int i = nchain; i < ICON_HEADS_MAX_CHAIN; ++i) h->chain[i] = 0;
+    // slots in table order: static [Ls,3], the lookup table [79,Ld,3], extra [E,3]
+    const int nf = Ls + HEADS_LUT * Ld + E, N = 3 * nf;
+    std::vector<int> vid(N), joint_reg(J, -1), reg_joint(R, -1), off(V + 1, 0), inc(N);
+    std::vector<float> bc(N);
+    struct Tab { const char *name; const int64_t *f; const float *w; int n; int base; };
+    const Tab tabs[3] = {{"lmk_faces_idx", h_lmk_faces_idx, h_lmk_bary, Ls, 0},
+                         {"dynamic_lmk_faces_idx", h_dyn_faces_idx, h_dyn_bary, HEADS_LUT * Ld, Ls},
+                         {"face_ids", h_face_ids, h_bcs, E, Ls + HEADS_LUT * Ld}};
+    for (const Tab &t : tabs)
+        for (int i = 0; i < t.n; ++i) {
+            const int64_t f = t.f[i];
+            ICON_CHECK_ARG(f >= 0 && f < F, "icon_smplx_heads_prepare: %s[%d] = %lld, a face id outside [0,%d)",
+                           t.name, i, (long long)f, F);
+            for (int k = 0; k < 3; ++k) {
+                const int64_t v = h_faces[3 * f + k];
+                ICON_CHECK_ARG(v >= 0 && v < V,
+                               "icon_smplx_heads_prepare: faces[%lld][%d] = %lld (used by %s[%d]), a vertex id "
+                               "outside [0,%d)", (long long)f, k, (long long)v, t.name, i, V);
+                vid[3 * (t.base + i) + k] = (int)v;
+                bc[3 * (t.base + i) + k] = t.w[3 * i + k];
+            }
+        }
+    for (int s = 0; s < S; ++s) {
+        ICON_CHECK_ARG(h_source[s] >= 0 && h_source[s] < J,
+                       "icon_smplx_heads_prepare: source_idxs[%d] = %lld outside [0,%d)", s, (long long)h_source[s],
+                       J);
+        ICON_CHECK_ARG(h_target[s] >= 0 && h_target[s] < R,
+                       "icon_smplx_heads_prepare: target_idxs[%d] = %lld outside [0,%d)", s, (long long)h_target[s],
+                       R);
+        ICON_CHECK_ARG(joint_reg[h_source[s]] < 0 && reg_joint[h_target[s]] < 0,
+                       "icon_smplx_heads_prepare: source_idxs / target_idxs[%d] repeats an index", s);
+        joint_reg[h_source[s]] = (int)h_target[s];
+        reg_joint[h_target[s]] = (int)h_source[s];
+    }
+    // per-vertex slot lists, stable in (entry, table row, corner) order: a counting sort of that enumeration
+    std::vector<int> order;
+    order.reserve(N);
+    for (int i = 0; i < 3 * Ls; ++i) order.push_back(i);
+    for (int l = 0; l < Ld; ++l)
+        for (int row = 0; row < HEADS_LUT; ++row)
+            for (int k = 0; k < 3; ++k) order.push_back(3 * (Ls + row * Ld + l) + k);
+    for (int i = 3 * (Ls + HEADS_LUT * Ld); i < N; ++i) order.push_back(i);
+    for (int slot : order) ++off[vid[slot] + 1];
+    for (int v = 0; v < V; ++v) off[v + 1] += off[v];
+    std::vector<int> fill(off.begin(), off.end() - 1);
+    for (int slot : order) inc[fill[vid[slot]]++] = slot;
+    if (N > 0) {
+        ICON_CUDA(cudaMemcpyAsync(h->vid, vid.data(), N * sizeof(int), cudaMemcpyHostToDevice, stream));
+        ICON_CUDA(cudaMemcpyAsync(h->bc, bc.data(), N * sizeof(float), cudaMemcpyHostToDevice, stream));
+        ICON_CUDA(cudaMemcpyAsync(h->inc, inc.data(), N * sizeof(int), cudaMemcpyHostToDevice, stream));
+    }
+    ICON_CUDA(cudaMemcpyAsync(h->joint_reg, joint_reg.data(), J * sizeof(int), cudaMemcpyHostToDevice, stream));
+    ICON_CUDA(cudaMemcpyAsync(h->reg_joint, reg_joint.data(), R * sizeof(int), cudaMemcpyHostToDevice, stream));
+    ICON_CUDA(cudaMemcpyAsync(h->inc_off, off.data(), (V + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
+    ICON_CUDA(cudaStreamSynchronize(stream));          // the host vectors go out of scope
+    return ICON_OK;
+}
+
+extern "C" size_t icon_smplx_heads_state_bytes(int B, int V, int R) {
+    if (B <= 0 || V <= 0 || R <= 0) return 0;
+    return icon::align_up((size_t)B * icon::heads_chunks(V) * 3 * R * sizeof(double), 256);
+}
+
+extern "C" int icon_smplx_heads_forward(const icon_smplx_heads *h, int B, const float *verts,
+                                        const float *joints_lbs, const float *pose, float *landmarks, float *joints,
+                                        int *rows, void *state, size_t state_bytes, icon_stream_t stream_) {
+    using namespace icon;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    ICON_CHECK_ARG(heads_ok(h), "icon_smplx_heads_forward: heads not prepared");
+    ICON_CHECK_ARG(B > 0 && B <= 65535, "icon_smplx_heads_forward: B=%d", B);
+    ICON_CHECK_ARG(verts && joints_lbs && pose && joints && rows && state && (landmarks || h->Ls + h->Ld == 0),
+                   "icon_smplx_heads_forward: null pointer");
+    ICON_CHECK_ARG(state_bytes >= icon_smplx_heads_state_bytes(B, h->V, h->R),
+                   "icon_smplx_heads_forward: state too small");
+    const int S = heads_chunks(h->V);
+    k_heads_reg_partial<<<dim3((unsigned)S, (unsigned)B), HEADS_T, 0, stream>>>(*h, verts, (double *)state);
+    ICON_LAUNCHED();
+    k_heads_finish<<<(unsigned)B, HEADS_T, 0, stream>>>(*h, S, (const double *)state, verts, joints_lbs, pose,
+                                                        landmarks, joints, rows);
+    ICON_LAUNCHED();
+    return ICON_OK;
+}
+
+extern "C" int icon_smplx_heads_backward(const icon_smplx_heads *h, int B, const int *rows,
+                                         const float *grad_landmarks, const float *grad_joints, float *grad_verts,
+                                         float *grad_joints_lbs, icon_stream_t stream_) {
+    using namespace icon;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    ICON_CHECK_ARG(heads_ok(h), "icon_smplx_heads_backward: heads not prepared");
+    ICON_CHECK_ARG(B > 0 && B <= 65535, "icon_smplx_heads_backward: B=%d", B);
+    ICON_CHECK_ARG(rows && grad_verts && (grad_joints || !grad_joints_lbs),
+                   "icon_smplx_heads_backward: null pointer");
+    const int64_t cols = 3 * ((int64_t)h->V + h->J);
+    k_heads_backward<<<dim3((unsigned)((cols + HEADS_T - 1) / HEADS_T), (unsigned)B), HEADS_T, 0, stream>>>(
+        *h, rows, grad_landmarks, grad_joints, grad_verts, grad_joints ? grad_joints_lbs : nullptr);
     ICON_LAUNCHED();
     return ICON_OK;
 }

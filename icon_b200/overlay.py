@@ -7,7 +7,7 @@
 The reference's `lib` package stays the reference's: every module, helper and constant that is not part of the
 accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.dataset.Evaluator` but for
 `calculate_chamfer_p2s`, `init_gl` and `_render_normal`, `lib.smplx` but for the `lbs` its body models call,
-`lib.common.config`, the rest of
+`lib.pixielib` but for `SMPLX.forward` in `lib/pixielib/models/SMPLX.py`, `lib.common.config`, the rest of
 `train_util` / `mesh_util` / `net_util` ...) is imported from the checkout unchanged.  An import hook on
 `sys.meta_path` then does two things, only for the modules listed below:
 
@@ -21,7 +21,8 @@ accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.
               `Evaluator.calculate_chamfer_p2s`, `Evaluator.init_gl` and `Evaluator._render_normal` in
               `lib/dataset/Evaluator.py`, `Render.get_rendered_video` in `lib/common/render.py`, and in
               `lib/dataset/TestDataset.py` an `__init__` that rebinds `get_rgb_image` / `get_silhouette_image` /
-              `VF2Mesh` on the instance's `self.render` only, `lbs` in `lib/smplx/body_models.py`), so
+              `VF2Mesh` on the instance's `self.render` only, `lbs` in `lib/smplx/body_models.py`, `SMPLX` in
+              `lib/pixielib/models/SMPLX.py`: the same class, its `forward` patched to run on the kernels), so
               `from lib.common.train_util import *` (apps/ICON.py:20) still finds everything else it uses.
 
 Callers and call sites this serves: apps/ICON.py:17-22, 52-90 (HGPIFuNet, Seg3dLossless, query_func, get_visibility),
@@ -30,7 +31,8 @@ render_normal and calculate_normal_consist through _render_normal: no OpenGL con
 apps/infer.py:168-273, 431-505 (the body-fit and cloth loops: differentiable normal / silhouette renders through
 TestDataset.render_normal and render.get_silhouette_image),
 apps/infer.py:175-180 (the body-fit loop's `dataset.smpl_model(...)`: SMPL / SMPLH / SMPLX.forward call `lbs`
-through lib/smplx/body_models.py's namespace; fp32 CUDA calls run the fused skinning kernels, forward and backward),
+through lib/smplx/body_models.py's namespace; fp32 CUDA calls run the fused skinning kernels, forward and backward;
+with `-hps_type pixie` it is PIXIE's SMPLX.forward, whose skinning and landmark / joint heads run on the kernels),
 apps/infer.py:405-476 and apps/ICON.py:483 (the cloth loop's LocalAffine and shape priors; VF2Mesh's differentiable
 vertex colours),
 apps/infer.py:548-562 (`-export_video`: get_rendered_video's 360 views per mesh, a chunk of views per kernel call),
@@ -93,6 +95,7 @@ def _patches():
         "lib.common.render": {"Render": mesh_views.make_Render},            # get_rendered_video
         "lib.dataset.TestDataset": {"TestDataset": mesh_views.make_TestDataset},  # self.render's fit renders, VF2Mesh
         "lib.smplx.body_models": {"lbs": body_model.make_lbs},              # SMPL / SMPLH / SMPLX.forward's skinning
+        "lib.pixielib.models.SMPLX": {"SMPLX": body_model.make_pixie_SMPLX},  # PIXIE's SMPL-X: skinning and heads
     }
 
 

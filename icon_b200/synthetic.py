@@ -289,3 +289,115 @@ def model_arrays(v, parents, NB, rng):
                shapedirs=(0.01 * rng.standard_normal((nv, 3, NB))).astype(np.float32),
                posedirs=(0.01 * rng.standard_normal((9 * (J - 1), 3 * nv))).astype(np.float32),
                parents=np.asarray(parents, np.int64))
+
+
+PIXIE_SIZES = {"tiny": dict(rings=8, segs=12, V=98, F=192, n_shape=10, n_exp=10),
+               "real": dict(rings=100, segs=104, V=10475, F=20908, n_shape=200, n_exp=50)}
+# PIXIE's J14 regressor rows written over SMPL-X joints: SMPLX.__init__'s (source, target) pairs for its
+# keypoint_names and J14_NAMES (lib/pixielib/models/SMPLX.py:186-198)
+PIXIE_J14_SOURCE = [1, 2, 4, 5, 7, 8, 12, 15, 16, 17, 18, 19, 20, 21]
+PIXIE_J14_TARGET = [3, 2, 4, 1, 5, 0, 12, 13, 9, 8, 10, 7, 11, 6]
+PIXIE_HEAD_CHAIN = [15, 12, 9, 6, 3, 0]
+
+
+def pixie_model(kind="tiny", seed=0, grid=None):
+    """Seeded arrays shaped like PIXIE's SMPL-X model file and side files (lib/pixielib/models/SMPLX.py:114-202):
+    v_template [V,3], f [F,3], shapedirs [V,3,300 + n_exp] (the class keeps [:n_shape] and [300:300 + n_exp]; the
+    columns between are zero), posedirs [V,3,9(J-1)] (the file's layout), J_regressor [J,V], kintree_table [2,J],
+    weights [V,J], lmk_faces_idx [51], lmk_bary_coords [51,3], dynamic_lmk_faces_idx [79,17],
+    dynamic_lmk_bary_coords [79,17,3], the extra joints' face_ids [22] / bcs [22,3] and the J14 regressor [14,V];
+    n_shape, n_exp.  "tiny": body_mesh(8, 12) (V 98, F 192), n_shape = n_exp = 10; "real": V 10 475, F 20 908,
+    n_shape 200, n_exp 50 (a closed body_mesh plus loose vertices and faces to SMPL-X's counts).  J = 55 (the
+    smplx_parents() tree).  `grid`: round blend shapes to multiples of 2^-grid.  Barycentrics are positive and sum
+    to about 1."""
+    z = PIXIE_SIZES[kind]
+    rng = np.random.RandomState(seed)
+    v, f = body_mesh(rings=z["rings"], segs=z["segs"], seed=seed)
+    extra_v = z["V"] - len(v)
+    if extra_v:
+        v = np.concatenate([v, (0.05 * rng.standard_normal((extra_v, 3)) + [0.0, 0.85, 0.1]).astype(np.float32)], 0)
+        lo = z["V"] - extra_v
+        tri = np.stack([rng.choice(extra_v, 3, replace=False) + lo for _ in range(z["F"] - len(f))])
+        f = np.concatenate([f, tri.astype(np.int64)], 0)
+    parents = smplx_parents()
+    J, ns, ne = len(parents), z["n_shape"], z["n_exp"]
+    m = model_arrays(v, parents, ns + ne, rng)
+    sd = np.zeros((z["V"], 3, 300 + ne), np.float32)
+    sd[:, :, :ns], sd[:, :, 300:] = m["shapedirs"][:, :, :ns], m["shapedirs"][:, :, ns:]
+    pd = m["posedirs"]
+    if grid is not None:
+        sd = (np.round(sd.astype(np.float64) * 2.0 ** grid) / 2.0 ** grid).astype(np.float32)
+        pd = (np.round(pd.astype(np.float64) * 2.0 ** grid) / 2.0 ** grid).astype(np.float32)
+    F = len(f)
+
+    def bary(*shape):
+        w = rng.uniform(0.05, 1.0, shape + (3,))
+        return (w / w.sum(-1, keepdims=True)).astype(np.float32)
+    j14 = np.zeros((14, z["V"]), np.float64)
+    for r in range(14):
+        near = rng.choice(z["V"], 6, replace=False)
+        w = rng.uniform(0.2, 1.0, 6)
+        j14[r, near] = w / w.sum()
+    kin = np.stack([np.asarray(parents, np.int64), np.arange(J, dtype=np.int64)])
+    kin[0, 0] = 4294967295                     # the file's root entry; the class sets parents[0] = -1
+    return dict(v_template=v.astype(np.float32), f=f.astype(np.int64), shapedirs=sd,
+                posedirs=pd.T.reshape(z["V"], 3, 9 * (J - 1)).copy(), J_regressor=m["J_regressor"],
+                kintree_table=kin, weights=m["lbs_weights"], lmk_faces_idx=rng.randint(0, F, 51).astype(np.int64),
+                lmk_bary_coords=bary(51), dynamic_lmk_faces_idx=rng.randint(0, F, (79, 17)).astype(np.int64),
+                dynamic_lmk_bary_coords=bary(79, 17), face_ids=rng.randint(0, F, 22).astype(np.int64), bcs=bary(22),
+                j14_regressor=j14.astype(np.float32), n_shape=ns, n_exp=ne)
+
+
+def pixie_buffers(arr):
+    """The buffers PIXIE's SMPLX.__init__ registers from pixie_model() arrays (float32 / int64 numpy), by the same
+    slicing and reshapes: v_template, shapedirs [V,3,n_shape + n_exp], posedirs [9(J-1),3V], J_regressor, parents,
+    lbs_weights, faces_tensor, the landmark tables, head_kin_chain, face_ids, bcs, extra_joint_regressor,
+    source_idxs, target_idxs."""
+    ns, ne = arr["n_shape"], arr["n_exp"]
+    P = arr["posedirs"].shape[-1]
+    parents = arr["kintree_table"][0].astype(np.int64).copy()
+    parents[0] = -1
+    return dict(v_template=arr["v_template"], shapedirs=np.concatenate([arr["shapedirs"][:, :, :ns],
+                                                                         arr["shapedirs"][:, :, 300:300 + ne]], 2),
+                posedirs=np.ascontiguousarray(arr["posedirs"].reshape(-1, P).T), J_regressor=arr["J_regressor"],
+                parents=parents, lbs_weights=arr["weights"], faces_tensor=arr["f"],
+                lmk_faces_idx=arr["lmk_faces_idx"], lmk_bary_coords=arr["lmk_bary_coords"],
+                dynamic_lmk_faces_idx=arr["dynamic_lmk_faces_idx"],
+                dynamic_lmk_bary_coords=arr["dynamic_lmk_bary_coords"],
+                head_kin_chain=np.asarray(PIXIE_HEAD_CHAIN, np.int64), face_ids=arr["face_ids"], bcs=arr["bcs"],
+                extra_joint_regressor=arr["j14_regressor"], source_idxs=np.asarray(PIXIE_J14_SOURCE, np.int64),
+                target_idxs=np.asarray(PIXIE_J14_TARGET, np.int64))
+
+
+def pixie_smplx_standin():
+    """A fresh class standing in for PIXIE's SMPLX (lib/pixielib/models/SMPLX.py) where no checkout exists, for
+    body_model.make_pixie_SMPLX to patch: `__init__(buffers, n_shape)` registers what the reference's `__init__` registers,
+    from pixie_buffers() arrays (the extra joints under `extra_joint_selector`, the default poses and parameters as
+    identities and zeros) and calls `super(SMPLX, self).__init__()` as the reference does; `forward(*args)` records
+    its arguments in the class's `calls` list and returns "reference"."""
+    import torch.nn as nn
+
+    class SMPLX(nn.Module):
+        calls = []
+
+        def __init__(self, buffers, n_shape=10):
+            super(SMPLX, self).__init__()
+            for k, v in buffers.items():
+                if k not in ("face_ids", "bcs"):
+                    self.register_buffer(k, torch.as_tensor(np.asarray(v)).clone())
+            self.extra_joint_selector = nn.Module()
+            for k in ("face_ids", "bcs"):
+                self.extra_joint_selector.register_buffer(k, torch.as_tensor(np.asarray(buffers[k])).clone())
+            ne = int(np.asarray(buffers["shapedirs"]).shape[2]) - n_shape
+            self.register_buffer("shape_params", torch.zeros(1, n_shape))
+            self.register_buffer("expression_params", torch.zeros(1, ne))
+            for k, n in (("global_pose", 1), ("body_pose", 21), ("jaw_pose", 1), ("eye_pose", 2),
+                         ("left_hand_pose", 15), ("right_hand_pose", 15)):
+                self.register_buffer(k, torch.eye(3)[None].repeat(n, 1, 1))
+            self.use_joint_regressor = True
+
+        def forward(self, *args):
+            SMPLX.calls.append(args)
+            return "reference"
+
+    return SMPLX

@@ -399,6 +399,49 @@ int icon_lbs_backward(const icon_lbs_model *m, int B, const void *state, size_t 
                       const float *grad_joints, float *grad_betas, float *grad_pose, void *ws, size_t ws_bytes,
                       icon_stream_t stream);
 
+/* ------------------------------------------------------------------ SMPL-X heads (PIXIE's landmarks and joints)
+ * The landmark and joint heads PIXIE's SMPLX.forward (lib/pixielib/models/SMPLX.py) runs on the skinned vertices:
+ * the head-yaw lookup-table row, the static and dynamic face landmarks, the extra joints picked from faces and the
+ * dense joint regressor written over `source` joints.  Rules, tolerances and the backward's order in the "heads"
+ * section of the csrc/body_model.cu header.  No float atomics.
+ *
+ * icon_smplx_heads: the caller fills V, J (2..64), R (regressor rows, 1..64), `regressor` (device fp32 [R,V]) and
+ *   allocates the device arrays below with N = 3 (Ls + 79 Ld + E) slots; icon_smplx_heads_prepare checks the host
+ *   tables (every face id in [0,F), every vertex id of a used face in [0,V), chain and source in [0,J), target in
+ *   [0,R), sources and targets each distinct), fills Ls, Ld, E, nchain, chain and writes the arrays.  It copies to
+ *   the device and synchronises `stream` (a one-time fill, not a per-call cost). */
+#define ICON_HEADS_LUT_ROWS 79
+#define ICON_HEADS_MAX_CHAIN 8
+typedef struct {
+    int V, J, R;
+    int Ls, Ld, E, nchain;
+    int chain[ICON_HEADS_MAX_CHAIN];
+    const float *regressor;  /* [R,V] */
+    int *vid;                /* [N]   corner vertex ids: static [Ls,3], then the table [79,Ld,3], then extra [E,3] */
+    float *bc;               /* [N]   their barycentric weights, same layout */
+    int *joint_reg;          /* [J]   the regressor row written over joint j, or -1 */
+    int *reg_joint;          /* [R]   the joint regressor row r is written over, or -1 */
+    int *inc_off;            /* [V+1] per vertex, its range of `inc` */
+    int *inc;                /* [N]   the slots that read each vertex, in (entry, table row, corner) order */
+} icon_smplx_heads;
+int icon_smplx_heads_prepare(icon_smplx_heads *h, const int64_t *h_faces, int F, const int64_t *h_lmk_faces_idx,
+                             const float *h_lmk_bary, int Ls, const int64_t *h_dyn_faces_idx, const float *h_dyn_bary,
+                             int Ld, const int64_t *h_face_ids, const float *h_bcs, int E, const int64_t *h_source,
+                             const int64_t *h_target, int S, const int64_t *h_chain, int nchain,
+                             icon_stream_t stream);
+/* Forward: verts [B,V,3] and joints_lbs [B,J,3] (icon_lbs_forward's outputs), pose [B,J,3,3] -> landmarks
+ * [B,Ls+Ld,3], joints [B,J+Ls+Ld+E,3] and rows [B] (int32 lookup-table rows); `state` (icon_smplx_heads_state_bytes)
+ * is scratch for the regressor's partial sums.  Two launches.  Backward: grad_landmarks and / or grad_joints
+ * (NULL = zero) -> grad_verts [B,V,3] (overwritten) and, when grad_joints is given, grad_joints_lbs [B,J,3] (zero
+ * at the regressed joints).  One launch. */
+size_t icon_smplx_heads_state_bytes(int B, int V, int R);
+int icon_smplx_heads_forward(const icon_smplx_heads *h, int B, const float *verts, const float *joints_lbs,
+                             const float *pose, float *landmarks, float *joints, int *rows, void *state,
+                             size_t state_bytes, icon_stream_t stream);
+int icon_smplx_heads_backward(const icon_smplx_heads *h, int B, const int *rows, const float *grad_landmarks,
+                              const float *grad_joints, float *grad_verts, float *grad_joints_lbs,
+                              icon_stream_t stream);
+
 /* ------------------------------------------------------------------ encoder operators
  * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
  * two take NCHW fp32 tensors; every 2-D convolution and normalisation runs on the NHWC path after them. */
