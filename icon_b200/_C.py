@@ -109,6 +109,15 @@ _SIGS = {
     "icon_smplx_heads_state_bytes": (_sz, [_i, _i, _i]),
     "icon_smplx_heads_forward": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "icon_smplx_heads_backward": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "icon_remesh_workspace_bytes": (_sz, [_i, _i, _i]),
+    "icon_remesh_compact": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_remesh_classify": (_i, [_vp, _vp, _vp, _sz, _vp]),
+    "icon_remesh_smooth_step": (_i, [_vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_remesh_midpoints": (_i, [_vp, _vp, _vp, _vp]),
+    "icon_remesh_select": (_i, [_i, _vp, _vp, ctypes.c_double, _i, _vp, ctypes.c_double, _vp, _vp, _sz, _vp]),
+    "icon_remesh_apply": (_i, [_i, _vp, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "icon_remesh_relax": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_remesh_reproject": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "icon_mc_workspace_bytes": (_sz, [_i, _i]),
     "icon_mc_count": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _sz, _vp, _vp]),
     "icon_mc_emit": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _vp, _vp, _i64, _i64, _vp]),

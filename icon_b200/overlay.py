@@ -16,7 +16,7 @@ accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.
               (`lib/net/HGPIFuNet.py` -> kaolin / pytorch3d / voxelize_cuda, `lib/net/voxelize.py` -> voxelize_cuda,
               `lib/common/seg3d_lossless.py` -> kaolin marching cubes / PyMCubes).
 * PATCH    -- the reference module is executed normally, then the accelerated names are rebound in its namespace
-              (`query_func` in `lib/common/train_util.py`, `get_visibility` in `lib/dataset/mesh_util.py`, the
+              (`query_func` in `lib/common/train_util.py`, `get_visibility` and `remesh` in `lib/dataset/mesh_util.py`, the
               encoder classes in `lib/net/{NormalNet,MLP,HGFilters,VE}.py`, `define_G` in `lib/net/FBNet.py`,
               `Evaluator.calculate_chamfer_p2s`, `Evaluator.init_gl` and `Evaluator._render_normal` in
               `lib/dataset/Evaluator.py`, `Render.get_rendered_video` in `lib/common/render.py`, and in
@@ -33,6 +33,8 @@ TestDataset.render_normal and render.get_silhouette_image),
 apps/infer.py:175-180 (the body-fit loop's `dataset.smpl_model(...)`: SMPL / SMPLH / SMPLX.forward call `lbs`
 through lib/smplx/body_models.py's namespace; fp32 CUDA calls run the fused skinning kernels, forward and backward;
 with `-hps_type pixie` it is PIXIE's SMPLX.forward, whose skinning and landmark / joint heads run on the kernels),
+apps/infer.py:402 (`remesh` of the reconstruction: smoothing and isotropic remeshing on the kernels, the same
+`_remesh.obj` written),
 apps/infer.py:405-476 and apps/ICON.py:483 (the cloth loop's LocalAffine and shape priors; VF2Mesh's differentiable
 vertex colours),
 apps/infer.py:548-562 (`-export_video`: get_rendered_video's 360 views per mesh, a chunk of views per kernel call),
@@ -63,7 +65,7 @@ def _replacements():
 
 
 def _patches():
-    from . import body_model, encoders, mesh, mesh_priors, mesh_views, metrics, net, visibility, voxelize
+    from . import body_model, encoders, mesh, mesh_priors, mesh_views, metrics, net, remesh, visibility, voxelize
 
     def make_define_G(reference_define_G):
         import torch.nn as nn
@@ -84,7 +86,8 @@ def _patches():
                                   "get_visibility": visibility.get_visibility},      # duplicate at train_util.py:361
         "lib.dataset.mesh_util": {"get_visibility": visibility.get_visibility, "clean_mesh": mesh.clean_mesh,
                                   "read_smpl_constants": voxelize.read_smpl_constants,
-                                  "update_mesh_shape_prior_losses": mesh_priors.update_mesh_shape_prior_losses},
+                                  "update_mesh_shape_prior_losses": mesh_priors.update_mesh_shape_prior_losses,
+                                  "remesh": remesh.remesh},
         "lib.net.local_affine": {"LocalAffine": mesh_priors.LocalAffine},
         "lib.net.NormalNet": {"NormalNet": encoders.NormalNet},
         "lib.net.MLP": {"MLP": net.MLP},

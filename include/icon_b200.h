@@ -355,6 +355,35 @@ int icon_mesh_priors_forward(const icon_mesh_topology *t, const float *verts, fl
                              float *out_lap, void *ws, size_t ws_bytes, icon_stream_t stream);
 int icon_mesh_priors_backward(const icon_mesh_topology *t, const float *verts, const float *g_edge, const float *g_nc,
                               const float *g_lap, float *grad_verts, void *ws, size_t ws_bytes, icon_stream_t stream);
+/* ------------------------------------------------------------------ remeshing of the reconstruction
+ * lib/dataset/mesh_util.py:109-121 (remesh: pymeshlab laplacian_smooth + isotropic explicit remeshing); rules
+ * (parity unpinned) in the csrc/remesh.cu header; the host loop is icon_b200/remesh.py.  Vertices are f64 [V,3].
+ * ws: icon_remesh_workspace_bytes(V, F, E) bytes for the topology t the call is given; classify fills it and the
+ * other calls of the same round read it.
+ * compact: drop unreferenced vertices (out_verts [V,3], out_faces [F,3], *d_count (device i64) = vertices kept;
+ *   ws sized for (V, F, 1)).  smooth_step: one Jacobi step (after classify).  midpoints: fp32 edge midpoints [E,3].
+ * select: op 0 split, 1 collapse (sqdist [E] f32: squared distance of each midpoint to the reference surface), 2
+ *   flip; marks the round's winners, *d_count (device i64) = their number W.  apply: split -> out_verts [V+W,3],
+ *   out_faces [F+2W,3]; collapse -> [V-W,3], [F-2W,3]; flip -> out_faces [F,3] (out_verts unused).
+ * relax: normals [V,3] f32 (icon_area_vertex_normals) -> out [V,3] f64, out32 [V,3] f32, moved [V] i32.
+ * reproject: each moved vertex onto its nearest reference face face[v] (icon_mesh_distance of out32). */
+size_t icon_remesh_workspace_bytes(int V, int F, int E);
+int icon_remesh_compact(const double *verts, int V, const int64_t *faces, int F, double *out_verts,
+                        int64_t *out_faces, int64_t *d_count, void *ws, size_t ws_bytes, icon_stream_t stream);
+int icon_remesh_classify(const icon_mesh_topology *t, const double *verts, void *ws, size_t ws_bytes,
+                         icon_stream_t stream);
+int icon_remesh_smooth_step(const icon_mesh_topology *t, const double *verts, double *out, void *ws,
+                            size_t ws_bytes, icon_stream_t stream);
+int icon_remesh_midpoints(const icon_mesh_topology *t, const double *verts, float *out, icon_stream_t stream);
+int icon_remesh_select(int op, const icon_mesh_topology *t, const double *verts, double L, int adaptive,
+                       const float *sqdist, double dlim2, int64_t *d_count, void *ws, size_t ws_bytes,
+                       icon_stream_t stream);
+int icon_remesh_apply(int op, const icon_mesh_topology *t, const double *verts, int W, double *out_verts,
+                      int64_t *out_faces, void *ws, size_t ws_bytes, icon_stream_t stream);
+int icon_remesh_relax(const icon_mesh_topology *t, const double *verts, const float *normals, double *out,
+                      float *out32, int32_t *moved, void *ws, size_t ws_bytes, icon_stream_t stream);
+int icon_remesh_reproject(const double *verts, int V, const int32_t *moved, const int32_t *face,
+                          const double *ref_verts, const int64_t *ref_faces, double *out, icon_stream_t stream);
 /* LocalAffine, B = 1: A [N,3,3], b [N,3], x [N,3], edges [E,2] i64 -> out [N,3], w_diff [E,3,4], w_rigid [N] (all
  * f32).  Backward: g_out / g_diff / g_rigid shaped as those (NULL = absent), vert_off / vert_edges from
  * icon_vertex_edges of the same edges -> grad_A, grad_b and (when not NULL) grad_x, overwritten. */
