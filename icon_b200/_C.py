@@ -109,6 +109,9 @@ _SIGS = {
     "icon_smplx_heads_state_bytes": (_sz, [_i, _i, _i]),
     "icon_smplx_heads_forward": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "icon_smplx_heads_backward": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "icon_tetra_prepare": (_i, [_vp, _vp, _i, _i, _i]),
+    "icon_tetra_state_bytes": (_sz, []),
+    "icon_tetra_forward": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "icon_remesh_workspace_bytes": (_sz, [_i, _i, _i]),
     "icon_remesh_compact": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     "icon_remesh_classify": (_i, [_vp, _vp, _vp, _sz, _vp]),
@@ -149,6 +152,13 @@ class SmplxHeads(ctypes.Structure):
     _fields_ = [("V", _i), ("J", _i), ("R", _i), ("Ls", _i), ("Ld", _i), ("E", _i), ("nchain", _i),
                 ("chain", _i * 8), ("regressor", _vp), ("vid", _vp), ("bc", _vp), ("joint_reg", _vp),
                 ("reg_joint", _vp), ("inc_off", _vp), ("inc", _vp)]
+
+
+class TetraModel(ctypes.Structure):
+    """icon_tetra_model (include/icon_b200.h): PaMIR's tetrahedral SMPL, both vertex sets, on the device."""
+    _fields_ = [("V", _i), ("N", _i), ("T", _i), ("nnz", _i), ("parents", _i * 24), ("v_template", _vp),
+                ("shapedirs", _vp), ("posedirs", _vp), ("weights", _vp), ("jr_off", _vp), ("jr_col", _vp),
+                ("jr_val", _vp)]
 
 
 class IconError(RuntimeError):

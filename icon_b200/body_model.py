@@ -12,6 +12,10 @@
                   the overlay's patch of lib.pixielib.models.SMPLX.SMPLX: the same class, whose forward runs PIXIE's
                   skinning on the same kernels and its landmark / joint heads on the heads kernels (_Heads, composed
                   after _Lbs); calls that are not fp32 CUDA on one device go to the reference's forward.
+  tetra_voxel_verts(model, body_pose, global_orient, betas, trans, scale)
+                  PaMIR's TestDataset.compute_voxel_verts on the tetra kernels (two launches, no host sync), for a
+                  PreparedTetra (prepared_tetra, or tetra_from_files: cached on the three files' paths, sizes and
+                  mtimes); make_compute_voxel_verts is the overlay's binding of the method.
 
 A model's prepared constants (J_template = J_regressor v_template, J_dirs = J_regressor shapedirs, the parents) are
 cached on the buffer tensors' identity and version, for several models at once: PyMAF's SMPL and the dataset's SMPL
@@ -454,3 +458,189 @@ def make_pixie_SMPLX(reference_SMPLX):
     reference_SMPLX.forward = forward
     reference_SMPLX._icon_b200_reference_forward = reference_forward
     return reference_SMPLX
+
+
+# ---------------------------------------------------------------- PaMIR's tetrahedral body (compute_voxel_verts)
+
+TETRA_JOINTS, TETRA_BETAS, TETRA_POSE = 24, 10, 207
+PAD_V, PAD_F = 8000, 25100
+TETRA_FILES = ("smpl/SMPL_NEUTRAL.pkl", "tetra_neutral_adult_smpl.npz", "tetrahedrons_neutral_adult.txt")
+CACHED_TETRA = 2
+
+
+def check_tetra(model, tetrahedrons):
+    """The host-side checks of a TetraSMPLModel's arrays and the tetrahedra [T,4] (0-based) compute_voxel_verts pads;
+    returns (V, V_added, T, parents as a list of ints).  Messages name the reference's arrays."""
+    import numpy as np
+    pre = "tetra body:"
+    kin = np.asarray(model.kintree_table)
+    if kin.ndim != 2 or kin.shape[0] != 2 or kin.shape[1] != TETRA_JOINTS:
+        raise ValueError(f"{pre} kintree_table {kin.shape} must be [2,{TETRA_JOINTS}] (SMPL's 24 joints)")
+    par = [-1] + [int(model.parent[i]) for i in range(1, TETRA_JOINTS)]
+    for i in range(1, TETRA_JOINTS):
+        if not 0 <= par[i] < i:
+            raise ValueError(f"{pre} kintree_table gives joint {i} the parent {par[i]}, a joint's parent must come "
+                             "before it")
+    V, Va = np.shape(model.v_template)[0], np.shape(model.v_template_added)[0]
+    for suffix, n in (("", V), ("_added", Va)):
+        for name, want in (("v_template", (n, 3)), ("shapedirs", (n, 3, TETRA_BETAS)),
+                           ("posedirs", (n, 3, TETRA_POSE)), ("weights", (n, TETRA_JOINTS))):
+            shape = tuple(np.shape(getattr(model, name + suffix)))
+            if shape != want:
+                if name == "posedirs" and shape[:2] == want[:2]:
+                    raise ValueError(f"{pre} posedirs{suffix} has {shape[2]} columns, 9 (J - 1) = {TETRA_POSE}")
+                raise ValueError(f"{pre} {name}{suffix} {shape} must be [{','.join(map(str, want))}]")
+    if tuple(np.shape(model.J_regressor)) != (TETRA_JOINTS, V):
+        raise ValueError(f"{pre} J_regressor {tuple(np.shape(model.J_regressor))} must be [{TETRA_JOINTS},{V}]")
+    if V + Va > PAD_V:
+        raise ValueError(f"{pre} v_template ({V}) + v_template_added ({Va}) = {V + Va} vertices, the padded "
+                         f"voxel_verts hold {PAD_V}")
+    tets = np.asarray(tetrahedrons)
+    if tets.ndim != 2 or tets.shape[1] != 4:
+        raise ValueError(f"{pre} tetrahedrons {tets.shape} must be [T,4]")
+    if tets.shape[0] > PAD_F:
+        raise ValueError(f"{pre} {tets.shape[0]} tetrahedrons, the padded voxel_faces hold {PAD_F}")
+    return V, Va, tets.shape[0], par
+
+
+class PreparedTetra:
+    """One tetrahedral SMPL on the device (icon_tetra_model): both vertex sets stacked in fp64, the blend shapes
+    transposed to [k, 3N], J_regressor's nonzeros per joint (ascending columns: the order scipy's sparse product
+    sums in), and the padded tetrahedra [25100,4] int64."""
+
+    def __init__(self, model, tetrahedrons, device):
+        import numpy as np
+        V, Va, T, par = check_tetra(model, tetrahedrons)
+        N = V + Va
+        dev = torch.device(device)
+        f64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float64)).to(dev)  # noqa: E731
+        cat = lambda k: np.concatenate([np.asarray(getattr(model, k), np.float64),  # noqa: E731
+                                        np.asarray(getattr(model, k + "_added"), np.float64)], 0)
+        jr = model.J_regressor
+        if hasattr(jr, "tocsr"):
+            jr = jr.tocsr()
+            jr.sort_indices()
+            rows = [(jr.indices[jr.indptr[j]:jr.indptr[j + 1]], jr.data[jr.indptr[j]:jr.indptr[j + 1]])
+                    for j in range(TETRA_JOINTS)]
+        else:
+            jr = np.asarray(jr)
+            rows = [(np.flatnonzero(jr[j]), jr[j][np.flatnonzero(jr[j])]) for j in range(TETRA_JOINTS)]
+        keep = [(c[v != 0], v[v != 0]) for c, v in rows]
+        off = np.concatenate([[0], np.cumsum([len(c) for c, _ in keep])]).astype(np.int32)
+        self.V, self.N, self.T, self.parents = V, N, T, par
+        self.arrays = dict(v_template=f64(cat("v_template")),
+                           shapedirs=f64(cat("shapedirs").reshape(3 * N, TETRA_BETAS).T),
+                           posedirs=f64(cat("posedirs").reshape(3 * N, TETRA_POSE).T),
+                           weights=f64(cat("weights")),
+                           jr_off=torch.from_numpy(off).to(dev),
+                           jr_col=torch.from_numpy(np.concatenate([c for c, _ in keep] + [[0]]).astype(np.int32)).to(dev),
+                           jr_val=f64(np.concatenate([v for _, v in keep] + [[0.0]])))
+        faces = np.zeros((PAD_F, 4), np.int64)
+        faces[:T] = np.asarray(tetrahedrons, np.int64)
+        self.faces = torch.from_numpy(faces).to(dev)
+        self.c = _C.TetraModel(V, N, T, int(off[-1]), (ctypes.c_int * TETRA_JOINTS)(),
+                               *(_p(self.arrays[k]) for k in ("v_template", "shapedirs", "posedirs", "weights",
+                                                              "jr_off", "jr_col", "jr_val")))
+        with torch.cuda.device(dev):
+            check(lib.icon_tetra_prepare(ctypes.byref(self.c), (ctypes.c_int64 * TETRA_JOINTS)(*par), TETRA_JOINTS,
+                                         TETRA_POSE, TETRA_BETAS), "icon_tetra_prepare")
+        self.device = dev
+
+
+def prepared_tetra(model, tetrahedrons, device="cuda"):
+    """A PreparedTetra from an instance of the reference's own TetraSMPLModel (its loading, pickle encoding and
+    J_regressor, scipy sparse or dense, stay the reference's) and the 0-based tetrahedra [T,4]."""
+    return PreparedTetra(model, tetrahedrons, device)
+
+
+_TETRA = []            # [(key, PreparedTetra)], the CACHED_TETRA most recently used
+
+
+def _file_key(paths, device):
+    import os
+    return tuple((os.path.abspath(p), os.stat(p).st_size, os.stat(p).st_mtime_ns) for p in paths) + (str(device),)
+
+
+def tetra_from_files(smpl_path, tetra_path, tets_path, device, model_cls):
+    """The PreparedTetra of the three files compute_voxel_verts reads (model_cls(smpl_path, tetra_path, 'adult') and
+    np.loadtxt(tets_path) - 1), cached on the paths plus each file's size and mtime: a changed file re-prepares."""
+    import numpy as np
+    key = _file_key((smpl_path, tetra_path, tets_path), torch.device(device))
+    for k, (kk, hit) in enumerate(_TETRA):
+        if kk == key:
+            _TETRA.append(_TETRA.pop(k))
+            return hit
+    tets = np.loadtxt(tets_path, dtype=np.int32) - 1
+    hit = prepared_tetra(model_cls(smpl_path, tetra_path, "adult"), tets.reshape(-1, 4), device)
+    _TETRA.append((key, hit))
+    del _TETRA[:-CACHED_TETRA]
+    return hit
+
+
+def tetra_forward(model, rotmats=None, aa=None, betas=None, trans=None, scale=None):
+    """(voxel_verts [1,8000,3] f32, aa [24,3] f32) from rotation matrices [24,3,3] (aa is then their pymaf
+    axis-angle, computed on the device) or, with rotmats None, from the fp32 axis-angle aa [24,3] as given.  betas [10],
+    trans [3] and scale [1] fp32 on the model's device; two launches, no host sync."""
+    dev = model.device
+    src = rotmats if rotmats is not None else aa
+    if src.shape[-2:] != ((3, 3) if rotmats is not None else (TETRA_JOINTS, 3)) or src.numel() != TETRA_JOINTS * (
+            9 if rotmats is not None else 3):
+        raise ValueError(f"tetra body: pose {tuple(src.shape)} must be [24,3,3] rotation matrices or [24,3] axis-angle")
+    for name, t, n in (("betas[0]", betas, TETRA_BETAS), ("trans", trans, 3), ("scale", scale, 1)):
+        if t.numel() != n:
+            raise ValueError(f"tetra body: {name} {tuple(t.shape)} must hold {n} values")
+    f32 = lambda t: t.detach().to(dev, torch.float32).contiguous()  # noqa: E731
+    rm = f32(rotmats) if rotmats is not None else None
+    aa_out = torch.empty(TETRA_JOINTS, 3, dtype=torch.float32, device=dev) if rotmats is not None else f32(aa)
+    b, tr, sc = f32(betas), f32(trans), f32(scale)
+    out = torch.empty(1, PAD_V, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        sbytes = lib.icon_tetra_state_bytes()
+        state = torch.empty(sbytes, dtype=torch.uint8, device=dev)
+        check(lib.icon_tetra_forward(ctypes.byref(model.c), _p(rm) if rm is not None else None, _p(aa_out), _p(b),
+                                     _p(tr), _p(sc), _p(out), _p(state), sbytes, _stream()), "icon_tetra_forward")
+    return out, aa_out
+
+
+def tetra_voxel_verts(model, body_pose, global_orient, betas, trans, scale):
+    """TestDataset.compute_voxel_verts on the kernels: {voxel_verts [1,8000,3] f32, voxel_faces [1,25100,4] i64 (a
+    fresh tensor), pad_v_num [1] i64, pad_f_num [1] i64}, on the inputs' device.  body_pose [B,23,3,3] and
+    global_orient [B,1,3,3] rotation matrices, betas [B,10] (row 0 is used, as the reference does), trans [3],
+    scale (one value)."""
+    pose = torch.cat([global_orient[0], body_pose[0]], dim=0)
+    verts, _ = tetra_forward(model, rotmats=pose, betas=betas[0], trans=trans, scale=scale)
+    dev = model.device
+    return {"voxel_verts": verts, "voxel_faces": model.faces.clone().unsqueeze(0),
+            "pad_v_num": torch.full((1,), PAD_V - model.N, dtype=torch.long, device=dev),
+            "pad_f_num": torch.full((1,), PAD_F - model.T, dtype=torch.long, device=dev)}
+
+
+def tetra_on_kernels(body_pose, global_orient, betas, trans, scale):
+    """Whether the overlay's compute_voxel_verts sends a call to the kernels: every argument an fp32 CUDA tensor on
+    one device."""
+    ts = (body_pose, global_orient, betas, trans, scale)
+    if not all(torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 for t in ts):
+        return False
+    return all(t.device == body_pose.device for t in ts)
+
+
+def make_compute_voxel_verts(reference):
+    """TestDataset.compute_voxel_verts: the reference's file paths (under self.smpl_data), the cached PreparedTetra
+    and tetra_voxel_verts where tetra_on_kernels holds; the reference's own method, unchanged, for every other
+    call.  The TetraSMPLModel class is the one the reference's module imported."""
+    import os.path as osp
+    import sys
+
+    def compute_voxel_verts(self, body_pose, global_orient, betas, trans, scale):
+        if not tetra_on_kernels(body_pose, global_orient, betas, trans, scale):
+            return reference(self, body_pose, global_orient, betas, trans, scale)
+        paths = (osp.join(self.smpl_data.model_dir, TETRA_FILES[0]), osp.join(self.smpl_data.tedra_dir, TETRA_FILES[1]),
+                 osp.join(self.smpl_data.tedra_dir, TETRA_FILES[2]))
+        model_cls = sys.modules[reference.__module__].TetraSMPLModel
+        model = tetra_from_files(*paths, body_pose.device, model_cls)
+        return tetra_voxel_verts(model, body_pose, global_orient, betas, trans, scale)
+
+    compute_voxel_verts.reference = reference
+    compute_voxel_verts.__doc__ = reference.__doc__
+    compute_voxel_verts.__qualname__ = reference.__qualname__
+    return compute_voxel_verts

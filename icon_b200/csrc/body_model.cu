@@ -58,6 +58,41 @@
 //     dynamic slots of other table rows skipped), then + sum over r ascending of R[r,v] g_joints[source of r].
 //     g_J_transformed = g_joints[:, :J] with zeros at the sources (the `detach() * 0`).  No float atomics.
 //   Launches: two forward (k_heads_reg_partial, k_heads_finish), one backward (k_heads_backward).
+//
+// Tetra body: PaMIR's TestDataset.compute_voxel_verts (lib/dataset/TestDataset.py:150-192) with TetraSMPLModel.update
+// (lib/dataset/body_model.py:344-427) and pymaf's rotation_matrix_to_angle_axis (lib/pymaf/utils/geometry.py).
+// Restated by oracle/tetra_body.py; pinned against the reference's own class and conversion, run live, by
+// tests/golden/tetra_body.npz.
+//   Model (icon_tetra_model, fp64 device buffers, the SMPL vertices then the added ones, N = V + V_added <= 8000):
+//   v_template [N,3], shapedirs [10,3N], posedirs [207,3N] (transposed from the files' [N,3,k]), weights [N,24],
+//   J_regressor's nonzeros per joint in ascending column order (the order scipy's sparse product sums in; a dense
+//   file's zero entries add nothing), parents from kintree_table (checked at prepare: 24 joints, parents[i] < i).
+//   T <= 25100 tetrahedra are padded by the host; the kernels never read them.
+//   Promotion chain (NumPy >= 2, confirmed on the golden's live run): the pose and betas arrive as fp32 arrays;
+//   np.linalg.norm of the fp32 pose stays fp32, np.maximum with np.finfo(np.float64).tiny widens theta, and every
+//   later value is fp64 (the fp64 model arrays dotted with the widened betas; r / theta widens r).  NumPy 1.x would
+//   keep theta in fp32: this restates NumPy 2.
+//   Forward (k_tetra_chain, one CTA):
+//     aa_j (fp32): t = R_j^T; d2 = t22 < 1e-6f, d0d1 = t00 > t11, d0nd1 = t00 < -t11; t0 = ((1 + t00) - t11) - t22,
+//       t1 = ((1 - t00) + t11) - t22, t2 = ((1 - t00) - t11) + t22, t3 = ((1 + t00) + t11) + t22 and the four
+//       candidates q0..q3; with 0/1 masks m0..m3 (d2 d0d1, d2 !d0d1, !d2 d0nd1, !d2 !d0nd1):
+//       q = ((((q0 m0 + q1 m1) + q2 m2) + q3 m3) / sqrt(((t0 m0 + t1 m1) + t2 m2) + t3 m3)) 0.5;
+//       s2 = (q1^2 + q2^2) + q3^2, two = 2 (q0 < 0 ? atan2(-sqrt s2, -q0) : atan2(sqrt s2, q0)),
+//       k = s2 > 0 ? two / sqrt s2 : 2, aa = 0 + q_{1..3} k, NaN -> 0.  Each step one fp32 rounding, as each torch
+//       op is; atan2f differs from torch's CPU atan2 by a few ulps.  With rotmats = NULL, aa is read as given.
+//     R_j (fp64): theta = max((double)sqrtf((x^2 + y^2) + z^2), DBL_MIN), rh = r / theta,
+//       R = (cos I + (1 - cos) rh rh^T) + sin [rh]x (no 1e-8 shift: the model's own rodrigues, not batch_rodrigues).
+//     J_j = sum over J_regressor's nonzeros v (ascending) of w v_shaped[v], v_shaped = shapedirs . beta (k
+//       ascending) + v_template.  G_0 = [R_0 | J_0], G_j = G_parent [R_j | J_j - J_parent], level by level;
+//       A_j = [G_j.R | G_j.t - G_j.R J_j] (the rest-pose removal); lrotmin_p = R_{1 + p/9}[p%9] - I[p%9].
+//   Forward (k_tetra_skin, 64 output rows per CTA, one thread per (row, component) of the 8000 x 3 output):
+//     v_posed = v_shaped + sum_p lrotmin_p posedirs[p] (p ascending); T = sum_j weights[v,j] A_j (j ascending);
+//     v = (((T0 x + T1 y) + T2 z) + T3) + 0 (the model's zero trans); out = fp32(v (double)scale + (double)trans)
+//     (the reference's scale.item() and the fp32 trans widened), rows >= N are 0; then x 0.5f, and z x -1.0f (the
+//     padding's z is -0.0f, as the reference's array holds).
+//   No float atomics, no host sync: scale and trans are read on the device.  Launches: two (k_tetra_chain,
+//   k_tetra_skin).
+#include <float.h>
 #include <math.h>
 
 #include <vector>
@@ -646,6 +681,184 @@ static bool heads_ok(const icon_smplx_heads *h) {
            h->inc_off && h->inc;
 }
 
+// ---------------------------------------------------------------- tetra body (PaMIR's TetraSMPLModel)
+
+constexpr int TETRA_J = ICON_TETRA_JOINTS;
+constexpr int TETRA_P = 9 * (TETRA_J - 1);
+constexpr int TETRA_NB = ICON_TETRA_BETAS;
+constexpr int TETRA_CT = 128;           // chain threads (>= 3 TETRA_J)
+constexpr int TETRA_ST = 192;           // skin threads: 64 output rows x 3 components
+constexpr int TETRA_STATE = 12 * TETRA_J + TETRA_P;    // A [24,12], then lrotmin [207]
+
+// pymaf's rotation_matrix_to_angle_axis for one [3,3] matrix, op by op in fp32 (every torch op one rounding)
+__device__ __forceinline__ void tetra_rotmat_to_aa(const float *__restrict__ R, float aa[3]) {
+    float t[3][3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int b = 0; b < 3; ++b) t[a][b] = R[3 * b + a];          // rmat_t = R^T
+    const bool d2 = t[2][2] < 1e-6f, d0d1 = t[0][0] > t[1][1], d0nd1 = t[0][0] < -t[1][1];
+    const float t0 = ((1.0f + t[0][0]) - t[1][1]) - t[2][2];
+    const float t1 = ((1.0f - t[0][0]) + t[1][1]) - t[2][2];
+    const float t2 = ((1.0f - t[0][0]) - t[1][1]) + t[2][2];
+    const float t3 = ((1.0f + t[0][0]) + t[1][1]) + t[2][2];
+    const float q0[4] = {t[1][2] - t[2][1], t0, t[0][1] + t[1][0], t[2][0] + t[0][2]};
+    const float q1[4] = {t[2][0] - t[0][2], t[0][1] + t[1][0], t1, t[1][2] + t[2][1]};
+    const float q2[4] = {t[0][1] - t[1][0], t[2][0] + t[0][2], t[1][2] + t[2][1], t2};
+    const float q3[4] = {t3, t[1][2] - t[2][1], t[2][0] - t[0][2], t[0][1] - t[1][0]};
+    const float m0 = (d2 && d0d1) ? 1.0f : 0.0f, m1 = (d2 && !d0d1) ? 1.0f : 0.0f;
+    const float m2 = (!d2 && d0nd1) ? 1.0f : 0.0f, m3 = (!d2 && !d0nd1) ? 1.0f : 0.0f;
+    const float den = sqrtf(((t0 * m0 + t1 * m1) + t2 * m2) + t3 * m3);
+    float q[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) q[i] = ((((q0[i] * m0 + q1[i] * m1) + q2[i] * m2) + q3[i] * m3) / den) * 0.5f;
+    const float s2 = (q[1] * q[1] + q[2] * q[2]) + q[3] * q[3];
+    const float st = sqrtf(s2), ct = q[0];
+    const float two = 2.0f * (ct < 0.0f ? atan2f(-st, -ct) : atan2f(st, ct));
+    const float k = s2 > 0.0f ? two / st : 2.0f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float v = 0.0f + q[1 + c] * k;
+        aa[c] = isnan(v) ? 0.0f : v;
+    }
+}
+
+// TetraSMPLModel.rodrigues: theta = max(fp32 |r|, DBL_MIN) widened, R = (cos I + (1 - cos) rh rh^T) + sin [rh]x
+__device__ __forceinline__ void tetra_rodrigues(const float r[3], double R[9]) {
+    const float th32 = sqrtf((r[0] * r[0] + r[1] * r[1]) + r[2] * r[2]);
+    const double th = fmax((double)th32, DBL_MIN);
+    const double rh[3] = {(double)r[0] / th, (double)r[1] / th, (double)r[2] / th};
+    const double cs = cos(th), sn = sin(th), c1 = 1.0 - cs;
+    const double K[9] = {0.0, -rh[2], rh[1], rh[2], 0.0, -rh[0], -rh[1], rh[0], 0.0};
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) R[3 * i + j] = (cs * (i == j ? 1.0 : 0.0) + c1 * (rh[i] * rh[j])) + sn * K[3 * i + j];
+}
+
+// v_shaped of column col = 3 v + c: shapedirs . beta (k ascending) + v_template
+__device__ __forceinline__ double tetra_vshaped(const icon_tetra_model &m, const double *beta, int col) {
+    const int N3 = 3 * m.N;
+    double acc = 0.0;
+#pragma unroll
+    for (int k = 0; k < TETRA_NB; ++k) acc = acc + m.shapedirs[(size_t)k * N3 + col] * beta[k];
+    return acc + m.v_template[col];
+}
+
+// one CTA: rotations (from matrices, or the axis-angle as given), rest joints, the chain, A and lrotmin
+__global__ void __launch_bounds__(TETRA_CT) k_tetra_chain(icon_tetra_model m, const float *__restrict__ rotmats,
+                                                          float *__restrict__ aa, const float *__restrict__ betas,
+                                                          double *__restrict__ st) {
+    __shared__ double sJ[TETRA_J][3], sR[TETRA_J][9], sG[TETRA_J][12], s_beta[TETRA_NB];
+    const int t = threadIdx.x;
+    if (t < TETRA_NB) s_beta[t] = (double)betas[t];
+    int depth = 0;
+    if (t < TETRA_J) {
+        float r[3];
+        if (rotmats) {
+            tetra_rotmat_to_aa(rotmats + 9 * t, r);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) aa[3 * t + c] = r[c];
+        } else {
+#pragma unroll
+            for (int c = 0; c < 3; ++c) r[c] = aa[3 * t + c];
+        }
+        tetra_rodrigues(r, sR[t]);
+        for (int i = m.parents[t]; i >= 0; i = m.parents[i]) ++depth;
+    }
+    __syncthreads();
+    if (t < 3 * TETRA_J) {
+        const int j = t / 3, c = t % 3;
+        double acc = 0.0;
+        for (int e = m.jr_off[j]; e < m.jr_off[j + 1]; ++e)
+            acc = acc + m.jr_val[e] * tetra_vshaped(m, s_beta, 3 * m.jr_col[e] + c);
+        sJ[j][c] = acc;
+    }
+    __syncthreads();
+    for (int d = 0; __syncthreads_or(t < TETRA_J && depth >= d); ++d) {
+        if (t < TETRA_J && depth == d) {
+            const int p = m.parents[t];
+            double G[12];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+                if (p < 0) {
+#pragma unroll
+                    for (int c = 0; c < 3; ++c) G[4 * r + c] = sR[t][3 * r + c];
+                    G[4 * r + 3] = sJ[t][r];
+                } else {
+                    const double rel[3] = {sJ[t][0] - sJ[p][0], sJ[t][1] - sJ[p][1], sJ[t][2] - sJ[p][2]};
+#pragma unroll
+                    for (int c = 0; c < 3; ++c)
+                        G[4 * r + c] = (sG[p][4 * r] * sR[t][c] + sG[p][4 * r + 1] * sR[t][3 + c]) +
+                                       sG[p][4 * r + 2] * sR[t][6 + c];
+                    G[4 * r + 3] = ((sG[p][4 * r] * rel[0] + sG[p][4 * r + 1] * rel[1]) + sG[p][4 * r + 2] * rel[2]) +
+                                   sG[p][4 * r + 3];
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < 12; ++e) sG[t][e] = G[e];
+#pragma unroll
+            for (int r = 0; r < 3; ++r) {
+                const double gj = (G[4 * r] * sJ[t][0] + G[4 * r + 1] * sJ[t][1]) + G[4 * r + 2] * sJ[t][2];
+#pragma unroll
+                for (int c = 0; c < 3; ++c) st[12 * t + 4 * r + c] = G[4 * r + c];
+                st[12 * t + 4 * r + 3] = G[4 * r + 3] - gj;
+            }
+        }
+    }
+    for (int p = t; p < TETRA_P; p += TETRA_CT) {
+        const int e = p % 9;
+        st[12 * TETRA_J + p] = sR[1 + p / 9][e] - ((e == 0 || e == 4 || e == 8) ? 1.0 : 0.0);
+    }
+}
+
+// 64 output rows per CTA, one thread per (row, component): v_posed, the skinning and the epilogue; rows >= N are the
+// padding (0 x 0.5, z negated: -0.0f, as the reference's float32 array holds)
+__global__ void __launch_bounds__(TETRA_ST) k_tetra_skin(icon_tetra_model m, const float *__restrict__ betas,
+                                                         const float *__restrict__ trans,
+                                                         const float *__restrict__ scale,
+                                                         const double *__restrict__ st, float *__restrict__ out) {
+    __shared__ double s_pf[TETRA_P], s_A[12 * TETRA_J], s_beta[TETRA_NB], s_vp[TETRA_ST];
+    const int t = threadIdx.x, col = blockIdx.x * TETRA_ST + t, row = col / 3, c = col % 3, N3 = 3 * m.N;
+    for (int p = t; p < TETRA_P; p += TETRA_ST) s_pf[p] = st[12 * TETRA_J + p];
+    for (int i = t; i < 12 * TETRA_J; i += TETRA_ST) s_A[i] = st[i];
+    if (t < TETRA_NB) s_beta[t] = (double)betas[t];
+    __syncthreads();
+    const bool live = col < N3;
+    double vp = 0.0;
+    if (live) {
+        double po = 0.0;
+        const double *pd = m.posedirs + col;
+#pragma unroll 9
+        for (int p = 0; p < TETRA_P; ++p) po = po + s_pf[p] * __ldg(pd + (size_t)p * N3);
+        vp = tetra_vshaped(m, s_beta, col) + po;
+    }
+    s_vp[t] = vp;
+    __syncthreads();
+    if (col >= 3 * ICON_TETRA_PAD_V) return;
+    float o = 0.0f;
+    if (live) {
+        double T[4] = {0.0, 0.0, 0.0, 0.0};
+        const double *w = m.weights + (size_t)row * TETRA_J;
+        for (int j = 0; j < TETRA_J; ++j) {
+            const double wj = w[j];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) T[q] = T[q] + wj * s_A[12 * j + 4 * c + q];
+        }
+        const int l = 3 * (t / 3);
+        const double v = (((T[0] * s_vp[l] + T[1] * s_vp[l + 1]) + T[2] * s_vp[l + 2]) + T[3]) + 0.0;
+        o = (float)(v * (double)scale[0] + (double)trans[c]);
+    }
+    o = o * 0.5f;
+    if (c == 2) o = o * -1.0f;
+    out[col] = o;
+}
+
+static bool tetra_model_ok(const icon_tetra_model *m) {
+    return m && m->V >= 1 && m->N >= m->V && m->N <= ICON_TETRA_PAD_V && m->T >= 0 && m->T <= ICON_TETRA_PAD_F &&
+           m->v_template && m->shapedirs && m->posedirs && m->weights && m->jr_off && m->jr_col && m->jr_val;
+}
+
 }  // namespace icon
 
 // ---------------------------------------------------------------- C ABI
@@ -868,6 +1081,51 @@ extern "C" int icon_smplx_heads_backward(const icon_smplx_heads *h, int B, const
     const int64_t cols = 3 * ((int64_t)h->V + h->J);
     k_heads_backward<<<dim3((unsigned)((cols + HEADS_T - 1) / HEADS_T), (unsigned)B), HEADS_T, 0, stream>>>(
         *h, rows, grad_landmarks, grad_joints, grad_verts, grad_joints ? grad_joints_lbs : nullptr);
+    ICON_LAUNCHED();
+    return ICON_OK;
+}
+
+// ---------------------------------------------------------------- C ABI: tetra body
+
+extern "C" int icon_tetra_prepare(icon_tetra_model *m, const int64_t *h_parents, int J, int posedirs_cols,
+                                  int nbetas) {
+    using namespace icon;
+    ICON_CHECK_ARG(m && h_parents, "icon_tetra_prepare: null pointer");
+    ICON_CHECK_ARG(J == TETRA_J, "icon_tetra_prepare: kintree_table has %d joints, the kernels take %d", J, TETRA_J);
+    ICON_CHECK_ARG(posedirs_cols == TETRA_P, "icon_tetra_prepare: posedirs has %d columns, 9 (J - 1) = %d",
+                   posedirs_cols, TETRA_P);
+    ICON_CHECK_ARG(nbetas == TETRA_NB, "icon_tetra_prepare: shapedirs has %d columns, the kernels take %d", nbetas,
+                   TETRA_NB);
+    ICON_CHECK_ARG(h_parents[0] == -1, "icon_tetra_prepare: parents[0] = %lld, the root's must be -1",
+                   (long long)h_parents[0]);
+    for (int i = 1; i < J; ++i)
+        ICON_CHECK_ARG(h_parents[i] >= 0 && h_parents[i] < i,
+                       "icon_tetra_prepare: parents[%d] = %lld, a joint's parent must come before it", i,
+                       (long long)h_parents[i]);
+    ICON_CHECK_ARG(m->N >= m->V && m->N <= ICON_TETRA_PAD_V,
+                   "icon_tetra_prepare: V + V_added = %d vertices, the padded voxel_verts hold %d", m->N,
+                   ICON_TETRA_PAD_V);
+    ICON_CHECK_ARG(m->T >= 0 && m->T <= ICON_TETRA_PAD_F,
+                   "icon_tetra_prepare: %d tetrahedra, the padded voxel_faces hold %d", m->T, ICON_TETRA_PAD_F);
+    ICON_CHECK_ARG(tetra_model_ok(m), "icon_tetra_prepare: null buffer or bad sizes V=%d N=%d", m->V, m->N);
+    for (int i = 0; i < J; ++i) m->parents[i] = (int)h_parents[i];
+    return ICON_OK;
+}
+
+extern "C" size_t icon_tetra_state_bytes(void) { return icon::align_up(icon::TETRA_STATE * sizeof(double), 256); }
+
+extern "C" int icon_tetra_forward(const icon_tetra_model *m, const float *rotmats, float *aa, const float *betas,
+                                  const float *trans, const float *scale, float *voxel_verts, void *state,
+                                  size_t state_bytes, icon_stream_t stream_) {
+    using namespace icon;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    ICON_CHECK_ARG(tetra_model_ok(m), "icon_tetra_forward: model not prepared");
+    ICON_CHECK_ARG(aa && betas && trans && scale && voxel_verts && state, "icon_tetra_forward: null pointer");
+    ICON_CHECK_ARG(state_bytes >= icon_tetra_state_bytes(), "icon_tetra_forward: state too small");
+    k_tetra_chain<<<1, TETRA_CT, 0, stream>>>(*m, rotmats, aa, betas, (double *)state);
+    ICON_LAUNCHED();
+    k_tetra_skin<<<(3 * ICON_TETRA_PAD_V + TETRA_ST - 1) / TETRA_ST, TETRA_ST, 0, stream>>>(
+        *m, betas, trans, scale, (const double *)state, voxel_verts);
     ICON_LAUNCHED();
     return ICON_OK;
 }

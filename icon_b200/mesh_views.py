@@ -380,9 +380,15 @@ def bind_fit_renders(render):
 def make_TestDataset(reference_cls):
     """Overlay patch of lib.dataset.TestDataset: after the reference __init__, the instance's `render` (the Render
     both fitting loops of apps/infer.py draw through, via render_normal and render.get_silhouette_image) gets the
-    device get_rgb_image / get_silhouette_image and the VF2Mesh whose colours VertexNormals differentiates."""
+    device get_rgb_image / get_silhouette_image and the VF2Mesh whose colours VertexNormals differentiates; and the
+    class's compute_voxel_verts (the pamir demo's tetrahedral body) runs on the tetra kernels for fp32 CUDA calls
+    (body_model.make_compute_voxel_verts).  Patching twice keeps the first original."""
     if reference_cls is None:
         return None
+    from .body_model import make_compute_voxel_verts
+    cvv = reference_cls.__dict__.get("compute_voxel_verts")
+    if cvv is not None:
+        reference_cls.compute_voxel_verts = make_compute_voxel_verts(getattr(cvv, "reference", cvv))
     reference_init = reference_cls.__init__
 
     @functools.wraps(reference_init)

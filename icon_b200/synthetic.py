@@ -401,3 +401,62 @@ def pixie_smplx_standin():
             return "reference"
 
     return SMPLX
+
+
+TETRA_SIZES = {"tiny": dict(rings=4, segs=6, V_added=7, T=60),
+               "smpl": dict(rings=82, segs=84, V_added=1110, T=25100)}
+TETRA_FILES = ("smpl/SMPL_NEUTRAL.pkl", "tetra_neutral_adult_smpl.npz", "tetrahedrons_neutral_adult.txt")
+
+
+def tetra_model(kind="tiny", seed=0, folder=None):
+    """Seeded arrays of PaMIR's tetrahedral SMPL (lib/dataset/body_model.py:234-306), float64 on a 2^-20 grid (so
+    they do not depend on the machine's libm): the SMPL pkl's v_template [V,3], f, J_regressor (scipy csc [24,V], 4
+    to 8 nearby vertices per joint, as SMPL's file stores it), weights [V,24], posedirs [V,3,207], shapedirs
+    [V,3,10], kintree_table [2,24] (SMPL's tree, root entry 4294967295); the tetra npz's v_template_added [Va,3],
+    weights_added, shapedirs_added, posedirs_added, tetrahedrons; and `tets` [T,4], the 1-based text file's rows.
+    Built on tet_body: "tiny" is tet_body(4, 6) (V 26) with 7 added vertices and 60 tetrahedra; "smpl" is
+    tet_body() (V 6890) with V + V_added = 8000 and T = 25100, the padded sizes TestDataset.compute_voxel_verts
+    allots, exactly.  The added vertices are the interior one at the origin and shrunken surface vertices; the extra
+    tetrahedra join surface faces to them.  With `folder`, writes the three files under TETRA_FILES' names and
+    returns their paths as well."""
+    import pickle
+
+    import scipy.sparse as sp
+    z = TETRA_SIZES[kind]
+    rng = np.random.RandomState(seed)
+    allv, V, tets, _ = tet_body(rings=z["rings"], segs=z["segs"], seed=seed)
+    surf = allv[:V].astype(np.float64)
+    Va, F = z["V_added"], len(tets)
+    shrink = 0.5 * surf[rng.choice(V, Va - 1, replace=False)]
+    va = np.concatenate([np.zeros((1, 3)), shrink], 0)
+    extra = tets[rng.choice(F, z["T"] - F, replace=F < z["T"] - F)].copy()
+    extra[:, 3] = V + 1 + rng.randint(0, Va - 1, len(extra))
+    tets = np.concatenate([tets, extra], 0).astype(np.int64)
+    q = lambda x: np.round(np.asarray(x, np.float64) * 2.0 ** 20) / 2.0 ** 20   # noqa: E731
+    both = np.concatenate([surf, va], 0)
+    m = model_arrays(both.astype(np.float32), SMPL_PARENTS, 10, rng)
+    jr = np.zeros((24, V))
+    for j in range(24):
+        near = np.argsort(((surf - surf[rng.randint(V)]) ** 2).sum(1), kind="stable")[:rng.randint(4, 9)]
+        w = rng.uniform(0.5, 1.5, len(near))
+        jr[j, near] = w / w.sum()
+    pd = m["posedirs"].T.reshape(V + Va, 3, 207)
+    kin = np.stack([np.asarray(SMPL_PARENTS, np.int64), np.arange(24, dtype=np.int64)])
+    kin[0, 0] = 4294967295
+    out = dict(v_template=q(surf), f=tets[:F, :3].copy(), J_regressor=sp.csc_matrix(q(jr)),
+               weights=q(m["lbs_weights"][:V]), posedirs=q(pd[:V]), shapedirs=q(m["shapedirs"][:V]),
+               kintree_table=kin, v_template_added=q(va), weights_added=q(m["lbs_weights"][V:]),
+               shapedirs_added=q(m["shapedirs"][V:]), posedirs_added=q(pd[V:]), tetrahedrons=tets,
+               tets=tets + 1)
+    if folder is None:
+        return out
+    import os
+    paths = tuple(os.path.join(folder, n) for n in TETRA_FILES)
+    os.makedirs(os.path.dirname(paths[0]), exist_ok=True)
+    with open(paths[0], "wb") as fh:
+        pickle.dump({k: out[k] for k in ("v_template", "f", "J_regressor", "weights", "posedirs", "shapedirs",
+                                         "kintree_table")}, fh, protocol=2)
+    np.savez(paths[1], **{k: out[k] for k in ("v_template_added", "weights_added", "shapedirs_added",
+                                              "posedirs_added", "tetrahedrons")})
+    np.savetxt(paths[2], out["tets"], fmt="%d")
+    return out, paths

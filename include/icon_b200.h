@@ -471,6 +471,39 @@ int icon_smplx_heads_backward(const icon_smplx_heads *h, int B, const int *rows,
                               const float *grad_joints, float *grad_verts, float *grad_joints_lbs,
                               icon_stream_t stream);
 
+/* ------------------------------------------------------------------ tetra body (PaMIR's TetraSMPLModel)
+ * TestDataset.compute_voxel_verts of the pamir demo: rotation matrices -> pymaf's axis-angle (fp32) ->
+ * TetraSMPLModel.update (fp64) of the SMPL vertices and the added interior vertices -> the padded, halved, z-flipped
+ * voxel_verts [8000,3].  Rules and promotion chain in the "tetra body" section of the csrc/body_model.cu header.
+ *
+ * icon_tetra_model: the caller fills V (SMPL vertices), N = V + V_added, T (tetrahedra), nnz and the device buffers
+ *   (fp64 / int32, contiguous; both vertex sets stacked, SMPL's first); icon_tetra_prepare checks J = 24,
+ *   posedirs_cols = 207, nbetas = 10, h_parents (host [24] i64: parents[0] = -1, parents[i] < i), N <= 8000 and
+ *   T <= 25100, and copies the parents into the struct.  It launches nothing. */
+#define ICON_TETRA_JOINTS 24
+#define ICON_TETRA_BETAS 10
+#define ICON_TETRA_PAD_V 8000
+#define ICON_TETRA_PAD_F 25100
+typedef struct {
+    int V, N, T, nnz;
+    int parents[ICON_TETRA_JOINTS];
+    const double *v_template;  /* [N,3] */
+    const double *shapedirs;   /* [10,3N]  column k of shapedirs / shapedirs_added */
+    const double *posedirs;    /* [207,3N] column p of posedirs / posedirs_added */
+    const double *weights;     /* [N,24] */
+    const int *jr_off;         /* [25]    per joint, its range of jr_col / jr_val */
+    const int *jr_col;         /* [nnz]   J_regressor's nonzero columns (SMPL vertex ids), ascending per joint */
+    const double *jr_val;      /* [nnz]   their values */
+} icon_tetra_model;
+int icon_tetra_prepare(icon_tetra_model *m, const int64_t *h_parents, int J, int posedirs_cols, int nbetas);
+/* Forward: rotmats [24,3,3] fp32 (cat of global_orient[0], body_pose[0]) -> aa [24,3] (written), or rotmats = NULL
+ * and aa read as given; betas [10], trans [3], scale [1] fp32 (read on the device) -> voxel_verts [8000,3].  `state`:
+ * icon_tetra_state_bytes() bytes of scratch.  Two launches, no host sync. */
+size_t icon_tetra_state_bytes(void);
+int icon_tetra_forward(const icon_tetra_model *m, const float *rotmats, float *aa, const float *betas,
+                       const float *trans, const float *scale, float *voxel_verts, void *state, size_t state_bytes,
+                       icon_stream_t stream);
+
 /* ------------------------------------------------------------------ encoder operators
  * Replace the cuDNN / torch calls of the encoders (lib/net/HGFilters.py, FBNet.py, NormalNet.py, VE.py).  The first
  * two take NCHW fp32 tensors; every 2-D convolution and normalisation runs on the NHWC path after them. */
