@@ -12,7 +12,8 @@
 //   (A) greedy descent to the leaf nearest the descent centre c: a first bound for every lane;
 //   (B) breadth-first cull of the tree, 32 child boxes per step, ballot-compacted into a frontier in shared memory,
 //       against the warp's bound; the bound tightens with the nearest far corner on the way down;
-//   (C) the surviving leaves' faces, 32 at a time: culled by bounding sphere against the warp's box, staged in shared
+//   (C) the surviving leaves' faces, 32 at a time: culled by bounding sphere against the warp's box (and, with 32
+//       points per warp, by a support bound that follows the lanes' own bounds: NearestFace::beats), staged in shared
 //       memory, then every lane tests them against ITS OWN best through two cheap lower bounds (sphere, support
 //       function) before the exact Ericson distance (tri_sqdist).
 // A node or face is skipped only when its bound is strictly farther than the current best, and every bound carries
@@ -138,13 +139,26 @@ struct WalkSmem : ChunkSmem {
 template <int PPW>
 struct NearestFace {
     static constexpr int REP = 32 / PPW;
+    // `beats` pays where 32 distinct points share the box; with fewer per warp the box is small and the lanes' own
+    // support tests already cut nearly as much, and it measured slower at PPW 1 and 8 (H100 80GB HBM3, 700 W)
+    static constexpr bool CULL = PPW == 32;
     const int lane;
     V3 p;
     float tol, tol_sup;                // additive slack on lengths / on the support bound
     float best = FLT_MAX;              // squared distance
     int bi = 0x7fffffff;               // original face id
     float sb = 0.f, ub = 0.f;          // phase C: ~sqrt(best) inflated (this lane), the warp's loosest bound
+    V3 g;                              // phase C: slope of the lanes' bounds across the warp's box (see beats)
+    float beta = 0.f;                  // max over lanes of min(sb, ub) - g.(p - box centre)
     int staged = 0;                    // faces staged by phase C (ICON_SDF_STATS)
+#ifdef ICON_SDF_STATS
+    int n_sph = 0, n_exact = 0, n_win = 0;   // this lane's faces past the sphere test, past the support test, taken
+    int n_dead = 0;                    // staged faces no lane got past the sphere test with
+    bool last_sph = false;
+#define NF_STAT(x) x
+#else
+#define NF_STAT(x)
+#endif
 
     __device__ __forceinline__ NearestFace(V3 p_, float tol_, float tol_sup_)
         : lane(threadIdx.x & 31), p(p_), tol(tol_), tol_sup(tol_sup_) {}
@@ -184,10 +198,31 @@ struct NearestFace {
         for (int k = 4 * node; k < min(4 * node + 4, t.F); ++k) try_face(t.tri_s + 3 * (size_t)k, __ldg(t.order + k));
     }
 
-    // phase C's bounds, given that every lane's nearest face is within ubw
-    __device__ __forceinline__ void start_scan(float ubw) {
+    __device__ __forceinline__ static float warp_sum(float v) {
+        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        return v;
+    }
+    __device__ __forceinline__ V3 box_offset(float4 wlo, float4 whi) const {
+        return mk3(p.x - 0.5f * (wlo.x + whi.x), p.y - 0.5f * (wlo.y + whi.y), p.z - 0.5f * (wlo.z + whi.z));
+    }
+    __device__ __forceinline__ void update_beta(float4 wlo, float4 whi) {
+        beta = warp_max(fminf(sb, ub) - dot3(g, box_offset(wlo, whi)));
+    }
+
+    // phase C's bounds, given that every lane's nearest face is within ubw; [wlo, whi] holds every lane's point.
+    // g is the least-squares slope of the lanes' first bounds over their offsets from the box centre, about the
+    // gradient of the distance across the warp: it only makes `beats` tighter, any finite g keeps it a bound
+    __device__ __forceinline__ void start_scan(float ubw, float4 wlo, float4 whi) {
         sb = sphere_bound(best);
         ub = ubw * 1.00001f + tol;
+        if (!CULL) return;
+        const V3 o = box_offset(wlo, whi);
+        const float sx = warp_sum(o.x * o.x), sy = warp_sum(o.y * o.y), sz = warp_sum(o.z * o.z);
+        const float bx = warp_sum(o.x * sb), by = warp_sum(o.y * sb), bz = warp_sum(o.z * sb);
+        // 0 on an axis the points do not span, clamped to [-1, 1] (the distance is 1-Lipschitz)
+        auto slope = [](float num, float den) { return den > 0.f ? fminf(fmaxf(num / den, -1.f), 1.f) : 0.f; };
+        g = mk3(slope(bx, sx), slope(by, sy), slope(bz, sz));
+        update_beta(wlo, whi);
     }
 
     // phase C, one lane: sorted face k with bounding sphere s and record tr (dereferenced only past the sphere test)
@@ -195,7 +230,9 @@ struct NearestFace {
         const float dx = p.x - s.x, dy = p.y - s.y, dz = p.z - s.z;
         const float dd = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
         const float l = sb + s.w;
+        NF_STAT(last_sph = false);
         if (dd > l * l) return;                                // sphere bound beats this lane's best
+        NF_STAT(++n_sph; last_sph = true);
         // support-function bound d >= |w| - max_k u.(v_k - c_f), u = w/|w|, w = p - c_f: nearly exact head-on
         const float4 r0 = tr[0], r1 = tr[1], r2 = tr[2];
         const V3 ab = mk3(r0.w, r1.x, r1.y), ac = mk3(r1.z, r1.w, r2.x);
@@ -204,8 +241,10 @@ struct NearestFace {
         const float M = fmaxf(fmaxf(-(S1 + T1), fmaf(2.f, S1, -T1)), fmaf(2.f, T1, -S1)) * (1.f / 3.f);
         const float g = dd - M - tol_sup;                      // |w|^2 - |w| h(u)
         if (g > 0.f && g * g > best * dd * 1.0001f) return;   // support bound beats this lane's best
+        NF_STAT(++n_exact);
         const float d = tri_sqdist(p, mk3(r0.x, r0.y, r0.z), ab, ac);
         if (!(d <= best)) return;                              // also drops NaN, as the brute-force scans do
+        NF_STAT(++n_win);
         const int f = __ldg(t.order + k);
         if (d < best || f < bi) { best = d; bi = f; sb = sphere_bound(d); }
     }
@@ -220,18 +259,46 @@ struct NearestFace {
         }
     }
 
-    // phase C, one step: this lane's slot holds `leaf` (-1: none), 4 lanes per leaf, 8 leaves = 32 faces, culled by
-    // bounding sphere against the warp's box [wlo, whi] and bound, staged compacted, then split over the replicas
+    // True when no lane can take the face (s: centroid, r0..r2: record): a support bound against the warp's box
+    // [wlo, whi] (centre pc, half extents hb) that follows the lanes' own bounds sb_i <= beta + g.(p_i - pc).  For the
+    // unit vector e from the centroid c towards pc, lane i's distance to any point q of the face is at least
+    //   e.(p_i - q) >= e.(pc - c) + e.(p_i - pc) - max_k e.(v_k - c)
+    //              >= sb_i + |pc - c| - max_k e.(v_k - c) - beta - sum_k |e_k - g_k| hb_k,
+    // so the face is out for every lane once the last four terms are positive, with float slack.  Seen from afar the
+    // lanes' distances to a flat region move with g, so the box's extent costs only where e leaves that direction.
+    // False on a NaN (box centre on the centroid).
+    __device__ __forceinline__ bool beats(float4 s, float4 r0, float4 r1, float4 r2, float4 wlo, float4 whi) const {
+        const float vx = 0.5f * (wlo.x + whi.x) - s.x, vy = 0.5f * (wlo.y + whi.y) - s.y,
+                    vz = 0.5f * (wlo.z + whi.z) - s.z;
+        const float L = sqrtf(fmaf(vz, vz, fmaf(vy, vy, vx * vx)));
+        const float il = 1.f / L;
+        const float ex = vx * il, ey = vy * il, ez = vz * il;
+        const float S1 = fmaf(ez, r1.y, fmaf(ey, r1.x, ex * r0.w));           // e.ab
+        const float T1 = fmaf(ez, r2.x, fmaf(ey, r1.w, ex * r1.z));           // e.ac
+        const float he = fmaxf(fmaxf(-(S1 + T1), fmaf(2.f, S1, -T1)), fmaf(2.f, T1, -S1)) * (1.f / 3.f);
+        const float pr = fmaf(fabsf(ez - g.z), 0.5f * (whi.z - wlo.z),
+                              fmaf(fabsf(ey - g.y), 0.5f * (whi.y - wlo.y), fabsf(ex - g.x) * (0.5f * (whi.x - wlo.x))));
+        return L - he - pr - beta > tol + 1e-5f * (L + fabsf(he) + pr + fabsf(beta));
+    }
+
+    // phase C, one step: this lane's slot holds `leaf` (-1: none), 4 lanes per leaf, 8 leaves = 32 faces, culled
+    // against the warp's box [wlo, whi] by bounding sphere and the loosest lane bound, then by `beats`, staged
+    // compacted, then split over the replicas
     __device__ __forceinline__ void chunk(const FaceTree &t, ChunkSmem &S, int leaf, float4 wlo, float4 whi) {
         bool pass = false;
         int k = 0;
-        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+        float4 s = make_float4(0.f, 0.f, 0.f, 0.f), r0 = s, r1 = s, r2 = s;
         if (leaf >= 0) {
             k = 4 * leaf + (lane & 3);
             if (k < t.F) {
                 s = __ldg(t.sph_s + k);
                 const float l2 = ub + s.w;                     // sphere vs the warp's box: some lane may be that close
                 pass = box_dist2(mk3(s.x, s.y, s.z), wlo, whi) <= l2 * l2;
+                if (CULL && pass) {
+                    const float4 *tp = t.tri_s + 3 * (size_t)k;
+                    r0 = __ldg(tp); r1 = __ldg(tp + 1); r2 = __ldg(tp + 2);
+                    pass = !beats(s, r0, r1, r2, wlo, whi);
+                }
             }
         }
         const unsigned mask = __ballot_sync(0xffffffffu, pass);
@@ -239,18 +306,25 @@ struct NearestFace {
         staged += cnt;
         if (pass) {
             const int at = __popc(mask & ((1u << lane) - 1u));
-            const float4 *tp = t.tri_s + 3 * (size_t)k;
             S.sph[at] = s;
             S.kk[at] = k;
-            S.tri[at][0] = __ldg(tp); S.tri[at][1] = __ldg(tp + 1); S.tri[at][2] = __ldg(tp + 2);
+            if (!CULL) {
+                const float4 *tp = t.tri_s + 3 * (size_t)k;
+                r0 = __ldg(tp); r1 = __ldg(tp + 1); r2 = __ldg(tp + 2);
+            }
+            S.tri[at][0] = r0; S.tri[at][1] = r1; S.tri[at][2] = r2;
         }
         __syncwarp();
-        for (int j = lane / PPW; j < cnt; j += REP) test(t, S.kk[j], S.sph[j], &S.tri[j][0]);
+        for (int j = lane / PPW; j < cnt; j += REP) {
+            test(t, S.kk[j], S.sph[j], &S.tri[j][0]);
+            NF_STAT(if (REP == 1) n_dead += !__any_sync(0xffffffffu, last_sph));
+        }
         if (REP > 1) {
             merge();
             sb = sphere_bound(best);
         }
         ub = fminf(ub, warp_max(sb));                          // the lanes' bounds only shrink: cull the next chunk harder
+        if (CULL) update_beta(wlo, whi);
         __syncwarp();
     }
 
@@ -329,7 +403,7 @@ __device__ __forceinline__ int tree_nearest(const FaceTree &t, WalkSmem<Id, CAP>
     float ubw = warp_max(sqrtf(q.best));                       // every lane's nearest is within ubw
     int cur, n;
     const bool ok = tree_cull(t, S.fr, c, rw, wlo, whi, q.tol, ubw, cur, n);
-    q.start_scan(ubw);
+    q.start_scan(ubw, wlo, whi);
     if (ok) q.scan_leaves(t, S, S.fr[cur], n, wlo, whi);
     else q.scan_all(t);
     q.merge();

@@ -142,10 +142,18 @@ __global__ void k_points_scatter(const int32_t *__restrict__ bid, int64_t N, con
 }
 
 #ifdef ICON_SDF_STATS
-__device__ unsigned long long g_stats[8];   // warps, overflow warps, sum leaves, sum faces, sum exact tests, sum ray tests
+// Diagnostics build only (tools/sdf_brick_counters.py).  g_stats: warps, overflow warps, leaves, faces staged (tree
+// walk), then the deferred tree walk's warps and cycles.  g_wstat: one record of WS_N words per brick-path warp.
+__device__ unsigned long long g_stats[8];
+__device__ unsigned *g_wstat;
+enum { WS_DEFER, WS_LEAVES, WS_STEPS, WS_STAGED, WS_SPH, WS_EXACT, WS_WIN, WS_RAY, WS_CYC_START, WS_CYC_C,
+       WS_CYC_RAY, WS_CYC_EMIT, WS_UB0, WS_UBEND, WS_LIST, WS_IDEAL_LEAVES, WS_IDEAL_FACES, WS_DEAD, WS_N = 20 };
 #define STAT(i, v) do { if (lane == 0) atomicAdd(&g_stats[i], (unsigned long long)(v)); } while (0)
+#define WSTAT(i, v) do { if (lane == 0 && g_wstat) g_wstat[(size_t)wid * WS_N + (i)] = (unsigned)(v); } while (0)
+#define WCLK(t) __syncwarp(); const long long t = clock64()
 #else
 #define STAT(i, v) do { } while (0)
+#define WSTAT(i, v) do { } while (0)
 #endif
 
 // 16-bit frontier ids: icon_smpl_prepare checks that the leaf count is <= 65535.  The brick path reads its leaf list
@@ -209,6 +217,12 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
 
     // the body lies in [-1.5, 1.5]^3 and the points that matter in [-1, 1]^3: the walk's fixed slacks
     NearestFace<PPW> nf(p, 1e-6f, 1e-7f);
+#ifdef ICON_SDF_STATS
+    WCLK(t_start);
+    long long t_c = 0, t_ray = 0;
+    int st_leaves = 0, st_steps = 0, st_brick = -1;
+    float st_ub0 = 0.f;
+#endif
     if constexpr (BRICK) {
         bool ok = h.brick_built && !h.brick_overflow && c.x >= -1.f && c.x < 1.f && c.y >= -1.f && c.y < 1.f &&
                   c.z >= -1.f && c.z < 1.f;
@@ -224,12 +238,19 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
         }
         if (!ok) {                     // straddles bricks, leaves the cube or the lists overflowed: the tree walk takes it
             if (lane == 0) defer[atomicAdd(ndefer, 1)] = (int32_t)wid;
+            WSTAT(WS_DEFER, 1);
             return;
         }
         const int f = __ldg(m.bface + b);
         nf.try_face(m.tri + 3 * (size_t)f, f);                // not taken if NaN here; the brick's bound still holds
-        nf.start_scan(fminf(warp_max(sqrtf(nf.best)), __ldg(m.bub + b)));
+        nf.start_scan(fminf(warp_max(sqrtf(nf.best)), __ldg(m.bub + b)), wlo, whi);
         STAT(0, 1);
+#ifdef ICON_SDF_STATS
+        WCLK(t_c0);
+        t_c = t_c0;
+        st_brick = b;
+        st_ub0 = nf.ub;
+#endif
         // the list is sorted by box distance to the brick, which bounds from below every lane's distance to the
         // leaf's faces: once a step's first leaf is farther than the loosest lane bound, so is the rest of the list
         const int o1 = __ldg(m.boff + b + 1);
@@ -240,6 +261,10 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
             if (lane == 0) key = leaf_key(m, leaf, blo, bhi);
             if (__shfl_sync(0xffffffffu, key, 0) > nf.ub * nf.ub) break;
             STAT(2, min(8, o1 - base));
+#ifdef ICON_SDF_STATS
+            st_leaves += min(8, o1 - base);
+            ++st_steps;
+#endif
             nf.chunk(m, S, leaf, wlo, whi);
         }
         nf.merge();
@@ -248,6 +273,10 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
         STAT(0, 1); STAT(1, n > fr_cap(PPW) ? 1 : 0); STAT(2, n);
     }
     STAT(3, nf.staged);
+#ifdef ICON_SDF_STATS
+    WCLK(t_c1);
+    int st_ray = 0;
+#endif
     // ---- +x ray parity
     int hits = 0;
     if (!h.ray_overflow) {
@@ -260,6 +289,9 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
                 if (__ldg(&m.rbox[2 * (size_t)f + 1].x) < p.x - 1e-3f) continue;     // wholly behind the ray origin
                 const Tri tr = load_tri(m.tri + 3 * (size_t)f);
                 hits += ray_hit_px(p, tr.a, tr.ab, tr.ac);
+#ifdef ICON_SDF_STATS
+                ++st_ray;
+#endif
             }
         }
     } else {
@@ -272,13 +304,64 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
 #pragma unroll
         for (int o = PPW; o < 32; o <<= 1) hits += __shfl_xor_sync(0xffffffffu, hits, o);
     }
+#ifdef ICON_SDF_STATS
+    WCLK(t_ray0);
+    t_ray = t_ray0;
+#endif
     if (live && rep_id == 0) emit_record(p, nf.bi, nf.best, hits, m, rec, face, idx);
+#ifdef ICON_SDF_STATS
+    WCLK(t_end);
+    if (BRICK && st_brick >= 0) {
+        // what box distance and bounding sphere alone keep at the final bound: leaves and faces within it of the box
+        const float ube = nf.ub;
+        int il = 0, ifc = 0;
+        const int o0 = __ldg(m.boff + st_brick), o1 = __ldg(m.boff + st_brick + 1);
+        for (int s = o0 + lane; s < o1; s += 32) {
+            const int leaf = __ldg(m.blist + s);
+            const float4 a = __ldg(m.nodes + 2 * (size_t)leaf), z = __ldg(m.nodes + 2 * (size_t)leaf + 1);
+            const float gx = fmaxf(fmaxf(a.x - whi.x, wlo.x - z.x), 0.f);
+            const float gy = fmaxf(fmaxf(a.y - whi.y, wlo.y - z.y), 0.f);
+            const float gz = fmaxf(fmaxf(a.z - whi.z, wlo.z - z.z), 0.f);
+            if (fmaf(gz, gz, fmaf(gy, gy, gx * gx)) > ube * ube) continue;
+            ++il;
+            for (int k = 4 * leaf; k < min(4 * leaf + 4, m.F); ++k) {
+                const float4 s4 = __ldg(m.sph_s + k);
+                const float l2 = ube + s4.w;
+                ifc += box_dist2(mk3(s4.x, s4.y, s4.z), wlo, whi) <= l2 * l2;
+            }
+        }
+        const int s_sph = __reduce_add_sync(0xffffffffu, nf.n_sph), s_exact = __reduce_add_sync(0xffffffffu, nf.n_exact);
+        const int s_win = __reduce_add_sync(0xffffffffu, nf.n_win), s_ray = __reduce_add_sync(0xffffffffu, st_ray);
+        const int s_il = __reduce_add_sync(0xffffffffu, il), s_if = __reduce_add_sync(0xffffffffu, ifc);
+        WSTAT(WS_LEAVES, st_leaves);
+        WSTAT(WS_STEPS, st_steps);
+        WSTAT(WS_STAGED, nf.staged);
+        WSTAT(WS_SPH, s_sph);
+        WSTAT(WS_EXACT, s_exact);
+        WSTAT(WS_WIN, s_win);
+        WSTAT(WS_RAY, s_ray);
+        WSTAT(WS_CYC_START, t_c - t_start);
+        WSTAT(WS_CYC_C, t_c1 - t_c);
+        WSTAT(WS_CYC_RAY, t_ray - t_c1);
+        WSTAT(WS_CYC_EMIT, t_end - t_ray);
+        WSTAT(WS_UB0, __float_as_uint(st_ub0));
+        WSTAT(WS_UBEND, __float_as_uint(ube));
+        WSTAT(WS_LIST, o1 - o0);
+        WSTAT(WS_IDEAL_LEAVES, s_il);
+        WSTAT(WS_IDEAL_FACES, s_if);
+        WSTAT(WS_DEAD, nf.n_dead);
+    }
+    if (!BRICK && defer != nullptr) { STAT(4, 1); STAT(5, t_end - t_start); }
+#endif
 }
 
+// PPW = 32 is held to 64 registers (8 blocks, 32 warps per SM; about 50 bytes of spill): sdf_only on the 256^3 lattice
+// measured 4.65 ms against 5.2 ms at 79 registers and 24 warps (H100 80GB HBM3, 700 W).  The other PPWs keep the
+// compiler's choice (a minimum of 0 blocks is no bound).
 // Without `defer`, warp i of the grid takes the points of warp i.  BRICK appends the warps it leaves to the tree walk
 // to defer[] (count *ndefer); the tree walk given `defer` strides over those warps instead.
 template <int PPW, bool BRICK>
-__global__ void __launch_bounds__(SW_T) k_sdf_warp(const float4 *__restrict__ xyz4, const int32_t *__restrict__ perm,
+__global__ void __launch_bounds__(SW_T, PPW == 32 ? 8 : 0) k_sdf_warp(const float4 *__restrict__ xyz4, const int32_t *__restrict__ perm,
                                                    int64_t N, MeshView m, float *__restrict__ rec,
                                                    int32_t *__restrict__ face, int32_t *__restrict__ defer,
                                                    int32_t *__restrict__ ndefer) {
@@ -574,6 +657,12 @@ using namespace icon;
 extern "C" int icon_debug_sdf_stats(unsigned long long *out, int reset) {
     cudaMemcpyFromSymbol(out, icon::g_stats, sizeof(unsigned long long) * 8);
     if (reset) { unsigned long long z[8] = {0}; cudaMemcpyToSymbol(icon::g_stats, z, sizeof(z)); }
+    return 0;
+}
+
+// per-warp records of the brick path: WS_N words per warp, indexed by warp; nullptr stops recording
+extern "C" int icon_debug_sdf_warp_stats(unsigned *dev_buf) {
+    cudaMemcpyToSymbol(icon::g_wstat, &dev_buf, sizeof(dev_buf));
     return 0;
 }
 #endif
