@@ -1,5 +1,5 @@
-// Error state, launch counter and the device-wide exclusive scan used by the compaction,
-// outlier-rank and marching-cubes passes.
+// Error state, launch counter, the device-wide exclusive scan used by the compaction,
+// outlier-rank and marching-cubes passes, and the row-list (CSR) builder of the mesh steps.
 #include <stdarg.h>
 #include <atomic>
 
@@ -108,6 +108,98 @@ int scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t n, int64_t *d_to
     k_scan_add<<<(unsigned)nb, SCAN_T, 0, stream>>>(out, n, sums);
     ICON_LAUNCHED();
     return ICON_OK;
+}
+
+// ---------------------------------------------------------------- row lists (CSR) from (owner, key) items
+
+__global__ void k_csr_count(const int32_t *__restrict__ own, int64_t n, int32_t *__restrict__ cnt) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && own[i] >= 0) atomicAdd(&cnt[own[i]], 1);
+}
+
+// arrival order; k_csr_sort sorts each row
+__global__ void k_csr_fill(const int32_t *__restrict__ own, const int32_t *__restrict__ key, int64_t n,
+                           const int32_t *__restrict__ off, int32_t *__restrict__ cursor, int32_t *__restrict__ list) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && own[i] >= 0) list[off[own[i]] + atomicAdd(&cursor[own[i]], 1)] = key[i];
+}
+
+// sort each row ascending; ucnt != NULL: drop repeats in place and write the unique count
+__global__ void k_csr_sort(const int32_t *__restrict__ off, int R, int32_t *__restrict__ list,
+                           int32_t *__restrict__ ucnt) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= R) return;
+    int32_t *a = list + off[r];
+    const int n = off[r + 1] - off[r];
+    heap_sort_i32(a, n);
+    if (!ucnt) return;
+    int u = 0;
+    for (int i = 0; i < n; ++i)
+        if (u == 0 || a[i] != a[u - 1]) a[u++] = a[i];
+    ucnt[r] = u;
+}
+
+CsrWs csr_take(Carver &c, int64_t rows) {
+    CsrWs w;
+    w.cnt = c.take<int32_t>((size_t)rows + 1);
+    w.cursor = c.take<int32_t>((size_t)rows);
+    w.scan_ws = c.take<char>(scan_ws_bytes(rows + 1));
+    return w;
+}
+
+int csr_build(const int32_t *own, const int32_t *key, int64_t n, int R, int32_t *off, int32_t *list, int32_t *ucnt,
+              const CsrWs &w, cudaStream_t stream) {
+    ICON_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int32_t) * ((size_t)R + 1), stream));
+    ICON_CUDA(cudaMemsetAsync(w.cursor, 0, sizeof(int32_t) * (size_t)R, stream));
+    const unsigned nb = (unsigned)((n + 255) / 256), rb = (unsigned)((R + 255) / 256);
+    if (n > 0) {
+        k_csr_count<<<nb, 256, 0, stream>>>(own, n, w.cnt);
+        ICON_LAUNCHED();
+    }
+    int rc = scan_exclusive_i32(w.cnt, off, (int64_t)R + 1, nullptr, w.scan_ws, stream);
+    if (rc) return rc;
+    if (n > 0) {
+        k_csr_fill<<<nb, 256, 0, stream>>>(own, key, n, off, w.cursor, list);
+        ICON_LAUNCHED();
+    }
+    if (R > 0) {
+        k_csr_sort<<<rb, 256, 0, stream>>>(off, R, list, ucnt);
+        ICON_LAUNCHED();
+    }
+    return ICON_OK;
+}
+
+// vertex_corners items: corner i = 3 f + k under its vertex; owner -1 for every corner of a face with a bad index
+__global__ void k_corner_items(const int64_t *__restrict__ faces, int F, int V, int32_t *__restrict__ own,
+                               int32_t *__restrict__ key) {
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    int id[3];
+    if (!face_ids(faces, f, V, id)) id[0] = id[1] = id[2] = -1;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        own[3 * f + k] = id[k];
+        key[3 * f + k] = 3 * f + k;
+    }
+}
+
+static size_t vc_carve(void *ws, int V, int F, int32_t **own, int32_t **key, CsrWs *csr) {
+    Carver c(ws);
+    int32_t *o = c.take<int32_t>(3 * (size_t)F), *k = c.take<int32_t>(3 * (size_t)F);
+    const CsrWs w = csr_take(c, V);
+    if (csr) *own = o, *key = k, *csr = w;
+    return c.total();
+}
+
+size_t vertex_corners_ws_bytes(int V, int F) { return vc_carve(nullptr, V, F, nullptr, nullptr, nullptr); }
+
+int vertex_corners(const int64_t *faces, int F, int V, int32_t *off, int32_t *list, void *ws, cudaStream_t stream) {
+    int32_t *own, *key;
+    CsrWs w;
+    vc_carve(ws, V, F, &own, &key, &w);
+    k_corner_items<<<(unsigned)((F + 255) / 256), 256, 0, stream>>>(faces, F, V, own, key);
+    ICON_LAUNCHED();
+    return csr_build(own, key, 3 * (int64_t)F, V, off, list, nullptr, w, stream);
 }
 
 static bool g_prof = false;

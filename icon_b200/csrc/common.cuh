@@ -129,6 +129,17 @@ __device__ __forceinline__ void heap_sort_i32(int32_t *a, int n) {
     }
 }
 
+// face f's three vertex ids; false when one of them is outside [0, V)
+__device__ __forceinline__ bool face_ids(const int64_t *faces, int f, int V, int id[3]) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const int64_t x = faces[3 * (int64_t)f + k];
+        if (x < 0 || x >= V) return false;
+        id[k] = (int)x;
+    }
+    return true;
+}
+
 // ---------------------------------------------------------------- mesh workspace layout
 constexpr int TREE_MAX_LEVELS = 17;  // 4-ary implicit tree over leaves of 4 Morton-sorted faces: 4^16 leaves > 2^31 faces
 constexpr int RAY_GRID = 256;        // yz cell grid for the +x ray parity
@@ -171,6 +182,7 @@ struct MeshView : FaceTree {
     const float4 *attr;   // [F][6]: normals 9, cmap 9, vis 3, pad 3
     const float4 *rbox;   // [F][2]: (ymin, ymax, zmin, zmax) (xmax, xmin, -, -)
     float *vnormals;      // [V][3] scratch
+    void *vn_ws;          // area_vertex_normals' workspace
     unsigned long long *keys;   // [F] morton << 32 | face: the sort keys of the tree
     // ray grid
     int32_t *rcount;      // [RAY_GRID^2 + 1]
@@ -200,5 +212,35 @@ void profile_mark(int i, cudaStream_t stream);
 size_t scan_ws_bytes(int64_t n);
 int scan_exclusive_i32(const int32_t *in, int32_t *out, int64_t n, int64_t *d_total /*may be null*/,
                        void *ws, cudaStream_t stream);
+
+// row lists (CSR) from (owner, key) items: rows R from n items, an item with owner < 0 is dropped; off [R+1],
+// list [the n' listed items], each row ascending (with ucnt: repeats dropped in place, the unique count written)
+struct CsrWs {
+    int32_t *cnt, *cursor;
+    void *scan_ws;
+};
+CsrWs csr_take(Carver &c, int64_t rows);
+int csr_build(const int32_t *own, const int32_t *key, int64_t n, int R, int32_t *off, int32_t *list, int32_t *ucnt,
+              const CsrWs &w, cudaStream_t stream);
+
+// per vertex, the corners 3 f + k, ascending, of every face whose three indices are in [0, V): off [V+1], list [3F]
+size_t vertex_corners_ws_bytes(int V, int F);
+int vertex_corners(const int64_t *faces, int F, int V, int32_t *off, int32_t *list, void *ws, cudaStream_t stream);
+
+// pytorch3d's (pass, face) order over one vertex's corner list: passes 0, 1, 2 visit its corners 3 f + c with
+// c = 1, 2, 0, each pass in ascending f; fn(f, c)
+template <class Fn>
+__device__ __forceinline__ void for_each_pass_corner(const int32_t *corners, int n, Fn &&fn) {
+    for (int pass = 0; pass < 3; ++pass) {
+        const int c = (pass + 1) % 3;
+        for (int i = 0; i < n; ++i)
+            if (corners[i] % 3 == c) fn(corners[i] / 3, c);
+    }
+}
+
+// pytorch3d's area-weighted vertex normals (normals.cu): out [V,3]
+size_t area_vertex_normals_ws_bytes(int V, int F);
+int area_vertex_normals(const float *verts, int V, const int64_t *faces, int F, float *out, void *ws,
+                        cudaStream_t stream);
 
 }  // namespace icon

@@ -14,10 +14,11 @@
 //   vert_edges    per vertex, the ids of the edges it is an endpoint of, ascending; a self-loop is listed twice, so
 //                 deg_i = the row length = the count of edge endpoints at i.
 //   edge_entries  per edge, the face-corner entries 3 f + col (col of face_to_edge) that map to it, ascending.
-//   vert_corners  per vertex, the corners 3 f + c with faces[f][c] = i, ascending.
-//   Construction: each corner pair (min, max) is listed under min; each list is heap-sorted and de-duplicated in place,
-//   and a scan of the unique counts gives edge ids in (min, max) order with no global sort.  The edge count is read
-//   back to the host once per build (the caller caches the topology: the faces do not change across the loop).
+//   vert_corners  per vertex, the corners 3 f + c with faces[f][c] = i, ascending (common.cu's vertex_corners).
+//   Construction: every list comes from common.cu's row-list builder (csr_build).  Each corner pair (min, max) is
+//   listed under min; each list is heap-sorted and de-duplicated in place, and a scan of the unique counts gives edge
+//   ids in (min, max) order with no global sort.  The edge count is read back to the host once per build (the caller
+//   caches the topology: the faces do not change across the loop).
 //
 // Priors (icon_mesh_priors_forward / _backward), for one mesh:
 //   edge = (1/E) sum_e (L_e - 0)^2, L_e = sqrt(d.d), d = v_a - v_b.  Backward: 2 d (g/E) to a, -2 d (g/E) to b; at
@@ -67,71 +68,6 @@ __device__ __forceinline__ double pr_block_sum(double x, double *sh) {
     return r;
 }
 
-// ---------------------------------------------------------------- row lists (CSR) from (owner, key) items
-
-__global__ void k_csr_count(const int32_t *__restrict__ own, int64_t n, int32_t *__restrict__ cnt) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && own[i] >= 0) atomicAdd(&cnt[own[i]], 1);
-}
-
-// arrival order; k_csr_sort sorts each row
-__global__ void k_csr_fill(const int32_t *__restrict__ own, const int32_t *__restrict__ key, int64_t n,
-                           const int32_t *__restrict__ off, int32_t *__restrict__ cursor, int32_t *__restrict__ list) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && own[i] >= 0) list[off[own[i]] + atomicAdd(&cursor[own[i]], 1)] = key[i];
-}
-
-// sort each row ascending; ucnt != NULL: drop repeats in place and write the unique count
-__global__ void k_csr_sort(const int32_t *__restrict__ off, int R, int32_t *__restrict__ list,
-                           int32_t *__restrict__ ucnt) {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= R) return;
-    int32_t *a = list + off[r];
-    const int n = off[r + 1] - off[r];
-    heap_sort_i32(a, n);
-    if (!ucnt) return;
-    int u = 0;
-    for (int i = 0; i < n; ++i)
-        if (u == 0 || a[i] != a[u - 1]) a[u++] = a[i];
-    ucnt[r] = u;
-}
-
-struct CsrWs {
-    int32_t *cnt, *cursor;
-    void *scan_ws;
-};
-
-static CsrWs csr_take(Carver &c, int64_t rows) {
-    CsrWs w;
-    w.cnt = c.take<int32_t>((size_t)rows + 1);
-    w.cursor = c.take<int32_t>((size_t)rows);
-    w.scan_ws = c.take<char>(scan_ws_bytes(rows + 1));
-    return w;
-}
-
-// rows R from n items: off [R+1], list [n valid items], each row ascending (repeats dropped when ucnt is given)
-static int csr_build(const int32_t *own, const int32_t *key, int64_t n, int R, int32_t *off, int32_t *list,
-                     int32_t *ucnt, const CsrWs &w, cudaStream_t stream) {
-    ICON_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int32_t) * ((size_t)R + 1), stream));
-    ICON_CUDA(cudaMemsetAsync(w.cursor, 0, sizeof(int32_t) * (size_t)R, stream));
-    const unsigned nb = (unsigned)((n + 255) / 256), rb = (unsigned)((R + 255) / 256);
-    if (n > 0) {
-        k_csr_count<<<nb, 256, 0, stream>>>(own, n, w.cnt);
-        ICON_LAUNCHED();
-    }
-    int rc = scan_exclusive_i32(w.cnt, off, (int64_t)R + 1, nullptr, w.scan_ws, stream);
-    if (rc) return rc;
-    if (n > 0) {
-        k_csr_fill<<<nb, 256, 0, stream>>>(own, key, n, off, w.cursor, list);
-        ICON_LAUNCHED();
-    }
-    if (R > 0) {
-        k_csr_sort<<<rb, 256, 0, stream>>>(off, R, list, ucnt);
-        ICON_LAUNCHED();
-    }
-    return ICON_OK;
-}
-
 // ---------------------------------------------------------------- topology
 
 // corner pair col of a face: col 0 = (v1, v2), 1 = (v2, v0), 2 = (v0, v1)
@@ -144,18 +80,16 @@ __global__ void k_tp_pairs(const int64_t *__restrict__ faces, int F, int V, int3
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= F) return;
     int id[3];
-    bool ok = true;
+    if (!face_ids(faces, f, V, id)) {
+        *bad = 1;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const int64_t x = faces[3 * (int64_t)f + k];
-        ok = ok && x >= 0 && x < V;
-        id[k] = ok ? (int)x : 0;
+        for (int col = 0; col < 3; ++col) own[3 * f + col] = -1;
+        return;
     }
-    if (!ok) *bad = 1;
 #pragma unroll
     for (int col = 0; col < 3; ++col) {
         const int a = id[tp_c1(col)], b = id[tp_c2(col)];
-        own[3 * f + col] = ok ? min(a, b) : -1;
+        own[3 * f + col] = min(a, b);
         key[3 * f + col] = max(a, b);
     }
 }
@@ -198,15 +132,6 @@ __global__ void k_tp_f2e(const int64_t *__restrict__ faces, int F, const int32_t
     }
 }
 
-// vert_corners items
-__global__ void k_tp_corners(const int64_t *__restrict__ faces, int F, int32_t *__restrict__ own,
-                             int32_t *__restrict__ key) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= 3 * F) return;
-    own[i] = (int)faces[i];
-    key[i] = i;
-}
-
 struct TpWs {
     int32_t *own, *key;       // [6F] items
     int32_t *poff, *plist;    // pair lists: [V+1], [3F]
@@ -229,7 +154,8 @@ static size_t tp_carve(void *ws, int V, int F, TpWs *o) {
     w.bad = c.take<int32_t>(1);
     w.csr = csr_take(c, (int64_t)(V > 3 * F ? V : 3 * F));
     if (o) *o = w;
-    return c.total();
+    const size_t vc = vertex_corners_ws_bytes(V, F);    // the corner lists are built last, over the whole workspace
+    return c.total() > vc ? c.total() : vc;
 }
 
 // vert_edges of `edges` [E,2] (every index in [0, V), checked by the caller): the own/key items, then the lists
@@ -706,9 +632,7 @@ extern "C" int icon_mesh_topology_build(const icon_mesh_topology *t, void *ws, s
     ICON_LAUNCHED();
     rc = csr_build(w.own, w.key, 3 * (int64_t)F, E, t->edge_off, t->edge_entries, nullptr, w.csr, stream);
     if (rc) return rc;
-    k_tp_corners<<<(unsigned)((3 * (int64_t)F + 255) / 256), 256, 0, stream>>>(t->faces, F, w.own, w.key);
-    ICON_LAUNCHED();
-    return csr_build(w.own, w.key, 3 * (int64_t)F, V, t->corner_off, t->vert_corners, nullptr, w.csr, stream);
+    return vertex_corners(t->faces, F, V, t->corner_off, t->vert_corners, ws, stream);
 }
 
 extern "C" size_t icon_vertex_edges_workspace_bytes(int V, int E) {

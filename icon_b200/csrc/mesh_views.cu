@@ -7,17 +7,8 @@
 // operation for operation by oracle/mesh_views.py (hence -fmad=false for this file).  All arithmetic is fp32, one
 // rounding per operation, in the order written; "e(p, a, b)" is (p.x - a.x)(b.y - a.y) - (p.y - a.y)(b.x - a.x).
 //
-// Vertex normals (icon_area_vertex_normals), pytorch3d's verts_normals_packed as oracle_vertex_normals restates it:
-//   three passes (corner 1, 2, 0), each in face order, add n = (p1 - p0) x (p2 - p0) to vertex p0, where p1, p2 are
-//   the next two corners of the face; then n / max(sqrt((x x + y y) + z z), 1e-6).  Each vertex's contributions are
-//   sorted by (pass, face) and summed in that order: no float atomics, bitwise reproducible.  Faces with an index
-//   outside [0, V) contribute nothing.
-//   Backward (icon_area_vertex_normals_backward; restated by oracle/mesh_priors.py with float64 autograd): the
-//   gradient of F.normalize(s, eps = 1e-6) with torch's semantics, from the fp32 s of the forward, in fp64:
-//   (g - n (n.g)) / |s| with n = s / |s| when the fp32 norm is >= 1e-6, else g / 1e-6 (clamp_min passes g there);
-//   then through each corner product n = u x w (u = p1 - p0, w = p2 - p0): p1 += w x G, p2 += G x u,
-//   p0 -= both.  Each vertex sums its contributions over the same sorted (pass, face) lists in fp64 (its own position
-//   in each listed face, all three products of that face) and rounds once.
+// The vertex normals behind those colours (icon_area_vertex_normals, with its backward) are normals.cu's
+// area-weighted rule.
 //
 // Views (icon_mesh_views).  Cameras: view a has eye = (100 cos t, y_c, 100 sin t), at = (0, y_c, 0), up = +y;
 //   look_at_view_transform's basis z = unit(at - eye), x = unit(up x z), y = unit(z x x), and FoVOrthographicCameras
@@ -99,8 +90,9 @@
 //   keys in the caller's state buffer; k_mr_pixel turns the upstream gradient into per-slot partials (NORMAL: Gcol,
 //   Gz, Gdist, with the slots' weights, colours and Gw parked there first; SILHOUETTE: Gdist); k_mr_face_small / _big re-traverse each (face, view)'s pixel box in a fixed order,
 //   find the face's own key among the pixel's slots and sum its three corners' (Gx, Gy, Gz, GC) in fp64 (big boxes: a
-//   block per face, fixed-order tree reduction); k_mr_vertex sums each vertex's corner contributions in the sorted
-//   (pass, face) order of k_an_*, view after view, applies M^T in fp64 and rounds to fp32 once.
+//   block per face, fixed-order tree reduction); k_mr_vertex sums each vertex's corner contributions over its
+//   vertex_corners list in the area rule's (pass, face) order, view after view, applies M^T in fp64 and rounds to fp32
+//   once.
 #include <math.h>
 
 #include "common.cuh"
@@ -127,158 +119,6 @@ struct MvSilhouette {                             // silhouette: sigmoid_alpha_b
     static constexpr bool CULL = true, CUT = false;
     static constexpr float BLUR = 4.605120047926903e-04f;              // ln(1/1e-4 - 1) 5e-5
 };
-
-// ---------------------------------------------------------------- area-weighted vertex normals
-
-__device__ __forceinline__ bool mv_face_ids(const int64_t *faces, int f, int V, int id[3]) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const int64_t x = faces[3 * (int64_t)f + k];
-        if (x < 0 || x >= V) return false;
-        id[k] = (int)x;
-    }
-    return true;
-}
-
-__global__ void k_an_count(const int64_t *__restrict__ faces, int F, int V, int32_t *__restrict__ cnt) {
-    const int f = blockIdx.x * blockDim.x + threadIdx.x;
-    int id[3];
-    if (f >= F || !mv_face_ids(faces, f, V, id)) return;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) atomicAdd(&cnt[id[k]], 1);
-}
-
-// contribution keys pass * F + f (pass 0, 1, 2 = corner 1, 2, 0), in arrival order; k_an_sum sorts each list
-__global__ void k_an_fill(const int64_t *__restrict__ faces, int F, int V, const int32_t *__restrict__ off,
-                          int32_t *__restrict__ cursor, int32_t *__restrict__ keys) {
-    const int f = blockIdx.x * blockDim.x + threadIdx.x;
-    int id[3];
-    if (f >= F || !mv_face_ids(faces, f, V, id)) return;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) keys[off[id[k]] + atomicAdd(&cursor[id[k]], 1)] = ((k + 2) % 3) * F + f;
-}
-
-__global__ void k_an_sum(const float *__restrict__ verts, const int64_t *__restrict__ faces, int F,
-                         const int32_t *__restrict__ off, int32_t *__restrict__ keys, int V, float *__restrict__ out) {
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    int32_t *a = keys + off[v];
-    const int n = off[v + 1] - off[v];
-    heap_sort_i32(a, n);
-    float sx = 0.f, sy = 0.f, sz = 0.f;
-    for (int i = 0; i < n; ++i) {
-        const int pass = a[i] / F, f = a[i] % F;
-        const int c = pass == 0 ? 1 : (pass == 1 ? 2 : 0);
-        const int64_t i0 = faces[3 * (int64_t)f + c], i1 = faces[3 * (int64_t)f + (c + 1) % 3];
-        const int64_t i2 = faces[3 * (int64_t)f + (c + 2) % 3];
-        const float p0x = verts[3 * i0], p0y = verts[3 * i0 + 1], p0z = verts[3 * i0 + 2];
-        const float ux = verts[3 * i1] - p0x, uy = verts[3 * i1 + 1] - p0y, uz = verts[3 * i1 + 2] - p0z;
-        const float wx = verts[3 * i2] - p0x, wy = verts[3 * i2 + 1] - p0y, wz = verts[3 * i2 + 2] - p0z;
-        sx = sx + (uy * wz - uz * wy);
-        sy = sy + (uz * wx - ux * wz);
-        sz = sz + (ux * wy - uy * wx);
-    }
-    float nrm = sqrtf((sx * sx + sy * sy) + sz * sz);
-    if (nrm < 1e-6f) nrm = 1e-6f;
-    out[3 * (int64_t)v] = sx / nrm; out[3 * (int64_t)v + 1] = sy / nrm; out[3 * (int64_t)v + 2] = sz / nrm;
-}
-
-// backward, 1: sort the vertex's list, recompute s as k_an_sum does, then the normalize gradient (fp64) into gs
-__global__ void k_an_grad_s(const float *__restrict__ verts, const int64_t *__restrict__ faces, int F,
-                            const int32_t *__restrict__ off, int32_t *__restrict__ keys, int V,
-                            const float *__restrict__ gn, double *__restrict__ gs) {
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    int32_t *a = keys + off[v];
-    const int n = off[v + 1] - off[v];
-    heap_sort_i32(a, n);
-    float sx = 0.f, sy = 0.f, sz = 0.f;
-    for (int i = 0; i < n; ++i) {
-        const int pass = a[i] / F, f = a[i] % F;
-        const int c = pass == 0 ? 1 : (pass == 1 ? 2 : 0);
-        const int64_t i0 = faces[3 * (int64_t)f + c], i1 = faces[3 * (int64_t)f + (c + 1) % 3];
-        const int64_t i2 = faces[3 * (int64_t)f + (c + 2) % 3];
-        const float p0x = verts[3 * i0], p0y = verts[3 * i0 + 1], p0z = verts[3 * i0 + 2];
-        const float ux = verts[3 * i1] - p0x, uy = verts[3 * i1 + 1] - p0y, uz = verts[3 * i1 + 2] - p0z;
-        const float wx = verts[3 * i2] - p0x, wy = verts[3 * i2 + 1] - p0y, wz = verts[3 * i2 + 2] - p0z;
-        sx = sx + (uy * wz - uz * wy);
-        sy = sy + (uz * wx - ux * wz);
-        sz = sz + (ux * wy - uy * wx);
-    }
-    const double s[3] = {sx, sy, sz};
-    const double g[3] = {gn[3 * (int64_t)v], gn[3 * (int64_t)v + 1], gn[3 * (int64_t)v + 2]};
-    const double len = sqrt((s[0] * s[0] + s[1] * s[1]) + s[2] * s[2]);
-    const float nrm = sqrtf((sx * sx + sy * sy) + sz * sz);
-    if (nrm < 1e-6f) {                                    // the clamp: g / eps
-#pragma unroll
-        for (int k = 0; k < 3; ++k) gs[3 * (int64_t)v + k] = g[k] / 1e-6;
-        return;
-    }
-    const double d = ((s[0] * g[0] + s[1] * g[1]) + s[2] * g[2]) / len;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) gs[3 * (int64_t)v + k] = (g[k] - (s[k] / len) * d) / len;
-}
-
-// backward, 2: per vertex, over its sorted (pass, face) entries, the derivative of the entry face's three corner
-// products n_k = (p_{k+1} - p_k) x (p_{k+2} - p_k) with respect to the vertex's own position in the face
-__global__ void k_an_grad_v(const float *__restrict__ verts, const int64_t *__restrict__ faces, int F,
-                            const int32_t *__restrict__ off, const int32_t *__restrict__ keys, int V,
-                            const double *__restrict__ gs, float *__restrict__ gv) {
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    const int32_t *a = keys + off[v];
-    const int n = off[v + 1] - off[v];
-    double acc[3] = {0.0, 0.0, 0.0};
-    for (int i = 0; i < n; ++i) {
-        const int pass = a[i] / F, f = a[i] % F;
-        const int c = pass == 0 ? 1 : (pass == 1 ? 2 : 0);              // the vertex's corner in face f
-        double p[3][3];
-        int64_t id[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            id[k] = faces[3 * (int64_t)f + k];
-#pragma unroll
-            for (int q = 0; q < 3; ++q) p[k][q] = (double)verts[3 * id[k] + q];
-        }
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {                                   // corner k's product, added to vertex id[k]
-            const double *G = gs + 3 * id[k];
-            double u[3], w[3];
-#pragma unroll
-            for (int q = 0; q < 3; ++q) {
-                u[q] = p[(k + 1) % 3][q] - p[k][q];
-                w[q] = p[(k + 2) % 3][q] - p[k][q];
-            }
-            const double gu[3] = {w[1] * G[2] - w[2] * G[1], w[2] * G[0] - w[0] * G[2], w[0] * G[1] - w[1] * G[0]};
-            const double gw[3] = {G[1] * u[2] - G[2] * u[1], G[2] * u[0] - G[0] * u[2], G[0] * u[1] - G[1] * u[0]};
-#pragma unroll
-            for (int q = 0; q < 3; ++q) {
-                if (c == k) acc[q] -= gu[q] + gw[q];
-                else if (c == (k + 1) % 3) acc[q] += gu[q];
-                else acc[q] += gw[q];
-            }
-        }
-    }
-#pragma unroll
-    for (int q = 0; q < 3; ++q) gv[3 * (int64_t)v + q] = (float)acc[q];
-}
-
-struct AnWs {
-    int32_t *cnt, *off, *cursor, *keys;
-    void *scan_ws;
-};
-
-static size_t an_carve(void *ws, int V, int F, AnWs *o) {
-    Carver c(ws);
-    AnWs w;
-    w.cnt = c.take<int32_t>((size_t)V + 1);
-    w.off = c.take<int32_t>((size_t)V + 1);
-    w.cursor = c.take<int32_t>((size_t)V);
-    w.keys = c.take<int32_t>(3 * (size_t)F);
-    w.scan_ws = c.take<char>(scan_ws_bytes((int64_t)V + 1));
-    if (o) *o = w;
-    return c.total();
-}
 
 // ---------------------------------------------------------------- views
 
@@ -316,7 +156,7 @@ template <class M>
 __device__ __forceinline__ bool mv_setup(const int64_t *__restrict__ faces, const float4 *__restrict__ vrec, int f,
                                          int V, int S, MvTri &t) {
     int id[3];
-    if (!mv_face_ids(faces, f, V, id)) return false;
+    if (!face_ids(faces, f, V, id)) return false;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         const float4 r = vrec[id[k]];
@@ -834,28 +674,25 @@ __global__ void __launch_bounds__(256, 1) k_mr_face_big(const int64_t *__restric
     }
 }
 
-// one thread per vertex: its corners in sorted (pass, face) order, view after view, M^T in fp64
+// one thread per vertex: its corners in pytorch3d's (pass, face) order, view after view, M^T in fp64
 template <class M>
-__global__ void k_mr_vertex(const int64_t *__restrict__ faces, int F, int V, int A, const float *__restrict__ mats,
-                            const int32_t *__restrict__ off, int32_t *__restrict__ keys,
-                            const double *__restrict__ fgrad, float *__restrict__ gverts, float *__restrict__ gcolors) {
+__global__ void k_mr_vertex(int F, int V, int A, const float *__restrict__ mats, const int32_t *__restrict__ off,
+                            const int32_t *__restrict__ corners, const double *__restrict__ fgrad,
+                            float *__restrict__ gverts, float *__restrict__ gcolors) {
     const int v = blockIdx.x * blockDim.x + threadIdx.x;
     if (v >= V) return;
-    int32_t *kl = keys + off[v];
+    const int32_t *kl = corners + off[v];
     const int n = off[v + 1] - off[v];
-    heap_sort_i32(kl, n);
     double gv[3] = {0.0, 0.0, 0.0}, gc[3] = {0.0, 0.0, 0.0};
     for (int a = 0; a < A; ++a) {
         double s[M::NG];
 #pragma unroll
         for (int q = 0; q < M::NG; ++q) s[q] = 0.0;
-        for (int i = 0; i < n; ++i) {
-            const int pass = kl[i] / F, f = kl[i] % F;
-            const int c = pass == 0 ? 1 : (pass == 1 ? 2 : 0);
+        for_each_pass_corner(kl, n, [&](int f, int c) {
             const double *g = fgrad + (((int64_t)a * F + f) * 3 + c) * M::NG;
 #pragma unroll
             for (int q = 0; q < M::NG; ++q) s[q] += g[q];
-        }
+        });
         const float *m = mats + 12 * a;
         if constexpr (M::NG == 6) {
 #pragma unroll
@@ -883,7 +720,8 @@ struct MvWs {
     int32_t *nbig;
     float *part;                     // backward: per-slot partials
     double *fgrad;                   // backward: per (view, face, corner) gradients
-    AnWs an;                         // backward: per-vertex corner lists
+    int32_t *coff, *corners;         // backward: per-vertex corner lists (vertex_corners)
+    void *vc_ws;
 };
 
 // slots == false: the caller keeps them (icon_mesh_render_*'s state); bwd: the backward's buffers too
@@ -900,8 +738,9 @@ static size_t mv_carve(void *ws, int V, int F, int S, int A, int K, bool slots, 
     if (bwd) {
         w.part = c.take<float>(npix * K * NP);
         w.fgrad = c.take<double>((size_t)A * F * 3 * NG);
-        void *an = c.take<char>(an_carve(nullptr, V, F, nullptr));
-        if (ws) an_carve(an, V, F, &w.an);
+        w.coff = c.take<int32_t>((size_t)V + 1);
+        w.corners = c.take<int32_t>(3 * (size_t)F);
+        w.vc_ws = c.take<char>(vertex_corners_ws_bytes(V, F));
     }
     if (o) *o = w;
     return c.total();
@@ -940,8 +779,6 @@ static int mr_backward(const float *verts, const float *colors, int V, const int
     ICON_CUDA(cudaMemcpyAsync(w.mats, h_view_mats, sizeof(float) * 12 * (size_t)A, cudaMemcpyHostToDevice, stream));
     ICON_CUDA(cudaMemsetAsync(w.nbig, 0, sizeof(int32_t), stream));
     ICON_CUDA(cudaMemsetAsync(w.fgrad, 0, sizeof(double) * (size_t)A * F * 3 * M::NG, stream));
-    ICON_CUDA(cudaMemsetAsync(w.an.cnt, 0, sizeof(int32_t) * ((size_t)V + 1), stream));
-    ICON_CUDA(cudaMemsetAsync(w.an.cursor, 0, sizeof(int32_t) * (size_t)V, stream));
     k_mv_vertex<<<dim3((unsigned)((V + 255) / 256), (unsigned)A), 256, 0, stream>>>(verts, V, w.mats, w.vrec);
     ICON_LAUNCHED();
     const unsigned pb = (unsigned)((npix + 255) / 256);
@@ -957,86 +794,14 @@ static int mr_backward(const float *verts, const float *colors, int V, const int
     k_mr_face_big<M><<<MV_BIG_BLOCKS, 256, 0, stream>>>(faces, F, V, S, w.vrec, colors, slots, w.part, w.fgrad, w.big,
                                                          w.nbig);
     ICON_LAUNCHED();
-    const unsigned fb2 = (unsigned)((F + 255) / 256), vb = (unsigned)((V + 255) / 256);
-    k_an_count<<<fb2, 256, 0, stream>>>(faces, F, V, w.an.cnt);
-    ICON_LAUNCHED();
-    int rc = scan_exclusive_i32(w.an.cnt, w.an.off, (int64_t)V + 1, nullptr, w.an.scan_ws, stream);
-    if (rc) return rc;
-    k_an_fill<<<fb2, 256, 0, stream>>>(faces, F, V, w.an.off, w.an.cursor, w.an.keys);
-    ICON_LAUNCHED();
-    k_mr_vertex<M><<<vb, 256, 0, stream>>>(faces, F, V, A, w.mats, w.an.off, w.an.keys, w.fgrad, gverts, gcolors);
+    if (int rc = vertex_corners(faces, F, V, w.coff, w.corners, w.vc_ws, stream)) return rc;
+    k_mr_vertex<M><<<(unsigned)((V + 255) / 256), 256, 0, stream>>>(F, V, A, w.mats, w.coff, w.corners, w.fgrad,
+                                                                     gverts, gcolors);
     ICON_LAUNCHED();
     return ICON_OK;
 }
 
 }  // namespace icon
-
-extern "C" size_t icon_area_vertex_normals_workspace_bytes(int V, int F) {
-    if (V <= 0 || F <= 0) return 0;
-    return icon::an_carve(nullptr, V, F, nullptr);
-}
-
-extern "C" int icon_area_vertex_normals(const float *verts, int V, const int64_t *faces, int F, float *out, void *ws,
-                                        size_t ws_bytes, icon_stream_t stream_) {
-    using namespace icon;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(verts && faces && out && ws, "icon_area_vertex_normals: null pointer");
-    ICON_CHECK_ARG(V > 0 && F > 0 && F <= (INT32_MAX - 2) / 3, "icon_area_vertex_normals: bad sizes V=%d F=%d", V, F);
-    ICON_CHECK_ARG(ws_bytes >= icon_area_vertex_normals_workspace_bytes(V, F),
-                   "icon_area_vertex_normals: workspace too small");
-    AnWs w;
-    an_carve(ws, V, F, &w);
-    ICON_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int32_t) * ((size_t)V + 1), stream));
-    ICON_CUDA(cudaMemsetAsync(w.cursor, 0, sizeof(int32_t) * (size_t)V, stream));
-    const unsigned fb = (unsigned)((F + 255) / 256), vb = (unsigned)((V + 255) / 256);
-    k_an_count<<<fb, 256, 0, stream>>>(faces, F, V, w.cnt);
-    ICON_LAUNCHED();
-    int rc = scan_exclusive_i32(w.cnt, w.off, (int64_t)V + 1, nullptr, w.scan_ws, stream);
-    if (rc) return rc;
-    k_an_fill<<<fb, 256, 0, stream>>>(faces, F, V, w.off, w.cursor, w.keys);
-    ICON_LAUNCHED();
-    k_an_sum<<<vb, 256, 0, stream>>>(verts, faces, F, w.off, w.keys, V, out);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
-
-extern "C" size_t icon_area_vertex_normals_backward_workspace_bytes(int V, int F) {
-    if (V <= 0 || F <= 0) return 0;
-    icon::Carver c(nullptr);
-    c.take<char>(icon::an_carve(nullptr, V, F, nullptr));
-    c.take<double>(3 * (size_t)V);
-    return c.total();
-}
-
-extern "C" int icon_area_vertex_normals_backward(const float *verts, int V, const int64_t *faces, int F,
-                                                 const float *grad_normals, float *grad_verts, void *ws,
-                                                 size_t ws_bytes, icon_stream_t stream_) {
-    using namespace icon;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(verts && faces && grad_normals && grad_verts && ws, "icon_area_vertex_normals_backward: null pointer");
-    ICON_CHECK_ARG(V > 0 && F > 0 && F <= (INT32_MAX - 2) / 3, "icon_area_vertex_normals_backward: bad sizes V=%d F=%d",
-                   V, F);
-    ICON_CHECK_ARG(ws_bytes >= icon_area_vertex_normals_backward_workspace_bytes(V, F),
-                   "icon_area_vertex_normals_backward: workspace too small");
-    Carver c(ws);
-    AnWs w;
-    an_carve(c.take<char>(an_carve(nullptr, V, F, nullptr)), V, F, &w);
-    double *gs = c.take<double>(3 * (size_t)V);
-    ICON_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int32_t) * ((size_t)V + 1), stream));
-    ICON_CUDA(cudaMemsetAsync(w.cursor, 0, sizeof(int32_t) * (size_t)V, stream));
-    const unsigned fb = (unsigned)((F + 255) / 256), vb = (unsigned)((V + 255) / 256);
-    k_an_count<<<fb, 256, 0, stream>>>(faces, F, V, w.cnt);
-    ICON_LAUNCHED();
-    int rc = scan_exclusive_i32(w.cnt, w.off, (int64_t)V + 1, nullptr, w.scan_ws, stream);
-    if (rc) return rc;
-    k_an_fill<<<fb, 256, 0, stream>>>(faces, F, V, w.off, w.cursor, w.keys);
-    ICON_LAUNCHED();
-    k_an_grad_s<<<vb, 256, 0, stream>>>(verts, faces, F, w.off, w.keys, V, grad_normals, gs);
-    ICON_LAUNCHED();
-    k_an_grad_v<<<vb, 256, 0, stream>>>(verts, faces, F, w.off, w.keys, V, gs, grad_verts);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
 
 extern "C" size_t icon_mesh_views_workspace_bytes(int V, int F, int S, int A) {
     if (V <= 0 || F <= 0 || S <= 0 || A <= 0) return 0;

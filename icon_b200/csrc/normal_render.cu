@@ -6,13 +6,7 @@
 // restated operation for operation by oracle/normal_render.py, and the images are compared bit for bit (hence
 // -fmad=false for this file).
 //
-// Vertex normals (icon_vertex_normals), trimesh 3.9.35's angle-weighted rule, in fp64, rounded to fp32 at the end:
-//   unit(v) = v / |v| if |v| > 1e-13 (trimesh's tol.zero) else 0, |v| = sqrt((x x + y y) + z z);
-//   face normal n_f = unit((b - a) x (c - a)); corner angles a0 = acos(clamp(u.v)), a1 = acos(clamp((-u).w)),
-//   a2 = (pi - a0) - a1 with u = unit(b - a), v = unit(c - a), w = unit(c - b);
-//   vertex normal = unit(sum of a_k n_f over its corners, added in corner order 3 f + k).
-//   No float atomics: each vertex's corner list is sorted by corner id, so the sums are bitwise reproducible.
-//   Unreferenced vertices, degenerate faces and faces with an index outside [0, V) contribute / get zero.
+// The default vertex normals (trimesh's `vertex_normals`, icon_vertex_normals) are normals.cu's angle-weighted rule.
 //
 // Normal image (icon_normal_render), NormalRender(W, H) with ModelMat M (3x4 rows, fp32, passed on the host) and the
 // projection diag(1, 1, -1, 1) (orthographic), all fp32 in the order written:
@@ -42,105 +36,6 @@ constexpr unsigned long long NR_EMPTY = 0xffffffffffffffffull;
 constexpr float NR_RANGE = 65536.f;          // |x_w|, |y_w| limit of the exact fixed-point path (pixels)
 constexpr int NR_SMALL = 64;                 // faces whose pixel box has at most this many pixels: one thread each
 constexpr int NR_BIG_BLOCKS = 1024;          // grid of the cooperative pass (one block per listed face, grid-stride)
-constexpr double NR_TOL_ZERO = 1e-13;
-
-// ---------------------------------------------------------------- vertex normals
-
-__device__ __forceinline__ double3 d3_sub(double3 a, double3 b) { return make_double3(a.x - b.x, a.y - b.y, a.z - b.z); }
-__device__ __forceinline__ double d3_dot(double3 a, double3 b) { return (a.x * b.x + a.y * b.y) + a.z * b.z; }
-__device__ __forceinline__ double3 d3_unit(double3 v) {
-    const double n = sqrt(d3_dot(v, v));
-    if (!(n > NR_TOL_ZERO)) return make_double3(0.0, 0.0, 0.0);
-    return make_double3(v.x / n, v.y / n, v.z / n);
-}
-__device__ __forceinline__ double clamp_acos(double c) { return acos(fmin(fmax(c, -1.0), 1.0)); }
-
-__device__ __forceinline__ bool face_ok(const int64_t *faces, int f, int V, int64_t id[3]) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        id[k] = faces[3 * (int64_t)f + k];
-        if (id[k] < 0 || id[k] >= V) return false;
-    }
-    return true;
-}
-
-// per face: unit normal and the three corner angles (zero for a face with a bad index), and the corner counts
-__global__ void k_vn_face(const double *__restrict__ verts, const int64_t *__restrict__ faces, int F, int V,
-                          double *__restrict__ fdata, int32_t *__restrict__ cnt) {
-    const int f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= F) return;
-    int64_t id[3];
-    double *o = fdata + 6 * (int64_t)f;
-    if (!face_ok(faces, f, V, id)) {
-        for (int k = 0; k < 6; ++k) o[k] = 0.0;
-        return;
-    }
-    double3 p[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        p[k] = make_double3(verts[3 * id[k]], verts[3 * id[k] + 1], verts[3 * id[k] + 2]);
-        atomicAdd(&cnt[id[k]], 1);
-    }
-    const double3 e1 = d3_sub(p[1], p[0]), e2 = d3_sub(p[2], p[0]);
-    const double3 n = d3_unit(make_double3(e1.y * e2.z - e1.z * e2.y, e1.z * e2.x - e1.x * e2.z,
-                                           e1.x * e2.y - e1.y * e2.x));
-    const double3 u = d3_unit(e1), v = d3_unit(e2), w = d3_unit(d3_sub(p[2], p[1]));
-    const double a0 = clamp_acos(d3_dot(u, v));
-    const double a1 = clamp_acos(d3_dot(make_double3(-u.x, -u.y, -u.z), w));
-    o[0] = n.x; o[1] = n.y; o[2] = n.z;
-    o[3] = a0; o[4] = a1; o[5] = (3.141592653589793 - a0) - a1;
-}
-
-// corner ids into their vertex's slots (in arrival order; k_vn_sum sorts each list)
-__global__ void k_vn_fill(const int64_t *__restrict__ faces, int F, int V, const int32_t *__restrict__ off,
-                          int32_t *__restrict__ cursor, int32_t *__restrict__ corners) {
-    const int f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= F) return;
-    int64_t id[3];
-    if (!face_ok(faces, f, V, id)) return;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) corners[off[id[k]] + atomicAdd(&cursor[id[k]], 1)] = 3 * f + k;
-}
-
-// per vertex: sort its corner list (heapsort: O(n log n) whatever the valence), sum a_k n_f in corner order, unit
-__global__ void k_vn_sum(const int32_t *__restrict__ off, int32_t *__restrict__ corners,
-                         const double *__restrict__ fdata, int V, float *__restrict__ out) {
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    int32_t *a = corners + off[v];
-    const int n = off[v + 1] - off[v];
-    heap_sort_i32(a, n);
-    double3 s = make_double3(0.0, 0.0, 0.0);
-    for (int i = 0; i < n; ++i) {
-        const int c = a[i];
-        const double *fd = fdata + 6 * (int64_t)(c / 3);
-        const double w = fd[3 + c % 3];
-        s.x = s.x + w * fd[0]; s.y = s.y + w * fd[1]; s.z = s.z + w * fd[2];
-    }
-    s = d3_unit(s);
-    out[3 * (int64_t)v] = (float)s.x; out[3 * (int64_t)v + 1] = (float)s.y; out[3 * (int64_t)v + 2] = (float)s.z;
-}
-
-struct VnWs {
-    int32_t *cnt, *off, *cursor, *corners;
-    double *fdata;
-    void *scan_ws;
-};
-
-static size_t vn_carve(void *ws, int V, int F, VnWs *o) {
-    Carver c(ws);
-    VnWs w;
-    w.cnt = c.take<int32_t>((size_t)V + 1);
-    w.off = c.take<int32_t>((size_t)V + 1);
-    w.cursor = c.take<int32_t>((size_t)V);
-    w.corners = c.take<int32_t>(3 * (size_t)F);
-    w.fdata = c.take<double>(6 * (size_t)F);
-    w.scan_ws = c.take<char>(scan_ws_bytes((int64_t)V + 1));
-    if (o) *o = w;
-    return c.total();
-}
-
-// ---------------------------------------------------------------- normal image
 
 struct NrModel {
     float m[12];
@@ -175,8 +70,8 @@ struct NrTri {
 
 __device__ __forceinline__ bool tri_setup(const int64_t *__restrict__ faces, const int4 *__restrict__ vrec, int f,
                                           int V, int W, int H, NrTri &t, float zw[3]) {
-    int64_t id[3];
-    if (!face_ok(faces, f, V, id)) return false;
+    int id[3];
+    if (!face_ids(faces, f, V, id)) return false;
     int4 r[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -326,34 +221,6 @@ static size_t nr_carve(void *ws, int V, int F, int W, int H, NrWs *o) {
 }
 
 }  // namespace icon
-
-extern "C" size_t icon_vertex_normals_workspace_bytes(int V, int F) {
-    if (V <= 0 || F <= 0) return 0;
-    return icon::vn_carve(nullptr, V, F, nullptr);
-}
-
-extern "C" int icon_vertex_normals(const double *verts, int V, const int64_t *faces, int F, float *out, void *ws,
-                                   size_t ws_bytes, icon_stream_t stream_) {
-    using namespace icon;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    ICON_CHECK_ARG(verts && faces && out && ws, "icon_vertex_normals: null pointer");
-    ICON_CHECK_ARG(V > 0 && F > 0 && F <= (INT32_MAX - 2) / 3, "icon_vertex_normals: bad sizes V=%d F=%d", V, F);
-    ICON_CHECK_ARG(ws_bytes >= icon_vertex_normals_workspace_bytes(V, F), "icon_vertex_normals: workspace too small");
-    VnWs w;
-    vn_carve(ws, V, F, &w);
-    ICON_CUDA(cudaMemsetAsync(w.cnt, 0, sizeof(int32_t) * ((size_t)V + 1), stream));
-    ICON_CUDA(cudaMemsetAsync(w.cursor, 0, sizeof(int32_t) * (size_t)V, stream));
-    const unsigned fb = (unsigned)((F + 255) / 256), vb = (unsigned)((V + 255) / 256);
-    k_vn_face<<<fb, 256, 0, stream>>>(verts, faces, F, V, w.fdata, w.cnt);
-    ICON_LAUNCHED();
-    int rc = scan_exclusive_i32(w.cnt, w.off, (int64_t)V + 1, nullptr, w.scan_ws, stream);
-    if (rc) return rc;
-    k_vn_fill<<<fb, 256, 0, stream>>>(faces, F, V, w.off, w.cursor, w.corners);
-    ICON_LAUNCHED();
-    k_vn_sum<<<vb, 256, 0, stream>>>(w.off, w.corners, w.fdata, V, out);
-    ICON_LAUNCHED();
-    return ICON_OK;
-}
 
 extern "C" size_t icon_normal_render_workspace_bytes(int V, int F, int width, int height) {
     if (V <= 0 || F <= 0 || width <= 0 || height <= 0) return 0;

@@ -1,5 +1,5 @@
-// SMPL body preparation: vertex normals, per-face records, Morton-ordered implicit AABB tree and
-// the yz ray grid.  Compiled with -fmad=false.
+// SMPL body preparation: vertex normals (normals.cu's area-weighted rule), per-face records, Morton-ordered implicit
+// AABB tree and the yz ray grid.  Compiled with -fmad=false.
 //
 // Replaces the per-query preamble of cal_sdf_batch (lib/dataset/mesh_util.py:367-372):
 //   normals = Meshes(verts, faces).verts_normals_padded()          (pytorch3d)
@@ -41,6 +41,7 @@ static MeshView carve_mesh(Carver &c, int V, int F) {
     m.boff = c.take<int32_t>(NBRICK + 1);
     m.brick_cap = brick_list_cap(F);
     m.blist = c.take<unsigned short>((size_t)m.brick_cap);
+    m.vn_ws = c.take<char>(area_vertex_normals_ws_bytes(V, F));
     m.vnormals = c.take<float>((size_t)V * 3);      // last: tests read it from the tail
     return m;
 }
@@ -54,45 +55,6 @@ size_t mesh_ws_bytes(int V, int F) {
 MeshView mesh_view(const void *ws, int V, int F) {
     Carver c((void *)ws);
     return carve_mesh(c, V, F);
-}
-
-// pytorch3d verts_normals_packed: three sequential index_add passes (corner 1, 2, 0), each in
-// face order, then normalize(eps=1e-6).  One thread per vertex walks the face list in that
-// exact order, so the fp32 sum is bit-identical to the sequential CPU evaluation
-// (oracle_vertex_normals) -- no atomics, deterministic.  Faces are staged through shared memory.
-__global__ void __launch_bounds__(128) k_vertex_normals(const float *__restrict__ verts,
-                                                        const int64_t *__restrict__ faces, int V, int F,
-                                                        float *__restrict__ out) {
-    __shared__ int s_faces[3 * 512];
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    float sx = 0.f, sy = 0.f, sz = 0.f;
-    for (int pass = 0; pass < 3; ++pass) {
-        const int corner = (pass == 0) ? 1 : (pass == 1 ? 2 : 0);
-        const int c1 = (corner + 1) % 3, c2 = (corner + 2) % 3;
-        for (int f0 = 0; f0 < F; f0 += 512) {
-            const int nf = min(512, F - f0);
-            __syncthreads();
-            for (int k = threadIdx.x; k < 3 * nf; k += blockDim.x) s_faces[k] = (int)faces[3 * (size_t)f0 + k];
-            __syncthreads();
-            if (v < V) {
-                for (int k = 0; k < nf; ++k) {
-                    if (s_faces[3 * k + corner] != v) continue;
-                    const int i1 = s_faces[3 * k + c1], i2 = s_faces[3 * k + c2];
-                    V3 p0 = mk3(verts[3 * v], verts[3 * v + 1], verts[3 * v + 2]);
-                    V3 p1 = mk3(verts[3 * i1], verts[3 * i1 + 1], verts[3 * i1 + 2]);
-                    V3 p2 = mk3(verts[3 * i2], verts[3 * i2 + 1], verts[3 * i2 + 2]);
-                    V3 n = cross3(sub3(p1, p0), sub3(p2, p0));
-                    sx += n.x; sy += n.y; sz += n.z;
-                }
-            }
-        }
-    }
-    if (v >= V) return;
-    float nrm = sqrtf(sx * sx + sy * sy + sz * sz);
-    if (nrm < 1e-6f) nrm = 1e-6f;
-    out[3 * v] = sx / nrm;
-    out[3 * v + 1] = sy / nrm;
-    out[3 * v + 2] = sz / nrm;
 }
 
 __global__ void k_face_records(const float *__restrict__ verts, const int64_t *__restrict__ faces,
@@ -231,8 +193,8 @@ extern "C" int icon_smpl_prepare(const float *verts, const int64_t *faces, const
     MeshView m = carve_mesh(c, V, F);
     bricks_forget(m);
     void *scan_ws = m.scan_ws;
-    k_vertex_normals<<<(V + 127) / 128, 128, 0, stream>>>(verts, faces, V, F, m.vnormals);
-    ICON_LAUNCHED();
+    int rc = area_vertex_normals(verts, V, faces, F, m.vnormals, m.vn_ws, stream);
+    if (rc) return rc;
     k_face_records<<<(F + 127) / 128, 128, 0, stream>>>(verts, faces, m.vnormals, cmap, vis, F, (float4 *)m.tri,
                                                         (float4 *)m.sph, (float4 *)m.attr, (float4 *)m.rbox, m.keys);
     ICON_LAUNCHED();
@@ -245,7 +207,7 @@ extern "C" int icon_smpl_prepare(const float *verts, const int64_t *faces, const
     ICON_CUDA(cudaMemsetAsync(m.rcount, 0, sizeof(int32_t) * (RAY_GRID * RAY_GRID + 1), stream));
     k_ray_count<<<(F + 127) / 128, 128, 0, stream>>>(m);
     ICON_LAUNCHED();
-    int rc = scan_exclusive_i32(m.rcount, m.roff, RAY_GRID * RAY_GRID + 1, nullptr, scan_ws, stream);
+    rc = scan_exclusive_i32(m.rcount, m.roff, RAY_GRID * RAY_GRID + 1, nullptr, scan_ws, stream);
     if (rc) return rc;
     ICON_CUDA(cudaMemsetAsync(m.rcount, 0, sizeof(int32_t) * (RAY_GRID * RAY_GRID + 1), stream));   // reuse as cursor
     k_ray_fill<<<(F + 127) / 128, 128, 0, stream>>>(m, m.rcount);

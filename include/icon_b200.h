@@ -254,7 +254,8 @@ int icon_visibility(const float *xyz, int V, const int64_t *faces, int F, int im
 
 /* ------------------------------------------------------------------ normal images of the evaluation
  * Replace the OpenGL NormalRender behind Evaluator._render_normal (lib/dataset/Evaluator.py:58-73) and trimesh's
- * vertex_normals it draws by default.  Rules (parity unpinned): csrc/normal_render.cu header.
+ * vertex_normals it draws by default.  Rules (parity unpinned): csrc/normal_render.cu header (the vertex normals:
+ * csrc/normals.cu header).
  *
  * icon_vertex_normals: trimesh's angle-weighted vertex normals of verts [V,3] f64, faces [F,3] i64, computed in fp64
  * and written as out [V,3] f32; bitwise reproducible (no float atomics).  Unreferenced vertices get zero. */
@@ -273,7 +274,7 @@ int icon_normal_render(const float *verts, const float *norms, int V, const int6
 /* ------------------------------------------------------------------ self-rotation video of the demo
  * Replace the pytorch3d renders of Render.get_rendered_video (lib/common/render.py:327-374; MeshRasterizer +
  * cleanShader at get_camera / init_renderer(camera, "clean_mesh", "gray")) and the colours VF2Mesh gives a mesh.
- * Rules (parity unpinned): csrc/mesh_views.cu header.
+ * Rules (parity unpinned): csrc/mesh_views.cu header (the vertex normals: csrc/normals.cu header).
  *
  * icon_area_vertex_normals: pytorch3d's verts_normals_packed of verts [V,3] f32, faces [F,3] i64 -> out [V,3] f32;
  * bitwise reproducible (no float atomics). */
@@ -281,7 +282,7 @@ size_t icon_area_vertex_normals_workspace_bytes(int V, int F);
 int icon_area_vertex_normals(const float *verts, int V, const int64_t *faces, int F, float *out, void *ws,
                              size_t ws_bytes, icon_stream_t stream);
 /* icon_area_vertex_normals_backward: grad_normals [V,3] f32 (the upstream gradient of out) -> grad_verts [V,3] f32,
- * overwritten; fp64 sums in the forward's sorted incidence order, bitwise reproducible.  ws:
+ * overwritten; fp64 sums in the forward's (pass, face) order, bitwise reproducible.  ws:
  * icon_area_vertex_normals_backward_workspace_bytes(V, F) bytes. */
 size_t icon_area_vertex_normals_backward_workspace_bytes(int V, int F);
 int icon_area_vertex_normals_backward(const float *verts, int V, const int64_t *faces, int F,

@@ -1,4 +1,5 @@
-"""CPU restatement of icon_mesh_views / icon_area_vertex_normals (csrc/mesh_views.cu) -- TEST INFRASTRUCTURE ONLY.
+"""CPU restatement of icon_mesh_views (csrc/mesh_views.cu) / icon_area_vertex_normals (csrc/normals.cu) -- TEST
+INFRASTRUCTURE ONLY.
 
 PARITY UNPINNED.  The reference renders Render.get_rendered_video's frames (lib/common/render.py:327-374) with
 pytorch3d's MeshRasterizer and cleanShader (softmax_rgb_blend), which are not installable here.  The rules are the

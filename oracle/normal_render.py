@@ -2,7 +2,8 @@
 
 PARITY UNPINNED.  The reference draws with lib.renderer.gl.normal_render.NormalRender (OpenGL, RGBA32F, no MSAA,
 depth test GL_LESS, no culling, orthographic "view" diag(1, 1, -1, 1)) and, by default, trimesh 3.9.35's
-`vertex_normals`; neither is a dependency of this project.  The rules are the ones written in csrc/normal_render.cu's header:
+`vertex_normals`; neither is a dependency of this project.  The rules are the ones written in the headers of
+csrc/normal_render.cu and csrc/normals.cu:
 
 * vertex normals: trimesh's angle-weighted rule in fp64 (face unit normal times corner angle, summed per vertex in
   corner order 3 f + k, then unit length; |v| <= 1e-13 counts as zero);

@@ -221,13 +221,16 @@ def test_no_state_without_grad():
     ct = MV.vertex_colors(vt, ft)
     mats = _mats(MV)[[0, 2]]
     vt.requires_grad_(True)
+    # bytes the live tensors requested: the allocated-block count also holds whatever remainder of a cached block
+    # the allocator did not split off, which depends on the earlier tests' allocations
+    requested = lambda: torch.cuda.memory_stats()["requested_bytes.all.current"]   # noqa: E731
     torch.cuda.synchronize()
-    base = torch.cuda.memory_allocated()
+    base = requested()
     with torch.no_grad():
         out = MV.normal_image(vt, ft, ct, mats, 512)
         sil = MV.silhouette_image(vt, ft, mats, 512)
     torch.cuda.synchronize()
-    assert torch.cuda.memory_allocated() - base == out.numel() * 4 + sil.numel() * 4
+    assert requested() - base == out.numel() * 4 + sil.numel() * 4
     assert out.grad_fn is None and sil.grad_fn is None
     plain = MV.normal_image(vt.detach(), ft, ct, mats, 512)              # no input requires grad
     assert plain.grad_fn is None and torch.equal(plain, out)
