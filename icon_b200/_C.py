@@ -44,6 +44,9 @@ _SIGS = {
     "icon_mesh_distance": (_i, [_vp, _i64, _vp, _i, _i, _vp, _vp, _vp]),
     "icon_mesh_sample_workspace_bytes": (_sz, [_i]),
     "icon_mesh_sample": (_i, [_vp, _vp, _i, _i, _vp, _i, ctypes.c_uint64, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "icon_prt_workspace_bytes": (_sz, [_i, _i, _i]),
+    "icon_prt": (_i, [_vp, _i, _i, _vp, _vp, _i, ctypes.c_double, _vp, _vp, _i, _i, ctypes.c_double, _vp, _vp, _vp, _sz,
+                      _vp]),
     "icon_mlp_only": (_i, [_vp, _i, _i64, _vp, _vp, _vp, _vp]),
     "icon_display": (_i, [_vp, _i, _vp, _vp]),
     "icon_grid_upsample": (_i, [_vp, _vp, _i, _f, _vp, _vp, _vp, _vp]),

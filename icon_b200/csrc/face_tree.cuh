@@ -124,6 +124,10 @@ __device__ __forceinline__ void write_parent_box(const FaceTree &t, int l, int n
     t.nodes[2 * ((size_t)t.lvl_off[l] + n) + 1] = hi;
 }
 
+// the tree of a workspace icon_mesh_prepare filled, and the device address of the mesh's largest |coordinate|
+// (defined in mesh_dist.cu; the PRT ray walk of prt.cu reads the same tree)
+FaceTree mesh_ws_tree(const void *mesh_ws, int V, int F, const float **absmax);
+
 // ---------------------------------------------------------------- the walk
 struct ChunkSmem {                     // phase C's staging area, one per warp
     float4 sph[32];                    // bounding spheres of the surviving faces of the current chunk (compacted)

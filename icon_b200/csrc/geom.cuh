@@ -106,4 +106,26 @@ __device__ __forceinline__ int ray_hit_px(V3 p, V3 a, V3 e1, V3 e2) {
     return t > 0.f ? 1 : 0;
 }
 
+// Ray o + t d (t > 0) against triangle (a, a + e1, a + e2): Moller-Trumbore without the division, the any-hit test of
+// the PRT transfer (prt.cu).  With det = e1.(d x e2), u' = s.(d x e2), v' = d.(s x e1), t' = e2.(s x e1), s = o - a,
+// each taken times sign(det) (exact), the convention is:
+//   * edges and vertices count as hits: u' >= 0, v' >= 0, u' + v' <= |det|  (u = u' / det, v = v' / det);
+//   * the hit must lie strictly ahead of the origin: t' > 0;
+//   * det == 0 (the ray parallel to the face's plane, or a zero-area face) is a miss, and so is a NaN anywhere
+//     (every comparison is written so that NaN fails it).
+// Mirrored face by face by any_hit_block() of oracle/prt_oracle.c.
+__device__ __forceinline__ bool ray_hit_tri(V3 o, V3 d, V3 a, V3 e1, V3 e2) {
+    const V3 p = cross3(d, e2);
+    const float det = dot3(e1, p);
+    if (det == 0.f) return false;
+    const float sg = det > 0.f ? 1.f : -1.f, ad = fabsf(det);
+    const V3 s = sub3(o, a);
+    const float u = dot3(s, p) * sg;
+    if (!(u >= 0.f && u <= ad)) return false;
+    const V3 q = cross3(s, e1);
+    const float v = dot3(d, q) * sg;
+    if (!(v >= 0.f && u + v <= ad)) return false;
+    return dot3(e2, q) * sg > 0.f;
+}
+
 }  // namespace icon

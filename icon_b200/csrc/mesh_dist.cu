@@ -263,6 +263,13 @@ static int scan64_inclusive(unsigned long long *x, int64_t n, unsigned long long
 
 __global__ void k_gm_total(GMesh m) { m.hdr->total = m.wcum[m.F - 1]; }
 
+FaceTree mesh_ws_tree(const void *mesh_ws, int V, int F, const float **absmax) {
+    Carver c((void *)mesh_ws);
+    GMesh m = carve_gmesh(c, V, F);
+    *absmax = &m.hdr->absmax;
+    return m;
+}
+
 // ---------------------------------------------------------------- nearest face, one point per warp
 using MeshDistSmem = WalkSmem<int32_t, GM_FR_CAP>;
 

@@ -7,7 +7,8 @@
 The reference's `lib` package stays the reference's: every module, helper and constant that is not part of the
 accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.dataset.Evaluator` but for
 `calculate_chamfer_p2s`, `init_gl` and `_render_normal`, `lib.smplx` but for the `lbs` its body models call,
-`lib.pixielib` but for `SMPLX.forward` in `lib/pixielib/models/SMPLX.py`, `lib.common.config`, the rest of
+`lib.pixielib` but for `SMPLX.forward` in `lib/pixielib/models/SMPLX.py`, `lib.renderer` but for `computePRT`,
+`lib.common.config`, the rest of
 `train_util` / `mesh_util` / `net_util` ...) is imported from the checkout unchanged.  An import hook on
 `sys.meta_path` then does two things, only for the modules listed below:
 
@@ -22,7 +23,8 @@ accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.
               `lib/dataset/Evaluator.py`, `Render.get_rendered_video` in `lib/common/render.py`, and in
               `lib/dataset/TestDataset.py` an `__init__` that rebinds `get_rgb_image` / `get_silhouette_image` /
               `VF2Mesh` on the instance's `self.render` only, `lbs` in `lib/smplx/body_models.py`, `SMPLX` in
-              `lib/pixielib/models/SMPLX.py`: the same class, its `forward` patched to run on the kernels), so
+              `lib/pixielib/models/SMPLX.py`: the same class, its `forward` patched to run on the kernels,
+              `computePRT` in `lib/renderer/prt_util.py`), so
               `from lib.common.train_util import *` (apps/ICON.py:20) still finds everything else it uses.
 
 Callers and call sites this serves: apps/ICON.py:17-22, 52-90 (HGPIFuNet, Seg3dLossless, query_func, get_visibility),
@@ -40,7 +42,9 @@ vertex colours),
 apps/infer.py:548-562 (`-export_video`: get_rendered_video's 360 views per mesh, a chunk of views per kernel call),
 lib/dataset/mesh_util.py:187-237 (load_checkpoint:
 identical state_dict keys),
-lib/dataset/TestDataset.py:137 (get_visibility).
+lib/dataset/TestDataset.py:137 (get_visibility),
+scripts/render_single.py:118 (computePRT of the dataset preparation: the rays cast on the kernels, the same
+prt/bounce.npy and prt/face.npy written).
 """
 import importlib.abc
 import importlib.machinery
@@ -65,7 +69,7 @@ def _replacements():
 
 
 def _patches():
-    from . import body_model, encoders, mesh, mesh_priors, mesh_views, metrics, net, remesh, visibility, voxelize
+    from . import body_model, encoders, mesh, mesh_priors, mesh_views, metrics, net, prt, remesh, visibility, voxelize
 
     def make_define_G(reference_define_G):
         import torch.nn as nn
@@ -99,6 +103,7 @@ def _patches():
         "lib.dataset.TestDataset": {"TestDataset": mesh_views.make_TestDataset},  # self.render's fit renders, VF2Mesh
         "lib.smplx.body_models": {"lbs": body_model.make_lbs},              # SMPL / SMPLH / SMPLX.forward's skinning
         "lib.pixielib.models.SMPLX": {"SMPLX": body_model.make_pixie_SMPLX},  # PIXIE's SMPL-X: skinning and heads
+        "lib.renderer.prt_util": {"computePRT": prt.make_computePRT},       # the dataset renderer's PRT transfer
     }
 
 

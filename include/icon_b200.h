@@ -175,6 +175,19 @@ size_t icon_mesh_sample_workspace_bytes(int count);
 int icon_mesh_sample(const float *verts, const int64_t *faces, int V, int F, const void *mesh_ws, int count,
                      uint64_t seed, float *out_points, int32_t *out_face, int32_t *out_count, void *ws,
                      size_t ws_bytes, icon_stream_t stream);
+/* Precomputed radiance transfer (lib/renderer/prt_util.py:115-182, computePRT) over a workspace icon_mesh_prepare
+ * filled for the mesh (Vm vertices, F faces).  For the V ray origins origins [V,3] f64 with unit normals normals [V,3]
+ * f64 and the D directions dirs [D,3] f64 with their K real SH values sh [D,K] f64:
+ *   prt_out[v,k] = w * sum_d (d.n_v > 0) (1 - hit) (d.n_v) sh[d,k]        [V,K] f64,
+ * hit = any face met by the ray fp32(o_v + delta n_v) + t fp32(d), t > 0 (Moller-Trumbore, convention in geom.cuh).
+ * The sum runs over blocks of n directions when D = n^2 (one block otherwise), in order.  hit_bits [V, ceil(D/32)]
+ * u32 (may be NULL): bit d % 32 of word d / 32 is ray d's verdict; when given, every ray is cast, else only the
+ * front-facing ones.  ws: at least ceil(D/32) * 4 bytes; vertices go in chunks of as many rows as it holds
+ * (icon_prt_workspace_bytes: up to 65536).  The results do not depend on the chunking. */
+size_t icon_prt_workspace_bytes(int V, int D, int K);
+int icon_prt(const void *mesh_ws, int Vm, int F, const double *origins, const double *normals, int V, double delta,
+             const double *dirs, const double *sh, int D, int K, double w, double *prt_out, uint32_t *hit_bits,
+             void *ws, size_t ws_bytes, icon_stream_t stream);
 
 /* MLP alone on a ready [c0,N] feature matrix (parity tap for lib/net/MLP.py:49-72). */
 int icon_mlp_only(const float *feature, int c0, int64_t N, const float *mlp_packed,
