@@ -80,6 +80,10 @@ _SIGS = {
     "icon_vertex_normals": (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "icon_normal_render_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "icon_normal_render": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "icon_dataset_render_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "icon_dataset_render": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "icon_dataset_texture_bytes": (_sz, [_i, _i]),
+    "icon_dataset_texture": (_i, [_vp, _i, _i, _vp, _sz, _vp]),
     "icon_area_vertex_normals_workspace_bytes": (_sz, [_i, _i]),
     "icon_area_vertex_normals": (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     "icon_area_vertex_normals_backward_workspace_bytes": (_sz, [_i, _i]),
@@ -162,6 +166,13 @@ class TetraModel(ctypes.Structure):
     _fields_ = [("V", _i), ("N", _i), ("T", _i), ("nnz", _i), ("parents", _i * 24), ("v_template", _vp),
                 ("shapedirs", _vp), ("posedirs", _vp), ("weights", _vp), ("jr_off", _vp), ("jr_col", _vp),
                 ("jr_val", _vp)]
+
+
+class DatasetMesh(ctypes.Structure):
+    """icon_dr_mesh (include/icon_b200.h): one mesh of the dataset renderer, device arrays indexed per face corner."""
+    _fields_ = [("mode", _i), ("F", _i), ("V", _i), ("Vn", _i), ("Vt", _i), ("Va", _i), ("pos", _vp), ("nrm", _vp),
+                ("uv", _vp), ("attr", _vp), ("f_pos", _vp), ("f_nrm", _vp), ("f_uv", _vp), ("f_attr", _vp),
+                ("tex", _vp), ("tex_w", _i), ("tex_h", _i)]
 
 
 class IconError(RuntimeError):

@@ -28,12 +28,12 @@
 //   n.y n.y) + n.z n.z); rgb = (n / r + 1) 0.5, alpha 1.  A zero interpolated normal (r == 0, which GLSL's normalize
 //   leaves undefined) is written as rgb (0.5, 0.5, 0.5).
 //   Output [H, W, 4] f32 in get_color's order: image row r is window row H - 1 - r; background (1, 1, 1, 0).
-#include "common.cuh"
+#include "raster.cuh"
 
 namespace icon {
 
-constexpr unsigned long long NR_EMPTY = 0xffffffffffffffffull;
-constexpr float NR_RANGE = 65536.f;          // |x_w|, |y_w| limit of the exact fixed-point path (pixels)
+constexpr unsigned long long NR_EMPTY = RS_EMPTY;
+constexpr float NR_RANGE = RS_RANGE;
 constexpr int NR_SMALL = 64;                 // faces whose pixel box has at most this many pixels: one thread each
 constexpr int NR_BIG_BLOCKS = 1024;          // grid of the cooperative pass (one block per listed face, grid-stride)
 
@@ -60,14 +60,9 @@ __global__ void k_nr_vertex(const float *__restrict__ verts, const float *__rest
     nrot[i] = make_float4(row3(M.m, nx, ny, nz), row3(M.m + 4, nx, ny, nz), row3(M.m + 8, nx, ny, nz), 0.f);
 }
 
-// one face, set up for coverage: internal corner order (0, 1, 2) or (0, 2, 1) so that the face is counter-clockwise
-struct NrTri {
-    int X[3], Y[3];      // internal order
-    long long area;      // > 0
-    bool swapped;
-    int bx0, bx1, by0, by1;   // pixel box clamped to the viewport (empty when bx0 > bx1 or by0 > by1)
-};
+typedef RsTri NrTri;
 
+// face f's records (one sample per pixel, at its centre)
 __device__ __forceinline__ bool tri_setup(const int64_t *__restrict__ faces, const int4 *__restrict__ vrec, int f,
                                           int V, int W, int H, NrTri &t, float zw[3]) {
     int id[3];
@@ -76,45 +71,13 @@ __device__ __forceinline__ bool tri_setup(const int64_t *__restrict__ faces, con
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         r[k] = vrec[id[k]];
-        if (!r[k].w) return false;
         zw[k] = __int_as_float(r[k].z);
     }
-    long long area = (long long)(r[1].x - r[0].x) * (r[2].y - r[0].y) - (long long)(r[1].y - r[0].y) * (r[2].x - r[0].x);
-    if (area == 0) return false;
-    t.swapped = area < 0;
-    t.area = t.swapped ? -area : area;
-    const int4 ra = t.swapped ? r[2] : r[1], rb = t.swapped ? r[1] : r[2];
-    t.X[0] = r[0].x; t.Y[0] = r[0].y; t.X[1] = ra.x; t.Y[1] = ra.y; t.X[2] = rb.x; t.Y[2] = rb.y;
-    const int xmin = min(min(t.X[0], t.X[1]), t.X[2]), xmax = max(max(t.X[0], t.X[1]), t.X[2]);
-    const int ymin = min(min(t.Y[0], t.Y[1]), t.Y[2]), ymax = max(max(t.Y[0], t.Y[1]), t.Y[2]);
-    // pixels whose centre 256 p + 128 lies in [min, max]; >> is a floor division
-    t.bx0 = max(-((128 - xmin) >> 8), 0); t.bx1 = min((xmax - 128) >> 8, W - 1);
-    t.by0 = max(-((128 - ymin) >> 8), 0); t.by1 = min((ymax - 128) >> 8, H - 1);
-    return t.bx0 <= t.bx1 && t.by0 <= t.by1;
+    return rs_setup(r, W, H, 128, 128, t);
 }
 
-// edge functions at pixel (px, py), indexed by ORIGINAL corner; false when the pixel is not covered
 __device__ __forceinline__ bool tri_cover(const NrTri &t, int px, int py, long long e[3]) {
-    const int Px = px * 256 + 128, Py = py * 256 + 128;
-    long long ei[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const int a = (k + 1) % 3, b = (k + 2) % 3;
-        const int dx = t.X[b] - t.X[a], dy = t.Y[b] - t.Y[a];
-        ei[k] = (long long)dx * (Py - t.Y[a]) - (long long)dy * (Px - t.X[a]);
-        const bool top_left = dy < 0 || (dy == 0 && dx < 0);
-        if (ei[k] < 0 || (ei[k] == 0 && !top_left)) return false;
-    }
-    e[0] = ei[0];
-    e[1] = t.swapped ? ei[2] : ei[1];
-    e[2] = t.swapped ? ei[1] : ei[2];
-    return true;
-}
-
-__device__ __forceinline__ void tri_weights(const NrTri &t, const long long e[3], float l[3]) {
-    const float fa = __ll2float_rn(t.area);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) l[k] = __ll2float_rn(e[k]) / fa;
+    return rs_cover(t, px * 256 + 128, py * 256 + 128, e);
 }
 
 __device__ __forceinline__ void tri_fragment(const NrTri &t, const float zw[3], int f, int px, int py, int W,
@@ -122,12 +85,10 @@ __device__ __forceinline__ void tri_fragment(const NrTri &t, const float zw[3], 
     long long e[3];
     if (!tri_cover(t, px, py, e)) return;
     float l[3];
-    tri_weights(t, e, l);
+    rs_weights(t, e, l);
     const float z = (l[0] * zw[0] + l[1] * zw[1]) + l[2] * zw[2];
-    if (!(z >= 0.f && z <= 1.f)) return;
-    const unsigned q = (unsigned)rintf(z * 16777215.f);
-    if (q >= 16777215u) return;                  // GL_LESS against the cleared depth 1.0
-    atomicMin(&zbuf[(size_t)py * W + px], ((unsigned long long)q << 32) | (unsigned)f);
+    unsigned long long key;
+    if (rs_depth_key(z, f, key)) atomicMin(&zbuf[(size_t)py * W + px], key);
 }
 
 // one thread per face: small faces rasterise here, faces with a larger pixel box go to the cooperative list
@@ -183,7 +144,7 @@ __global__ void k_nr_shade(const unsigned long long *__restrict__ zbuf, const in
         tri_setup(faces, vrec, f, V, W, H, t, zw);                 // succeeded in the raster pass
         tri_cover(t, px, py, e);
         float l[3];
-        tri_weights(t, e, l);
+        rs_weights(t, e, l);
         float4 nk[3];
 #pragma unroll
         for (int k = 0; k < 3; ++k) nk[k] = nrot[faces[3 * (int64_t)f + k]];

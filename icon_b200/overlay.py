@@ -7,7 +7,8 @@
 The reference's `lib` package stays the reference's: every module, helper and constant that is not part of the
 accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.dataset.Evaluator` but for
 `calculate_chamfer_p2s`, `init_gl` and `_render_normal`, `lib.smplx` but for the `lbs` its body models call,
-`lib.pixielib` but for `SMPLX.forward` in `lib/pixielib/models/SMPLX.py`, `lib.renderer` but for `computePRT`,
+`lib.pixielib` but for `SMPLX.forward` in `lib/pixielib/models/SMPLX.py`, `lib.renderer` but for `computePRT` and the
+GL renderers `PRTRender` / `ColorRender` / `initialize_GL_context`,
 `lib.common.config`, the rest of
 `train_util` / `mesh_util` / `net_util` ...) is imported from the checkout unchanged.  An import hook on
 `sys.meta_path` then does two things, only for the modules listed below:
@@ -15,7 +16,8 @@ accelerated path (`lib.common.render` but for `Render.get_rendered_video`, `lib.
 * REPLACE  -- the module is never executed; a synthetic module exporting the icon_b200 classes takes its place.
               Used where the reference file exists only to reach third-party CUDA wheels
               (`lib/net/HGPIFuNet.py` -> kaolin / pytorch3d / voxelize_cuda, `lib/net/voxelize.py` -> voxelize_cuda,
-              `lib/common/seg3d_lossless.py` -> kaolin marching cubes / PyMCubes).
+              `lib/common/seg3d_lossless.py` -> kaolin marching cubes / PyMCubes), or only to reach OpenGL
+              (`lib/renderer/gl/prt_render.py`, `color_render.py`, `init_gl.py` -> PyOpenGL and an EGL context).
 * PATCH    -- the reference module is executed normally, then the accelerated names are rebound in its namespace
               (`query_func` in `lib/common/train_util.py`, `get_visibility` and `remesh` in `lib/dataset/mesh_util.py`, the
               encoder classes in `lib/net/{NormalNet,MLP,HGFilters,VE}.py`, `define_G` in `lib/net/FBNet.py`,
@@ -44,7 +46,10 @@ lib/dataset/mesh_util.py:187-237 (load_checkpoint:
 identical state_dict keys),
 lib/dataset/TestDataset.py:137 (get_visibility),
 scripts/render_single.py:118 (computePRT of the dataset preparation: the rays cast on the kernels, the same
-prt/bounce.npy and prt/face.npy written).
+prt/bounce.npy and prt/face.npy written),
+scripts/render_single.py:41, 97-141, 144-239 (initialize_GL_context, ColorRender and PRTRender: every render/,
+normal_F/B and T_normal_F/B image drawn on the kernels with no GL context; opengl_util's render_result, load_calib,
+make_rotate and rotateSH, Camera, load_scan and the script's RNG use stay the reference's).
 """
 import importlib.abc
 import importlib.machinery
@@ -57,7 +62,7 @@ _INSTALLED = None
 
 
 def _replacements():
-    from . import encoders, engine, net, voxelize
+    from . import dataset_render, encoders, engine, net, voxelize
     return {
         "lib.net.HGPIFuNet": {"HGPIFuNet": net.HGPIFuNet, "MLP": net.MLP, "BasePIFuNet": net.BasePIFuNet,
                               "NormalNet": encoders.NormalNet, "HGFilter": encoders.HGFilter,
@@ -65,6 +70,10 @@ def _replacements():
                               "init_net": net.init_net},
         "lib.net.voxelize": {"Voxelization": voxelize.Voxelization},
         "lib.common.seg3d_lossless": {"Seg3dLossless": engine.Seg3dLossless},
+        # the dataset renderer: each of these imports OpenGL.GL at the top
+        "lib.renderer.gl.prt_render": {"PRTRender": dataset_render.PRTRender},
+        "lib.renderer.gl.color_render": {"ColorRender": dataset_render.ColorRender},
+        "lib.renderer.gl.init_gl": {"initialize_GL_context": dataset_render.initialize_GL_context},
     }
 
 

@@ -284,6 +284,35 @@ int icon_normal_render(const float *verts, const float *norms, int V, const int6
                        const float *h_model, int width, int height, float *out_rgba, int32_t *out_face,
                        void *ws, size_t ws_bytes, icon_stream_t stream);
 
+/* ------------------------------------------------------------------ views of the dataset renderer
+ * Replace the OpenGL PRTRender (lib/renderer/gl/prt_render.py, shaders prt.vs / prt.fs, 16x MSAA) and ColorRender
+ * (color_render.py, color.vs / color.fs) that scripts/render_single.py draws with.  Rules (parity unpinned):
+ * csrc/dataset_render.cu header.
+ *
+ * icon_dr_mesh: device arrays of one mesh, every attribute indexed per face corner by its own [F,3] i64 index array.
+ * mode ICON_DR_PRT: pos [V,3], nrm [Vn,3], uv [Vt,2], attr = PRT [Va,9] (f32); tex = icon_dataset_texture's levels or
+ * NULL (albedo 1; uv / f_uv are then not read).  ICON_DR_COLOR: attr = colour [Va,3]; tex must be NULL. */
+#define ICON_DR_PRT 0
+#define ICON_DR_COLOR 1
+typedef struct {
+    int mode, F, V, Vn, Vt, Va;
+    const float *pos, *nrm, *uv, *attr;
+    const int64_t *f_pos, *f_nrm, *f_uv, *f_attr;
+    const uint8_t *tex;
+    int tex_w, tex_h;
+} icon_dr_mesh;
+/* icon_dataset_render: one view at width x height (each <= 16384) with samples in {1, 16} per pixel.  h_view: HOST
+ * pointer to 69 floats: NormMat rows 0-2 (12), RotMat (9, row-major), PerspMat ModelMat rows 0-2 (12; its row 3 must
+ * be (0, 0, 0, 1)), mat3(ModelMat) RotMat (9), SHCoeffs [9][3] (27).  out [3][height][width][4] f32 (16-byte
+ * aligned): attachments 0-2 in get_color's layout.  ws: icon_dataset_render_workspace_bytes (0 for bad sizes). */
+size_t icon_dataset_render_workspace_bytes(int F, int width, int height, int samples);
+int icon_dataset_render(const icon_dr_mesh *mesh, const float *h_view, int width, int height, int samples, float *out,
+                        void *ws, size_t ws_bytes, icon_stream_t stream);
+/* icon_dataset_texture: the albedo's mip levels 0-3 (RGBA8, level 0 = rgb [h,w,3] u8 flipped vertically, then 2x2
+ * boxes) into tex (icon_dataset_texture_bytes(w, h) bytes, 4-byte aligned), once per texture. */
+size_t icon_dataset_texture_bytes(int w, int h);
+int icon_dataset_texture(const uint8_t *rgb, int w, int h, uint8_t *tex, size_t tex_bytes, icon_stream_t stream);
+
 /* ------------------------------------------------------------------ self-rotation video of the demo
  * Replace the pytorch3d renders of Render.get_rendered_video (lib/common/render.py:327-374; MeshRasterizer +
  * cleanShader at get_camera / init_renderer(camera, "clean_mesh", "gray")) and the colours VF2Mesh gives a mesh.
