@@ -155,11 +155,18 @@ static inline int64_t brick_list_cap(int F) {
     const int64_t all = (int64_t)NBRICK * ((F + 3) / 4);
     return all < BRICK_LIST_CAP ? all : BRICK_LIST_CAP;
 }
+// Each brick's face list is culled from its leaf list, which the build keeps as scratch
+constexpr int BRICK_MAX_FACES = 4096;            // longest face list of one brick (it is sorted in shared memory)
+constexpr int64_t BRICK_FACE_CAP = 1 << 23;      // face entries per body (48 MB of uint16 ids and float keys)
+static inline int64_t brick_face_cap(int F) {
+    const int64_t all = (int64_t)NBRICK * F;
+    return all < BRICK_FACE_CAP ? all : BRICK_FACE_CAP;
+}
 
 struct MeshHeader {                  // device-resident, written by icon_smpl_prepare
     float y0, z0, inv_cy, inv_cz;    // ray grid origin / inverse cell size over the mesh yz box
     int ray_overflow;                // 1 -> cell lists overflowed: kernels fall back to all faces
-    int brick_built;                 // 1 -> the brick leaf lists are complete (built on the first dense call)
+    int brick_built;                 // 1 -> the brick lists are complete (built on the first dense call)
     int brick_overflow;              // 1 -> they did not fit: dense calls walk the tree
     int pad;
 };
@@ -199,6 +206,10 @@ struct MeshView : FaceTree {
     int32_t *boff;        // [NBRICK + 1] list offsets
     unsigned short *blist;   // [brick_cap] leaf ids, ascending box distance to the brick per list
     int64_t brick_cap;
+    int32_t *foff;        // [NBRICK + 1] face list offsets
+    unsigned short *flist;   // [face_cap] sorted face positions, ascending key per list
+    float *fkey;          // [face_cap] their keys: squared lower bound on the distance from any point of the brick
+    int64_t face_cap;
     int V;
 };
 size_t mesh_ws_bytes(int V, int F);

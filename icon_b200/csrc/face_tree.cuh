@@ -285,24 +285,20 @@ struct NearestFace {
         return L - he - pr - beta > tol + 1e-5f * (L + fabsf(he) + pr + fabsf(beta));
     }
 
-    // phase C, one step: this lane's slot holds `leaf` (-1: none), 4 lanes per leaf, 8 leaves = 32 faces, culled
+    // phase C, one step: this lane's slot holds sorted face k (outside [0, F): none), 32 faces per step, culled
     // against the warp's box [wlo, whi] by bounding sphere and the loosest lane bound, then by `beats`, staged
     // compacted, then split over the replicas
-    __device__ __forceinline__ void chunk(const FaceTree &t, ChunkSmem &S, int leaf, float4 wlo, float4 whi) {
+    __device__ __forceinline__ void chunk(const FaceTree &t, ChunkSmem &S, int k, float4 wlo, float4 whi) {
         bool pass = false;
-        int k = 0;
         float4 s = make_float4(0.f, 0.f, 0.f, 0.f), r0 = s, r1 = s, r2 = s;
-        if (leaf >= 0) {
-            k = 4 * leaf + (lane & 3);
-            if (k < t.F) {
-                s = __ldg(t.sph_s + k);
-                const float l2 = ub + s.w;                     // sphere vs the warp's box: some lane may be that close
-                pass = box_dist2(mk3(s.x, s.y, s.z), wlo, whi) <= l2 * l2;
-                if (CULL && pass) {
-                    const float4 *tp = t.tri_s + 3 * (size_t)k;
-                    r0 = __ldg(tp); r1 = __ldg(tp + 1); r2 = __ldg(tp + 2);
-                    pass = !beats(s, r0, r1, r2, wlo, whi);
-                }
+        if (k >= 0 && k < t.F) {
+            s = __ldg(t.sph_s + k);
+            const float l2 = ub + s.w;                         // sphere vs the warp's box: some lane may be that close
+            pass = box_dist2(mk3(s.x, s.y, s.z), wlo, whi) <= l2 * l2;
+            if (CULL && pass) {
+                const float4 *tp = t.tri_s + 3 * (size_t)k;
+                r0 = __ldg(tp); r1 = __ldg(tp + 1); r2 = __ldg(tp + 2);
+                pass = !beats(s, r0, r1, r2, wlo, whi);
             }
         }
         const unsigned mask = __ballot_sync(0xffffffffu, pass);
@@ -332,13 +328,13 @@ struct NearestFace {
         __syncwarp();
     }
 
-    // phase C over n leaves
+    // phase C over n leaves: 4 lanes per leaf, 8 leaves per step
     template <typename Id>
     __device__ __forceinline__ void scan_leaves(const FaceTree &t, ChunkSmem &S, const Id *leaves, int n, float4 wlo,
                                                 float4 whi) {
         for (int base = 0; base < n; base += 8) {
             const int slot = base + (lane >> 2);
-            chunk(t, S, slot < n ? (int)leaves[slot] : -1, wlo, whi);
+            chunk(t, S, slot < n ? 4 * (int)leaves[slot] + (lane & 3) : -1, wlo, whi);
         }
     }
 

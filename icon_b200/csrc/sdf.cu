@@ -146,8 +146,8 @@ __global__ void k_points_scatter(const int32_t *__restrict__ bid, int64_t N, con
 // walk), then the deferred tree walk's warps and cycles.  g_wstat: one record of WS_N words per brick-path warp.
 __device__ unsigned long long g_stats[8];
 __device__ unsigned *g_wstat;
-enum { WS_DEFER, WS_LEAVES, WS_STEPS, WS_STAGED, WS_SPH, WS_EXACT, WS_WIN, WS_RAY, WS_CYC_START, WS_CYC_C,
-       WS_CYC_RAY, WS_CYC_EMIT, WS_UB0, WS_UBEND, WS_LIST, WS_IDEAL_LEAVES, WS_IDEAL_FACES, WS_DEAD, WS_N = 20 };
+enum { WS_DEFER, WS_ENTRIES, WS_STEPS, WS_STAGED, WS_SPH, WS_EXACT, WS_WIN, WS_RAY, WS_CYC_START, WS_CYC_C,
+       WS_CYC_RAY, WS_CYC_EMIT, WS_UB0, WS_UBEND, WS_LIST, WS_IDEAL_ENTRIES, WS_IDEAL_FACES, WS_DEAD, WS_N = 20 };
 #define STAT(i, v) do { if (lane == 0) atomicAdd(&g_stats[i], (unsigned long long)(v)); } while (0)
 #define WSTAT(i, v) do { if (lane == 0 && g_wstat) g_wstat[(size_t)wid * WS_N + (i)] = (unsigned)(v); } while (0)
 #define WCLK(t) __syncwarp(); const long long t = clock64()
@@ -220,7 +220,7 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
 #ifdef ICON_SDF_STATS
     WCLK(t_start);
     long long t_c = 0, t_ray = 0;
-    int st_leaves = 0, st_steps = 0, st_brick = -1;
+    int st_entries = 0, st_steps = 0, st_brick = -1;
     float st_ub0 = 0.f;
 #endif
     if constexpr (BRICK) {
@@ -251,21 +251,21 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
         st_brick = b;
         st_ub0 = nf.ub;
 #endif
-        // the list is sorted by box distance to the brick, which bounds from below every lane's distance to the
-        // leaf's faces: once a step's first leaf is farther than the loosest lane bound, so is the rest of the list
-        const int o1 = __ldg(m.boff + b + 1);
-        for (int base = __ldg(m.boff + b); base < o1; base += 8) {
-            const int slot = base + (lane >> 2);
-            const int leaf = slot < o1 ? (int)__ldg(m.blist + slot) : -1;
-            float key = 0.f;
-            if (lane == 0) key = leaf_key(m, leaf, blo, bhi);
+        // the keys bound from below every lane's distance to the face and ascend along the list: once a step's
+        // first key is farther than the loosest lane bound, so is the rest of the list
+        const int o1 = __ldg(m.foff + b + 1);
+        for (int base = __ldg(m.foff + b); base < o1; base += 32) {
+            const int slot = base + lane;
+            const bool in = slot < o1;
+            const int k = in ? (int)__ldg(m.flist + slot) : -1;
+            const float key = in ? __ldg(m.fkey + slot) : 0.f;
             if (__shfl_sync(0xffffffffu, key, 0) > nf.ub * nf.ub) break;
-            STAT(2, min(8, o1 - base));
+            STAT(2, min(32, o1 - base));
 #ifdef ICON_SDF_STATS
-            st_leaves += min(8, o1 - base);
+            st_entries += min(32, o1 - base);
             ++st_steps;
 #endif
-            nf.chunk(m, S, leaf, wlo, whi);
+            nf.chunk(m, S, k, wlo, whi);
         }
         nf.merge();
     } else {
@@ -312,28 +312,20 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
 #ifdef ICON_SDF_STATS
     WCLK(t_end);
     if (BRICK && st_brick >= 0) {
-        // what box distance and bounding sphere alone keep at the final bound: leaves and faces within it of the box
+        // at the final bound: list entries the break alone keeps, and faces whose sphere lies within it of the box
         const float ube = nf.ub;
         int il = 0, ifc = 0;
-        const int o0 = __ldg(m.boff + st_brick), o1 = __ldg(m.boff + st_brick + 1);
+        const int o0 = __ldg(m.foff + st_brick), o1 = __ldg(m.foff + st_brick + 1);
         for (int s = o0 + lane; s < o1; s += 32) {
-            const int leaf = __ldg(m.blist + s);
-            const float4 a = __ldg(m.nodes + 2 * (size_t)leaf), z = __ldg(m.nodes + 2 * (size_t)leaf + 1);
-            const float gx = fmaxf(fmaxf(a.x - whi.x, wlo.x - z.x), 0.f);
-            const float gy = fmaxf(fmaxf(a.y - whi.y, wlo.y - z.y), 0.f);
-            const float gz = fmaxf(fmaxf(a.z - whi.z, wlo.z - z.z), 0.f);
-            if (fmaf(gz, gz, fmaf(gy, gy, gx * gx)) > ube * ube) continue;
-            ++il;
-            for (int k = 4 * leaf; k < min(4 * leaf + 4, m.F); ++k) {
-                const float4 s4 = __ldg(m.sph_s + k);
-                const float l2 = ube + s4.w;
-                ifc += box_dist2(mk3(s4.x, s4.y, s4.z), wlo, whi) <= l2 * l2;
-            }
+            il += __ldg(m.fkey + s) <= ube * ube;
+            const float4 s4 = __ldg(m.sph_s + __ldg(m.flist + s));
+            const float l2 = ube + s4.w;
+            ifc += box_dist2(mk3(s4.x, s4.y, s4.z), wlo, whi) <= l2 * l2;
         }
         const int s_sph = __reduce_add_sync(0xffffffffu, nf.n_sph), s_exact = __reduce_add_sync(0xffffffffu, nf.n_exact);
         const int s_win = __reduce_add_sync(0xffffffffu, nf.n_win), s_ray = __reduce_add_sync(0xffffffffu, st_ray);
         const int s_il = __reduce_add_sync(0xffffffffu, il), s_if = __reduce_add_sync(0xffffffffu, ifc);
-        WSTAT(WS_LEAVES, st_leaves);
+        WSTAT(WS_ENTRIES, st_entries);
         WSTAT(WS_STEPS, st_steps);
         WSTAT(WS_STAGED, nf.staged);
         WSTAT(WS_SPH, s_sph);
@@ -347,7 +339,7 @@ __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, co
         WSTAT(WS_UB0, __float_as_uint(st_ub0));
         WSTAT(WS_UBEND, __float_as_uint(ube));
         WSTAT(WS_LIST, o1 - o0);
-        WSTAT(WS_IDEAL_LEAVES, s_il);
+        WSTAT(WS_IDEAL_ENTRIES, s_il);
         WSTAT(WS_IDEAL_FACES, s_if);
         WSTAT(WS_DEAD, nf.n_dead);
     }
@@ -447,8 +439,114 @@ __global__ void __launch_bounds__(128) k_brick_fill(MeshView m, int64_t cap) {
     }
 }
 
-__global__ void k_brick_done(MeshView m, int64_t cap) {
-    if (m.boff[NBRICK] > cap) m.hdr->brick_overflow = 1;
+// A bound beta + g.(p - pc) >= D(p) over the brick's box [lo, hi] (centre pc), D the distance to the mesh, for `beats`
+// with the brick as the box.  The distance to the face nearest the brick centre bounds D from above and is convex (the
+// face is a convex set), so on the box it lies below the trilinear blend of its corner values d_i, which lies below
+// beta + g.(p - pc) once beta >= d_i - g.(c_i - pc) at every corner.  g is the least-squares slope of the corner values,
+// clamped to [-1, 1] per axis like start_scan's; any finite g keeps the bound.
+__device__ __forceinline__ void brick_plane(const MeshView &m, int b, float4 lo, float4 hi, NearestFace<32> &nf) {
+    const Tri t = load_tri(m.tri + 3 * (size_t)__ldg(m.bface + b));
+    float d[8], sx = 0.f, sy = 0.f, sz = 0.f;
+    for (int i = 0; i < 8; ++i) {
+        const V3 c = mk3(i & 1 ? hi.x : lo.x, i & 2 ? hi.y : lo.y, i & 4 ? hi.z : lo.z);
+        d[i] = sqrtf(tri_sqdist(c, t.a, t.ab, t.ac)) * 1.00001f + 1e-6f;
+        sx += i & 1 ? d[i] : -d[i];
+        sy += i & 2 ? d[i] : -d[i];
+        sz += i & 4 ? d[i] : -d[i];
+    }
+    const float h = 0.5f * BRICK_W;
+    nf.g = mk3(fminf(fmaxf(sx / (8.f * h), -1.f), 1.f), fminf(fmaxf(sy / (8.f * h), -1.f), 1.f),
+               fminf(fmaxf(sz / (8.f * h), -1.f), 1.f));
+    float beta = -FLT_MAX;
+    for (int i = 0; i < 8; ++i)
+        beta = fmaxf(beta, d[i] - ((i & 1 ? nf.g.x : -nf.g.x) + (i & 2 ? nf.g.y : -nf.g.y) + (i & 4 ? nf.g.z : -nf.g.z)) * h);
+    nf.beta = beta;                    // NaN (a degenerate face): beats() never culls
+}
+
+// candidate j of the brick's leaf list (4 faces per leaf) if `beats` cannot rule it out for any point of the brick:
+// its sorted position and key, a squared lower bound on the distance from any point of the brick to the face
+__device__ __forceinline__ bool brick_face(const MeshView &m, int o0, int j, float4 lo, float4 hi,
+                                           const NearestFace<32> &nf, int &k, float &key) {
+    k = 4 * (int)__ldg(m.blist + o0 + j / 4) + (j & 3);
+    if (k >= m.F) return false;
+    const float4 s = __ldg(m.sph_s + k);
+    const float4 *tp = m.tri_s + 3 * (size_t)k;
+    if (nf.beats(s, __ldg(tp), __ldg(tp + 1), __ldg(tp + 2), lo, hi)) return false;
+    const float gap = sqrtf(box_dist2(mk3(s.x, s.y, s.z), lo, hi)) * 0.99999f - s.w - 1e-6f;
+    key = gap > 0.f ? gap * gap : 0.f;
+    return true;
+}
+
+// the lengths of the face lists; a list past BRICK_MAX_FACES marks them overflowed, as do more than 65535 faces
+// (uint16 positions)
+__global__ void __launch_bounds__(128) k_face_count(MeshView m, int64_t cap) {
+    __shared__ int s_cnt;
+    if (m.F > 65535) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) m.hdr->brick_overflow = 1;
+        return;
+    }
+    if (m.hdr->brick_overflow || m.boff[NBRICK] > cap) return;      // no leaf lists to cull
+    const int b = blockIdx.x, o0 = m.boff[b], n = 4 * (m.boff[b + 1] - o0);
+    float4 lo, hi;
+    brick_box(b, lo, hi);
+    NearestFace<32> nf(mk3(0.f, 0.f, 0.f), 1e-6f, 1e-7f);
+    brick_plane(m, b, lo, hi, nf);
+    if (threadIdx.x == 0) s_cnt = 0;
+    __syncthreads();
+    int cnt = 0, k;
+    float key;
+    for (int j = threadIdx.x; j < n; j += blockDim.x) cnt += brick_face(m, o0, j, lo, hi, nf, k, key);
+    for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(&s_cnt, cnt);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        m.foff[b] = s_cnt;
+        if (s_cnt > BRICK_MAX_FACES) m.hdr->brick_overflow = 1;
+        if (b == 0) m.foff[NBRICK] = 0;
+    }
+}
+
+// after the scan: the brick's faces compacted in leaf-list order, then rank-sorted by key (ties: that order)
+__global__ void __launch_bounds__(128) k_face_fill(MeshView m, int64_t cap, int64_t fcap) {
+    __shared__ float s_key[BRICK_MAX_FACES];
+    __shared__ unsigned short s_k[BRICK_MAX_FACES];
+    __shared__ int s_wcnt[4];
+    if (m.hdr->brick_overflow || m.boff[NBRICK] > cap || m.foff[NBRICK] > fcap) return;   // k_brick_done records it
+    const int b = blockIdx.x, o0 = m.boff[b], nc = 4 * (m.boff[b + 1] - o0), f0 = m.foff[b];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    float4 lo, hi;
+    brick_box(b, lo, hi);
+    NearestFace<32> nf(mk3(0.f, 0.f, 0.f), 1e-6f, 1e-7f);
+    brick_plane(m, b, lo, hi, nf);
+    int n = 0;
+    for (int j0 = 0; j0 < nc; j0 += 128) {
+        const int j = j0 + threadIdx.x;
+        int k = 0;
+        float key = 0.f;
+        const bool in = j < nc && brick_face(m, o0, j, lo, hi, nf, k, key);
+        const unsigned bal = __ballot_sync(0xffffffffu, in);
+        if (lane == 0) s_wcnt[wib] = __popc(bal);
+        __syncthreads();
+        int at = n + __popc(bal & ((1u << lane) - 1u));
+        for (int w = 0; w < wib; ++w) at += s_wcnt[w];
+        if (in) { s_key[at] = key; s_k[at] = (unsigned short)k; }
+        n += s_wcnt[0] + s_wcnt[1] + s_wcnt[2] + s_wcnt[3];
+        __syncthreads();
+    }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const float k = s_key[i];
+        int r = 0;
+        for (int j = 0; j < n; ++j) {
+            const float kj = s_key[j];
+            r += kj < k || (kj == k && j < i);
+        }
+        m.flist[f0 + r] = s_k[i];
+        m.fkey[f0 + r] = k;
+    }
+}
+
+__global__ void k_brick_done(MeshView m, int64_t cap, int64_t fcap) {
+    if (m.boff[NBRICK] > cap || m.foff[NBRICK] > fcap) m.hdr->brick_overflow = 1;
     m.hdr->brick_built = 1;
 }
 
@@ -518,11 +616,14 @@ static SdfWs carve_sdf(Carver &c, int64_t N) {
     return w;
 }
 
-// The brick leaf lists of one body (DESIGN.md 4.2): the exact nearest face of each brick centre (the SDF kernel on
-// the 32768 centres) bounds the nearest distance of every point of the brick; count, scan and fill the lists of leaves
-// within that bound, each sorted by box distance.  Stream-ordered: the header's flag is set last.
+// The brick lists of one body (DESIGN.md 4.2): the exact nearest face of each brick centre (the SDF kernel on the 32768
+// centres) bounds the nearest distance of every point of the brick; count, scan and fill the lists of leaves within
+// that bound, each sorted by box distance; then count, scan and fill the faces of those leaves that `beats` cannot
+// rule out for the whole brick, each list sorted by key.  The leaf lists are build scratch.  Stream-ordered: the
+// header's flag is set last.
 static int build_bricks(const MeshView &m, cudaStream_t stream) {
     const int64_t cap = g_brick_max_entries > 0 ? std::min(g_brick_max_entries, m.brick_cap) : m.brick_cap;
+    const int64_t fcap = g_brick_max_entries > 0 ? std::min(g_brick_max_entries, m.face_cap) : m.face_cap;
     k_brick_centres<<<NBRICK / 256, 256, 0, stream>>>(m);
     ICON_LAUNCHED();
     k_sdf_warp<1, false><<<NBRICK / (SW_T / 32), SW_T, sdf_smem_bytes<1, false>(), stream>>>(
@@ -534,7 +635,13 @@ static int build_bricks(const MeshView &m, cudaStream_t stream) {
     if (rc) return rc;
     k_brick_fill<<<NBRICK, 128, 0, stream>>>(m, cap);
     ICON_LAUNCHED();
-    k_brick_done<<<1, 1, 0, stream>>>(m, cap);
+    k_face_count<<<NBRICK, 128, 0, stream>>>(m, cap);
+    ICON_LAUNCHED();
+    rc = scan_exclusive_i32(m.foff, m.foff, NBRICK + 1, nullptr, m.scan_ws, stream);
+    if (rc) return rc;
+    k_face_fill<<<NBRICK, 128, 0, stream>>>(m, cap, fcap);
+    ICON_LAUNCHED();
+    k_brick_done<<<1, 1, 0, stream>>>(m, cap, fcap);
     ICON_LAUNCHED();
     return ICON_OK;
 }

@@ -41,6 +41,10 @@ static MeshView carve_mesh(Carver &c, int V, int F) {
     m.boff = c.take<int32_t>(NBRICK + 1);
     m.brick_cap = brick_list_cap(F);
     m.blist = c.take<unsigned short>((size_t)m.brick_cap);
+    m.foff = c.take<int32_t>(NBRICK + 1);
+    m.face_cap = brick_face_cap(F);
+    m.flist = c.take<unsigned short>((size_t)m.face_cap);
+    m.fkey = c.take<float>((size_t)m.face_cap);
     m.vn_ws = c.take<char>(area_vertex_normals_ws_bytes(V, F));
     m.vnormals = c.take<float>((size_t)V * 3);      // last: tests read it from the tail
     return m;

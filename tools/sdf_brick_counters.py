@@ -7,7 +7,7 @@ icon_b200/build.py left them; the product build is not touched), runs sdf_only o
 and the res^3 cell-centre lattice, and prints one JSON line: per brick-path warp, the median / p90 / p99 and the
 mean of each counter, and the cycle-weighted mean (warps weighted by their total cycles).  Also reports ptxas
 registers and spills of both dense instantiations as the product build compiles them.  DIR/warps.npz keeps the raw
-records.  The counters' own stores and the scan behind ideal_leaves / ideal_faces (what box distance and bounding sphere
+records.  The counters' own stores and the scan behind ideal_entries / ideal_faces (what the break and bounding sphere
 alone keep at the final bound) run outside the timed segments, but the clocks are those of a build that also counts,
 so use them as shares, not as the product kernel's time.
 """
@@ -22,8 +22,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 # record layout of sdf.cu (WS_* enum)
-FIELDS = ["defer", "leaves", "steps", "staged", "sph_pass", "exact", "win", "ray", "cyc_start", "cyc_c", "cyc_ray",
-          "cyc_emit", "ub0", "ub_end", "list_len", "ideal_leaves", "ideal_faces", "dead_staged"]
+FIELDS = ["defer", "entries", "steps", "staged", "sph_pass", "exact", "win", "ray", "cyc_start", "cyc_c", "cyc_ray",
+          "cyc_emit", "ub0", "ub_end", "list_len", "ideal_entries", "ideal_faces", "dead_staged"]
 WS_N = 20
 FLOAT_FIELDS = ("ub0", "ub_end")
 PER_LANE = ("sph_pass", "exact", "win", "ray")      # summed over the 32 lanes in the record

@@ -1,4 +1,4 @@
-"""Brick leaf lists of the dense SDF path: build cost, list size, and sdf_only with the path on / off (alternating).
+"""Brick lists of the dense SDF path: build cost, list size, and sdf_only with the path on / off (alternating).
 
     python tools/time_sdf_bricks.py [--reps 5]
 
