@@ -145,17 +145,12 @@ constexpr int TREE_MAX_LEVELS = 17;  // 4-ary implicit tree over leaves of 4 Mor
 constexpr int RAY_GRID = 256;        // yz cell grid for the +x ray parity
 constexpr int RAY_LIST_PER_FACE = 64;
 
-// Brick leaf lists for dense lattices (sdf.cu): a 32^3 grid of bricks over [-1,1]^3, one brick = 4^3 of the SDF's
-// 128^3 Morton bins, so every warp of 32 Morton-adjacent lattice points lies inside one brick.
+// Brick face lists for dense lattices (sdf.cu): a 32^3 grid of bricks over [-1,1]^3, one brick = 4^3 of the SDF's
+// 128^3 Morton bins, so every warp of 32 Morton-adjacent lattice points lies inside one brick.  Each brick's list is
+// culled from the faces of its nearby leaves, which the build gathers and sorts in shared memory.
 constexpr int BRICK_AX = 32;
 constexpr int NBRICK = BRICK_AX * BRICK_AX * BRICK_AX;
-constexpr int BRICK_MAX_LEAVES = 4096;           // longest list of one brick (it is sorted in shared memory)
-constexpr int64_t BRICK_LIST_CAP = 1 << 24;      // leaf entries per body (32 MB of uint16)
-static inline int64_t brick_list_cap(int F) {
-    const int64_t all = (int64_t)NBRICK * ((F + 3) / 4);
-    return all < BRICK_LIST_CAP ? all : BRICK_LIST_CAP;
-}
-// Each brick's face list is culled from its leaf list, which the build keeps as scratch
+constexpr int BRICK_MAX_LEAVES = 4096;           // most leaves one brick's list is culled from
 constexpr int BRICK_MAX_FACES = 4096;            // longest face list of one brick (it is sorted in shared memory)
 constexpr int64_t BRICK_FACE_CAP = 1 << 23;      // face entries per body (48 MB of uint16 ids and float keys)
 static inline int64_t brick_face_cap(int F) {
@@ -197,15 +192,12 @@ struct MeshView : FaceTree {
     int32_t *rlist;       // [F * RAY_LIST_PER_FACE]
     MeshHeader *hdr;
     void *scan_ws;
-    // brick leaf lists (CSR): built lazily by the first call that takes the dense path
+    // brick face lists (CSR): built lazily by the first call that takes the dense path
     float4 *bxyz;         // [NBRICK] brick centres (build input)
     int32_t *bperm;       // [NBRICK] identity (build input)
     float *brec;          // [NBRICK][8] build scratch
     int32_t *bface;       // [NBRICK] original id of the face nearest the brick centre
     float *bub;           // [NBRICK] bound on the nearest distance of every point of the brick (inflated)
-    int32_t *boff;        // [NBRICK + 1] list offsets
-    unsigned short *blist;   // [brick_cap] leaf ids, ascending box distance to the brick per list
-    int64_t brick_cap;
     int32_t *foff;        // [NBRICK + 1] face list offsets
     unsigned short *flist;   // [face_cap] sorted face positions, ascending key per list
     float *fkey;          // [face_cap] their keys: squared lower bound on the distance from any point of the brick

@@ -8,7 +8,7 @@
 // Design (DESIGN.md 4.2): one WARP per group of PPW query points (32 Morton-adjacent lattice points on the dense grid).
 //   nearest face  the tree walk of face_tree.cuh over the body's tree (icon_smpl_prepare), descending towards the
 //                 warp centre, with a 16-bit frontier and the fixed slacks of coordinates of magnitude ~1.
-//                 Dense lattices (PPW = 32) replace its phases A and B by a per-body leaf list of the warp's brick
+//                 Dense lattices (PPW = 32) replace its phases A and B by a per-body face list of the warp's brick
 //                 (32^3 bricks over [-1,1]^3, built by the body's first dense call), sorted by distance, so phase C
 //                 can stop early.
 //   sign          the faces listed in the point's yz cell (256 x 256 grid over the mesh's yz
@@ -142,8 +142,9 @@ __global__ void k_points_scatter(const int32_t *__restrict__ bid, int64_t N, con
 }
 
 #ifdef ICON_SDF_STATS
-// Diagnostics build only (tools/sdf_brick_counters.py).  g_stats: warps, overflow warps, leaves, faces staged (tree
-// walk), then the deferred tree walk's warps and cycles.  g_wstat: one record of WS_N words per brick-path warp.
+// Diagnostics build only (tools/sdf_brick_counters.py).  g_stats: warps, overflow warps, face-list entries (brick
+// path) or leaves (tree walk), faces staged, then the deferred tree walk's warps and cycles.  g_wstat: one record of
+// WS_N words per brick-path warp.
 __device__ unsigned long long g_stats[8];
 __device__ unsigned *g_wstat;
 enum { WS_DEFER, WS_ENTRIES, WS_STEPS, WS_STAGED, WS_SPH, WS_EXACT, WS_WIN, WS_RAY, WS_CYC_START, WS_CYC_C,
@@ -156,7 +157,7 @@ enum { WS_DEFER, WS_ENTRIES, WS_STEPS, WS_STAGED, WS_SPH, WS_EXACT, WS_WIN, WS_R
 #define WSTAT(i, v) do { } while (0)
 #endif
 
-// 16-bit frontier ids: icon_smpl_prepare checks that the leaf count is <= 65535.  The brick path reads its leaf list
+// 16-bit frontier ids: icon_smpl_prepare checks that the leaf count is <= 65535.  The brick path reads its face list
 // from global memory and needs no frontier (a third of the shared memory; at 64 registers per thread, registers then
 // bound residency at 32 warps per SM)
 template <int PPW, bool BRICK>
@@ -190,7 +191,7 @@ __device__ __forceinline__ float leaf_key(const MeshView &m, int l, float4 lo, f
 // per-point minimum and the 32 lanes only share the work.  The kernel is bound by the latency of the dependent
 // tree loads, so the shared-memory footprint (fr_cap) is kept small enough for >= 36 resident warps per SM.
 // BRICK (PPW = 32, dense lattices): a warp whose box lies inside one brick skips phases A and B: its first bound is
-// the brick's, its first candidate the face nearest the brick centre, and phase C scans the brick's leaf list.
+// the brick's, its first candidate the face nearest the brick centre, and phase C scans the brick's face list.
 template <int PPW, bool BRICK>
 __device__ __forceinline__ void sdf_warp(int64_t wid, SdfSmem<PPW, BRICK> &S, const float4 *__restrict__ xyz4,
                                          const int32_t *__restrict__ perm, int64_t N, const MeshView &m,
@@ -366,7 +367,7 @@ __global__ void __launch_bounds__(SW_T, PPW == 32 ? 8 : 0) k_sdf_warp(const floa
         sdf_warp<PPW, BRICK>(listed ? (int64_t)defer[i] : i, S, xyz4, perm, N, m, rec, face, defer, ndefer);
 }
 
-// ---------------------------------------------------------------- brick leaf lists (built once per body)
+// ---------------------------------------------------------------- brick face lists (built once per body)
 __global__ void k_brick_centres(MeshView m) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= NBRICK) return;
@@ -376,66 +377,35 @@ __global__ void k_brick_centres(MeshView m) {
     m.bperm[b] = b;
 }
 
-// bound of the brick (every point of it is within sqrt(d) + half-diagonal of the face nearest its centre) and the
-// length of its list: the leaves whose box lies within that bound of the brick's box
-__global__ void __launch_bounds__(128) k_brick_count(MeshView m) {
-    __shared__ int s_cnt;
-    const int b = blockIdx.x;
-    float4 lo, hi;
-    brick_box(b, lo, hi);
-    const float4 cc = m.bxyz[b];
-    const Tri t = load_tri(m.tri + 3 * (size_t)m.bface[b]);
-    const float d = tri_sqdist(mk3(cc.x, cc.y, cc.z), t.a, t.ab, t.ac);
-    const float ub = (sqrtf(d) + BRICK_HALF_DIAG) * 1.00001f + 1e-6f, ub2 = ub * ub;
-    if (threadIdx.x == 0) s_cnt = 0;
+// Block gather: put(at, key, tag) for the items i of [0, n) that take(i, key, tag) keeps, at = 0, 1, ... in no
+// particular order (*s_n = 0 before the call, which starts with a barrier); returns how many were kept.  The order is
+// restored by rank_sort, so no barrier per chunk of items is needed.
+template <class Take, class Put>
+__device__ __forceinline__ int block_gather(int n, int *s_n, Take &&take, Put &&put) {
     __syncthreads();
-    int cnt = 0;
-    for (int l = threadIdx.x; l < m.lvl_cnt[0]; l += blockDim.x) cnt += leaf_key(m, l, lo, hi) <= ub2;
-    for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(&s_cnt, cnt);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        m.bub[b] = ub;
-        m.boff[b] = s_cnt;
-        if (s_cnt > BRICK_MAX_LEAVES) m.hdr->brick_overflow = 1;
-        if (b == 0) m.boff[NBRICK] = 0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        float key;
+        int tag;
+        if (take(i, key, tag)) put(atomicAdd(s_n, 1), key, tag);
     }
+    __syncthreads();
+    return *s_n;
 }
 
-// after the scan: the brick's leaves compacted in leaf order, then rank-sorted by key (ties: leaf order)
-__global__ void __launch_bounds__(128) k_brick_fill(MeshView m, int64_t cap) {
-    __shared__ float s_key[BRICK_MAX_LEAVES];
-    __shared__ unsigned short s_leaf[BRICK_MAX_LEAVES];
-    __shared__ int s_wcnt[4];
-    if (m.hdr->brick_overflow || m.boff[NBRICK] > cap) return;      // k_brick_done records the overflow
-    const int b = blockIdx.x, o0 = m.boff[b], lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    float4 lo, hi;
-    brick_box(b, lo, hi);
-    const float ub = m.bub[b], ub2 = ub * ub;
-    const int nleaf = m.lvl_cnt[0];
-    int n = 0;
-    for (int l0 = 0; l0 < nleaf; l0 += 128) {
-        const int l = l0 + threadIdx.x;
-        float key = 0.f;
-        if (l < nleaf) key = leaf_key(m, l, lo, hi);
-        const bool in = l < nleaf && key <= ub2;
-        const unsigned bal = __ballot_sync(0xffffffffu, in);
-        if (lane == 0) s_wcnt[wib] = __popc(bal);
-        __syncthreads();
-        int at = n + __popc(bal & ((1u << lane) - 1u));
-        for (int w = 0; w < wib; ++w) at += s_wcnt[w];
-        if (in) { s_key[at] = key; s_leaf[at] = (unsigned short)l; }
-        n += s_wcnt[0] + s_wcnt[1] + s_wcnt[2] + s_wcnt[3];
-        __syncthreads();
-    }
+// A key >= +0 (never NaN or -0) and a distinct 16-bit tag as one word whose unsigned order is (key, tag): the bits of
+// a non-negative float order like its value
+__device__ __forceinline__ unsigned long long key_tag(float key, int tag) {
+    return (unsigned long long)__float_as_uint(key) << 32 | (unsigned)tag;
+}
+
+// Rank sort of the distinct words s_kt[0, n), ascending: put(rank, i) for every i
+template <class Put>
+__device__ __forceinline__ void rank_sort(const unsigned long long *s_kt, int n, Put &&put) {
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const float k = s_key[i];
+        const unsigned long long x = s_kt[i];
         int r = 0;
-        for (int j = 0; j < n; ++j) {
-            const float kj = s_key[j];
-            r += kj < k || (kj == k && j < i);
-        }
-        m.blist[o0 + r] = s_leaf[i];
+        for (int j = 0; j < n; ++j) r += s_kt[j] < x;
+        put(r, i);
     }
 }
 
@@ -463,11 +433,11 @@ __device__ __forceinline__ void brick_plane(const MeshView &m, int b, float4 lo,
     nf.beta = beta;                    // NaN (a degenerate face): beats() never culls
 }
 
-// candidate j of the brick's leaf list (4 faces per leaf) if `beats` cannot rule it out for any point of the brick:
+// candidate j of the brick's leaves (4 faces per leaf) if `beats` cannot rule it out for any point of the brick:
 // its sorted position and key, a squared lower bound on the distance from any point of the brick to the face
-__device__ __forceinline__ bool brick_face(const MeshView &m, int o0, int j, float4 lo, float4 hi,
+__device__ __forceinline__ bool brick_face(const MeshView &m, const unsigned short *leaves, int j, float4 lo, float4 hi,
                                            const NearestFace<32> &nf, int &k, float &key) {
-    k = 4 * (int)__ldg(m.blist + o0 + j / 4) + (j & 3);
+    k = 4 * (int)leaves[j / 4] + (j & 3);
     if (k >= m.F) return false;
     const float4 s = __ldg(m.sph_s + k);
     const float4 *tp = m.tri_s + 3 * (size_t)k;
@@ -477,76 +447,82 @@ __device__ __forceinline__ bool brick_face(const MeshView &m, int o0, int j, flo
     return true;
 }
 
-// the lengths of the face lists; a list past BRICK_MAX_FACES marks them overflowed, as do more than 65535 faces
-// (uint16 positions)
-__global__ void __launch_bounds__(128) k_face_count(MeshView m, int64_t cap) {
-    __shared__ int s_cnt;
-    if (m.F > 65535) {
-        if (blockIdx.x == 0 && threadIdx.x == 0) m.hdr->brick_overflow = 1;
-        return;
-    }
-    if (m.hdr->brick_overflow || m.boff[NBRICK] > cap) return;      // no leaf lists to cull
-    const int b = blockIdx.x, o0 = m.boff[b], n = 4 * (m.boff[b + 1] - o0);
+// One CTA per brick.  The brick's leaves are those whose box lies within its bound U_b (every point of the brick is
+// within sqrt(d) + half-diagonal of the face nearest its centre) of the brick's box, gathered into shared memory; its
+// face list keeps the faces of those leaves that `beats` cannot rule out for any point of the brick.
+// Count pass (!FILL): U_b into bub and the list's length into foff; more than BRICK_MAX_LEAVES leaves, a list past
+// BRICK_MAX_FACES or more than 65535 faces (uint16 positions) marks the lists overflowed.  Fill pass, after the scan:
+// the leaves rank-sorted by key (ties: leaf id), then the kept faces, tagged with their candidate position j over the
+// sorted leaves, rank-sorted by key (ties: j) into flist / fkey.  Both orders are those of an in-order compaction.
+template <bool FILL>
+__global__ void __launch_bounds__(128) k_brick_faces(MeshView m, int64_t fcap) {
+    static_assert(BRICK_MAX_FACES <= BRICK_MAX_LEAVES, "the face stage reuses the leaf array");
+    static_assert(4 * BRICK_MAX_LEAVES <= 65536, "candidate positions are 16-bit tags");
+    // count: the leaf ids; fill: (key, leaf id), then (key, candidate position j) of the faces, and the leaf ids in
+    // key order
+    __shared__ unsigned short s_leaf[BRICK_MAX_LEAVES];
+    __shared__ unsigned long long s_kt[FILL ? BRICK_MAX_LEAVES : 1];
+    __shared__ int s_n[2];                                // gathered leaves, faces
+    if (FILL && (m.hdr->brick_overflow || m.foff[NBRICK] > fcap)) return;    // k_brick_done records the overflow
+    if (threadIdx.x == 0) s_n[0] = s_n[1] = 0;
+    const int b = blockIdx.x;
     float4 lo, hi;
     brick_box(b, lo, hi);
+    float ub;
+    if (FILL) {
+        ub = m.bub[b];
+    } else {
+        const float4 cc = m.bxyz[b];
+        const Tri t = load_tri(m.tri + 3 * (size_t)m.bface[b]);
+        const float d = tri_sqdist(mk3(cc.x, cc.y, cc.z), t.a, t.ab, t.ac);
+        ub = (sqrtf(d) + BRICK_HALF_DIAG) * 1.00001f + 1e-6f;
+    }
+    const float ub2 = ub * ub;
+    const int n = block_gather(m.lvl_cnt[0], &s_n[0], [&](int l, float &key, int &tag) {
+        key = leaf_key(m, l, lo, hi);
+        tag = l;
+        return key <= ub2;
+    }, [&](int at, float key, int tag) {
+        if (at >= BRICK_MAX_LEAVES) return;
+        if (FILL) s_kt[at] = key_tag(key, tag);
+        else s_leaf[at] = (unsigned short)tag;
+    });
     NearestFace<32> nf(mk3(0.f, 0.f, 0.f), 1e-6f, 1e-7f);
     brick_plane(m, b, lo, hi, nf);
-    if (threadIdx.x == 0) s_cnt = 0;
-    __syncthreads();
-    int cnt = 0, k;
-    float key;
-    for (int j = threadIdx.x; j < n; j += blockDim.x) cnt += brick_face(m, o0, j, lo, hi, nf, k, key);
-    for (int o = 16; o; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(&s_cnt, cnt);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        m.foff[b] = s_cnt;
-        if (s_cnt > BRICK_MAX_FACES) m.hdr->brick_overflow = 1;
-        if (b == 0) m.foff[NBRICK] = 0;
-    }
-}
-
-// after the scan: the brick's faces compacted in leaf-list order, then rank-sorted by key (ties: that order)
-__global__ void __launch_bounds__(128) k_face_fill(MeshView m, int64_t cap, int64_t fcap) {
-    __shared__ float s_key[BRICK_MAX_FACES];
-    __shared__ unsigned short s_k[BRICK_MAX_FACES];
-    __shared__ int s_wcnt[4];
-    if (m.hdr->brick_overflow || m.boff[NBRICK] > cap || m.foff[NBRICK] > fcap) return;   // k_brick_done records it
-    const int b = blockIdx.x, o0 = m.boff[b], nc = 4 * (m.boff[b + 1] - o0), f0 = m.foff[b];
-    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    float4 lo, hi;
-    brick_box(b, lo, hi);
-    NearestFace<32> nf(mk3(0.f, 0.f, 0.f), 1e-6f, 1e-7f);
-    brick_plane(m, b, lo, hi, nf);
-    int n = 0;
-    for (int j0 = 0; j0 < nc; j0 += 128) {
-        const int j = j0 + threadIdx.x;
-        int k = 0;
-        float key = 0.f;
-        const bool in = j < nc && brick_face(m, o0, j, lo, hi, nf, k, key);
-        const unsigned bal = __ballot_sync(0xffffffffu, in);
-        if (lane == 0) s_wcnt[wib] = __popc(bal);
+    if constexpr (!FILL) {
+        const bool fits = n <= BRICK_MAX_LEAVES && m.F <= 65535;
+        int cnt = 0, k;
+        float key;
+        if (fits)
+            for (int j = threadIdx.x; j < 4 * n; j += blockDim.x) cnt += brick_face(m, s_leaf, j, lo, hi, nf, k, key);
+        cnt = __reduce_add_sync(0xffffffffu, cnt);
+        if ((threadIdx.x & 31) == 0) atomicAdd(&s_n[1], cnt);
         __syncthreads();
-        int at = n + __popc(bal & ((1u << lane) - 1u));
-        for (int w = 0; w < wib; ++w) at += s_wcnt[w];
-        if (in) { s_key[at] = key; s_k[at] = (unsigned short)k; }
-        n += s_wcnt[0] + s_wcnt[1] + s_wcnt[2] + s_wcnt[3];
-        __syncthreads();
-    }
-    for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const float k = s_key[i];
-        int r = 0;
-        for (int j = 0; j < n; ++j) {
-            const float kj = s_key[j];
-            r += kj < k || (kj == k && j < i);
+        if (threadIdx.x == 0) {
+            m.bub[b] = ub;
+            m.foff[b] = s_n[1];
+            if (!fits || s_n[1] > BRICK_MAX_FACES) m.hdr->brick_overflow = 1;
+            if (b == 0) m.foff[NBRICK] = 0;
         }
-        m.flist[f0 + r] = s_k[i];
-        m.fkey[f0 + r] = k;
+    } else {
+        rank_sort(s_kt, n, [&](int r, int i) { s_leaf[r] = (unsigned short)s_kt[i]; });
+        const int f0 = m.foff[b];
+        const int nkept = block_gather(4 * n, &s_n[1], [&](int j, float &key, int &tag) {
+            int k;
+            tag = j;
+            return brick_face(m, s_leaf, j, lo, hi, nf, k, key);
+        }, [&](int at, float key, int tag) { if (at < BRICK_MAX_FACES) s_kt[at] = key_tag(key, tag); });
+        rank_sort(s_kt, nkept, [&](int r, int i) {
+            const unsigned long long x = s_kt[i];
+            const int j = (int)(x & 0xffffu);
+            m.flist[f0 + r] = (unsigned short)(4 * s_leaf[j / 4] + (j & 3));
+            m.fkey[f0 + r] = __uint_as_float((unsigned)(x >> 32));
+        });
     }
 }
 
-__global__ void k_brick_done(MeshView m, int64_t cap, int64_t fcap) {
-    if (m.boff[NBRICK] > cap || m.foff[NBRICK] > fcap) m.hdr->brick_overflow = 1;
+__global__ void k_brick_done(MeshView m, int64_t fcap) {
+    if (m.foff[NBRICK] > fcap) m.hdr->brick_overflow = 1;
     m.hdr->brick_built = 1;
 }
 
@@ -582,8 +558,8 @@ __global__ void __launch_bounds__(256) k_sdf_brute(const float *__restrict__ pts
 // points-per-warp policy of k_sdf_warp (see its header comment); icon_set_sdf_policy() overrides it for tuning
 static int64_t g_sdf_ppw32_from = 6000000, g_sdf_ppw8_from = 300000;
 static int g_sdf_ppw_force = 0;
-static int g_sdf_bricks = 1;              // brick leaf lists on PPW = 32 calls (icon_set_sdf_bricks)
-static int64_t g_brick_max_entries = 0;   // > 0: a build may use at most this many list entries
+static int g_sdf_bricks = 1;              // brick face lists on PPW = 32 calls (icon_set_sdf_bricks)
+static int64_t g_brick_max_entries = 0;   // > 0: a build may use at most this many face-list entries
 
 // Prepared bodies whose brick lists have been enqueued, by mesh header.  icon_smpl_prepare forgets its workspace, so
 // a new body -- also one that reuses freed memory -- gets fresh lists.  The kernel itself only trusts the header.
@@ -617,31 +593,23 @@ static SdfWs carve_sdf(Carver &c, int64_t N) {
 }
 
 // The brick lists of one body (DESIGN.md 4.2): the exact nearest face of each brick centre (the SDF kernel on the 32768
-// centres) bounds the nearest distance of every point of the brick; count, scan and fill the lists of leaves within
-// that bound, each sorted by box distance; then count, scan and fill the faces of those leaves that `beats` cannot
-// rule out for the whole brick, each list sorted by key.  The leaf lists are build scratch.  Stream-ordered: the
-// header's flag is set last.
+// centres) bounds the nearest distance of every point of the brick; count, scan and fill the faces that `beats`
+// cannot rule out for the whole brick among the leaves within that bound, each list sorted by key.  Stream-ordered:
+// the header's flag is set last.
 static int build_bricks(const MeshView &m, cudaStream_t stream) {
-    const int64_t cap = g_brick_max_entries > 0 ? std::min(g_brick_max_entries, m.brick_cap) : m.brick_cap;
     const int64_t fcap = g_brick_max_entries > 0 ? std::min(g_brick_max_entries, m.face_cap) : m.face_cap;
     k_brick_centres<<<NBRICK / 256, 256, 0, stream>>>(m);
     ICON_LAUNCHED();
     k_sdf_warp<1, false><<<NBRICK / (SW_T / 32), SW_T, sdf_smem_bytes<1, false>(), stream>>>(
         m.bxyz, m.bperm, NBRICK, m, m.brec, m.bface, nullptr, nullptr);
     ICON_LAUNCHED();
-    k_brick_count<<<NBRICK, 128, 0, stream>>>(m);
+    k_brick_faces<false><<<NBRICK, 128, 0, stream>>>(m, fcap);
     ICON_LAUNCHED();
-    int rc = scan_exclusive_i32(m.boff, m.boff, NBRICK + 1, nullptr, m.scan_ws, stream);
+    const int rc = scan_exclusive_i32(m.foff, m.foff, NBRICK + 1, nullptr, m.scan_ws, stream);
     if (rc) return rc;
-    k_brick_fill<<<NBRICK, 128, 0, stream>>>(m, cap);
+    k_brick_faces<true><<<NBRICK, 128, 0, stream>>>(m, fcap);
     ICON_LAUNCHED();
-    k_face_count<<<NBRICK, 128, 0, stream>>>(m, cap);
-    ICON_LAUNCHED();
-    rc = scan_exclusive_i32(m.foff, m.foff, NBRICK + 1, nullptr, m.scan_ws, stream);
-    if (rc) return rc;
-    k_face_fill<<<NBRICK, 128, 0, stream>>>(m, cap, fcap);
-    ICON_LAUNCHED();
-    k_brick_done<<<1, 1, 0, stream>>>(m, cap, fcap);
+    k_brick_done<<<1, 1, 0, stream>>>(m, fcap);
     ICON_LAUNCHED();
     return ICON_OK;
 }
@@ -796,11 +764,11 @@ extern "C" int icon_sdf_brick_info(const void *mesh_ws, int V, int F, int64_t *o
     int32_t total = 0;
     ICON_CUDA(cudaDeviceSynchronize());
     ICON_CUDA(cudaMemcpy(&h, m.hdr, sizeof(h), cudaMemcpyDeviceToHost));
-    if (h.brick_built) ICON_CUDA(cudaMemcpy(&total, m.boff + NBRICK, sizeof(total), cudaMemcpyDeviceToHost));
+    if (h.brick_built) ICON_CUDA(cudaMemcpy(&total, m.foff + NBRICK, sizeof(total), cudaMemcpyDeviceToHost));
     out[0] = h.brick_built;
     out[1] = h.brick_overflow;
     out[2] = total;
-    out[3] = m.brick_cap;
+    out[3] = m.face_cap;
     {
         std::lock_guard<std::mutex> lk(icon::g_brick_mu);
         out[4] = icon::g_brick_builds;

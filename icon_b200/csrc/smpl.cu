@@ -38,9 +38,6 @@ static MeshView carve_mesh(Carver &c, int V, int F) {
     m.brec = c.take<float>((size_t)NBRICK * 8);
     m.bface = c.take<int32_t>(NBRICK);
     m.bub = c.take<float>(NBRICK);
-    m.boff = c.take<int32_t>(NBRICK + 1);
-    m.brick_cap = brick_list_cap(F);
-    m.blist = c.take<unsigned short>((size_t)m.brick_cap);
     m.foff = c.take<int32_t>(NBRICK + 1);
     m.face_cap = brick_face_cap(F);
     m.flist = c.take<unsigned short>((size_t)m.face_cap);

@@ -193,13 +193,14 @@ def set_sdf_policy(force_ppw=0, ppw8_from=-1, ppw32_from=-1):
 
 
 def set_sdf_bricks(enable=True, max_entries=0):
-    """Brick leaf lists of the dense SDF path on / off (include/icon_b200.h: icon_set_sdf_bricks); max_entries > 0
-    caps the list entries of later builds."""
+    """Brick face lists of the dense SDF path on / off (include/icon_b200.h: icon_set_sdf_bricks); max_entries > 0
+    caps the face-list entries of later builds."""
     check(lib.icon_set_sdf_bricks(int(bool(enable)), int(max_entries)), "icon_set_sdf_bricks")
 
 
 def sdf_brick_info(body):
-    """Brick list state of a prepared body: built, overflow, entries, capacity, builds (process-wide count)."""
+    """Brick list state of a prepared body: built, overflow, face-list entries and their capacity, builds
+    (process-wide count)."""
     out = (ctypes.c_int64 * 5)()
     check(lib.icon_sdf_brick_info(_p(body.ws), body.V, body.F, out), "icon_sdf_brick_info")
     return dict(zip(("built", "overflow", "entries", "capacity", "builds"), (int(v) for v in out)))

@@ -133,14 +133,14 @@ int icon_query_feats(int prior, const float *points, int64_t stride_c, int64_t s
  * points per call, 8 below ppw32_from, else 32; negative thresholds keep the current value).  Results are
  * identical for every setting. */
 int icon_set_sdf_policy(int force_ppw, int64_t ppw8_from, int64_t ppw32_from);
-/* Brick leaf lists of the PPW = 32 path (default on): a body's first dense call builds, into its mesh workspace, a
- * sorted list of candidate leaves for each of 32^3 bricks over [-1,1]^3; warps inside one brick then skip the tree
- * walk.  enable = 0 turns the path off (A/B runs).  max_entries > 0 caps the list entries later builds may use (a
- * build past the cap marks the lists overflowed and dense calls walk the tree); 0 = the workspace's capacity.
+/* Brick face lists of the PPW = 32 path (default on): a body's first dense call builds, into its mesh workspace, a
+ * sorted list of candidate faces for each of 32^3 bricks over [-1,1]^3; warps inside one brick then skip the tree
+ * walk.  enable = 0 turns the path off (A/B runs).  max_entries > 0 caps the face-list entries later builds may use
+ * (a build past the cap marks the lists overflowed and dense calls walk the tree); 0 = the workspace's capacity.
  * Results are identical either way. */
 int icon_set_sdf_bricks(int enable, int64_t max_entries);
-/* Brick list state of a prepared body (synchronises the device): out[0] built, [1] overflowed, [2] list entries,
- * [3] entry capacity of the workspace, [4] builds enqueued by this process so far (all bodies). */
+/* Brick list state of a prepared body (synchronises the device): out[0] built, [1] overflowed, [2] face-list
+ * entries, [3] face-list entry capacity of the workspace, [4] builds enqueued by this process so far (all bodies). */
 int icon_sdf_brick_info(const void *mesh_ws, int V, int F, int64_t *out);
 
 /* Debug / parity tap: the SMPL block alone (cal_sdf_batch outputs before the outlier rule).

@@ -1,4 +1,4 @@
-"""Brick leaf lists of the dense SDF path (sdf.cu, DESIGN.md 4.2) against the brute-force kernel, bit for bit.
+"""Brick face lists of the dense SDF path (sdf.cu, DESIGN.md 4.2) against the brute-force kernel, bit for bit.
 
 The brick path only changes which faces a warp looks at, so rec (sdf, cmap, normal, vis) and the nearest face must
 equal icon_sdf_bruteforce exactly: on dense lattices, on warps that straddle bricks or leave the cube (tree walk),

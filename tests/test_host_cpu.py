@@ -37,6 +37,8 @@ def test_library_exports_every_declared_symbol(built_lib):
     assert _C.lib.icon_version() == 1
     # size queries are host-only and must work without a GPU
     assert _C.lib.icon_smpl_workspace_bytes(6890, 13776) > 13776 * 64
+    # an SMPL body's workspace holds its brick face lists but no leaf lists
+    assert _C.lib.icon_smpl_workspace_bytes(6890, 13776) < 64 << 20
     assert _C.lib.icon_query_workspace_bytes(1 << 20, 13776, 0) > (1 << 20) * 32
     assert _C.lib.icon_mc_workspace_bytes(257, 1) >= 258 ** 3 * 6        # voff i32 + flags + case per voxel
     assert _C.lib.icon_voxelize_workspace_bytes(128) >= 128 ** 3

@@ -57,7 +57,8 @@ def main():
             builds.append(first - again)
     info = ops.sdf_brick_info(b)
     out["build_ms"] = {"median": median(builds), "min": min(builds), "max": max(builds)}
-    out["lists"] = {"entries": info["entries"], "list_bytes": 2 * info["entries"], "overflow": info["overflow"],
+    # a face-list entry is a uint16 face position and a float key
+    out["lists"] = {"entries": info["entries"], "list_bytes": 6 * info["entries"], "overflow": info["overflow"],
                     "workspace_bytes": int(b.ws.numel())}
     ops.set_sdf_policy(0)
     b = body(dev, 0)
