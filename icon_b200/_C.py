@@ -37,6 +37,7 @@ _SIGS = {
     "icon_set_sdf_policy": (_i, [_i, _i64, _i64]),
     "icon_set_sdf_bricks": (_i, [_i, _i64]),
     "icon_sdf_brick_info": (_i, [_vp, _i, _i, _vp]),
+    "icon_sdf_brick_lists": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "icon_sdf_only": (_i, [_vp, _i64, _i64, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "icon_sdf_bruteforce": (_i, [_vp, _i64, _i64, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "icon_mesh_workspace_bytes": (_sz, [_i, _i]),

@@ -22,6 +22,7 @@
 #include <mutex>
 #include <type_traits>
 #include <unordered_set>
+#include <vector>
 
 #include "common.cuh"
 #include "face_tree.cuh"
@@ -772,6 +773,39 @@ extern "C" int icon_sdf_brick_info(const void *mesh_ws, int V, int F, int64_t *o
     {
         std::lock_guard<std::mutex> lk(icon::g_brick_mu);
         out[4] = icon::g_brick_builds;
+    }
+    return ICON_OK;
+}
+
+extern "C" int icon_sdf_brick_lists(const void *mesh_ws, int V, int F, int64_t *dims, int32_t *foff, int32_t *flist,
+                                    float *fkey, float *bub, int32_t *bface, float *sph) {
+    ICON_CHECK_ARG(mesh_ws && dims && V > 0 && F > 0, "icon_sdf_brick_lists: bad argument");
+    MeshView m = mesh_view(mesh_ws, V, F);
+    MeshHeader h;
+    int32_t total = 0;
+    ICON_CUDA(cudaDeviceSynchronize());
+    ICON_CUDA(cudaMemcpy(&h, m.hdr, sizeof(h), cudaMemcpyDeviceToHost));
+    ICON_CHECK_ARG(h.brick_built, "icon_sdf_brick_lists: the body's brick lists are not built");
+    ICON_CHECK_ARG(!h.brick_overflow, "icon_sdf_brick_lists: the body's brick lists overflowed");
+    ICON_CUDA(cudaMemcpy(&total, m.foff + NBRICK, sizeof(total), cudaMemcpyDeviceToHost));
+    dims[0] = BRICK_AX;
+    dims[1] = total;
+    if (!foff && !flist && !fkey && !bub && !bface && !sph) return ICON_OK;
+    ICON_CHECK_ARG(foff && flist && fkey && bub && bface && sph, "icon_sdf_brick_lists: null array");
+    std::vector<int32_t> order((size_t)F);
+    std::vector<unsigned short> pos((size_t)total);
+    std::vector<float4> sph_s((size_t)F);
+    ICON_CUDA(cudaMemcpy(order.data(), m.order, sizeof(int32_t) * F, cudaMemcpyDeviceToHost));
+    ICON_CUDA(cudaMemcpy(pos.data(), m.flist, sizeof(unsigned short) * total, cudaMemcpyDeviceToHost));
+    ICON_CUDA(cudaMemcpy(sph_s.data(), m.sph_s, sizeof(float4) * F, cudaMemcpyDeviceToHost));
+    ICON_CUDA(cudaMemcpy(foff, m.foff, sizeof(int32_t) * (NBRICK + 1), cudaMemcpyDeviceToHost));
+    ICON_CUDA(cudaMemcpy(fkey, m.fkey, sizeof(float) * total, cudaMemcpyDeviceToHost));
+    ICON_CUDA(cudaMemcpy(bub, m.bub, sizeof(float) * NBRICK, cudaMemcpyDeviceToHost));
+    ICON_CUDA(cudaMemcpy(bface, m.bface, sizeof(int32_t) * NBRICK, cudaMemcpyDeviceToHost));
+    for (int32_t i = 0; i < total; ++i) flist[i] = order[pos[i]];
+    for (int k = 0; k < F; ++k) {
+        float *s = sph + 4 * (size_t)order[k];
+        s[0] = sph_s[k].x; s[1] = sph_s[k].y; s[2] = sph_s[k].z; s[3] = sph_s[k].w;
     }
     return ICON_OK;
 }

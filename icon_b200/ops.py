@@ -206,6 +206,25 @@ def sdf_brick_info(body):
     return dict(zip(("built", "overflow", "entries", "capacity", "builds"), (int(v) for v in out)))
 
 
+def sdf_brick_lists(body):
+    """A built body's brick face lists as CPU tensors (include/icon_b200.h: icon_sdf_brick_lists; a diagnostic tap):
+    brick_ax (bricks per axis; brick b = (bz * A + by) * A + bx), foff [B+1], flist [E] original face ids, fkey [E],
+    bub [B], bface [B] and sph [F,4], the per-face bounding spheres the keys were computed from.  Raises IconError when
+    the lists are not built or overflowed."""
+    dims = (ctypes.c_int64 * 2)()
+    args = (_p(body.ws), body.V, body.F, dims)
+    check(lib.icon_sdf_brick_lists(*args, *([None] * 6)), "icon_sdf_brick_lists")
+    A, E = int(dims[0]), int(dims[1])
+    B = A ** 3
+    out = {"foff": torch.empty(B + 1, dtype=torch.int32), "flist": torch.empty(E, dtype=torch.int32),
+           "fkey": torch.empty(E, dtype=torch.float32), "bub": torch.empty(B, dtype=torch.float32),
+           "bface": torch.empty(B, dtype=torch.int32), "sph": torch.empty(body.F, 4, dtype=torch.float32)}
+    check(lib.icon_sdf_brick_lists(*args, *(_p(out[k]) for k in ("foff", "flist", "fkey", "bub", "bface", "sph"))),
+          "icon_sdf_brick_lists")
+    out["brick_ax"] = A
+    return out
+
+
 # --------------------------------------------------------------------------- query
 def _point_strides(points):
     """points [1,3,N] (any strides) -> (tensor, stride_c, stride_n, N) in elements."""

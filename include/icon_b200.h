@@ -142,6 +142,14 @@ int icon_set_sdf_bricks(int enable, int64_t max_entries);
 /* Brick list state of a prepared body (synchronises the device): out[0] built, [1] overflowed, [2] face-list
  * entries, [3] face-list entry capacity of the workspace, [4] builds enqueued by this process so far (all bodies). */
 int icon_sdf_brick_info(const void *mesh_ws, int V, int F, int64_t *out);
+/* Read-back of a prepared body's built brick lists (diagnostics; synchronises the device).  dims[0] = bricks per axis
+ * A, dims[1] = face-list entries E; with every array null only dims is written.  Host arrays, B = A^3 bricks, brick
+ * b = (bz * A + by) * A + bx: foff [B + 1] list offsets, flist [E] original face ids, fkey [E] their keys, bub [B] the
+ * bound on every point's nearest distance, bface [B] the face nearest each brick centre, sph [F][4] the bounding
+ * sphere (centre, radius) of each original face that the keys were computed from.  ICON_EINVAL when the lists are not
+ * built or overflowed. */
+int icon_sdf_brick_lists(const void *mesh_ws, int V, int F, int64_t *dims, int32_t *foff, int32_t *flist,
+                         float *fkey, float *bub, int32_t *bface, float *sph);
 
 /* Debug / parity tap: the SMPL block alone (cal_sdf_batch outputs before the outlier rule).
  * rec [N,8] f32 = sdf, cmap xyz, norm xyz, vis(0/1); face [N] i32 nearest face id. */
