@@ -40,6 +40,7 @@ _SIGS = {
     "icon_sdf_brick_lists": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "icon_sdf_only": (_i, [_vp, _i64, _i64, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "icon_sdf_bruteforce": (_i, [_vp, _i64, _i64, _i64, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "icon_face_tree_read": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
     "icon_mesh_workspace_bytes": (_sz, [_i, _i]),
     "icon_mesh_prepare": (_i, [_vp, _vp, _i, _i, _vp, _sz, _vp]),
     "icon_mesh_distance": (_i, [_vp, _i64, _vp, _i, _i, _vp, _vp, _vp]),

@@ -166,12 +166,19 @@ struct MeshHeader {                  // device-resident, written by icon_smpl_pr
     int pad;
 };
 
-// Morton-sorted per-face records and the implicit 4-ary AABB tree over them (face_tree.cuh builds and walks it)
+struct TreeBounds {                  // device-resident, written by face_tree_build
+    unsigned lo[3], hi[3];           // bounding box of the faces' corners, order-preserving float encoding
+    float absmax;                    // largest |coordinate| of that box (scale of the slacks of a mesh in any unit)
+};
+
+// Morton-sorted per-face records and the implicit 4-ary AABB tree over them (face_tree.cu builds it, face_tree.cuh
+// walks it)
 struct FaceTree {
     float4 *tri_s;        // [F][3] per-face records (a.xyz, ab.x) (ab.yz, ac.xy) (ac.z, -, -, -), sorted
     float4 *sph_s;        // [F] bounding spheres (centre xyz, radius), conservative, sorted
     int32_t *order;       // [F] sorted position -> original face id
     float4 *nodes;        // [total_nodes][2]: (min.xyz, -) (max.xyz, -), level 0 (leaves) first
+    TreeBounds *bounds;
     int F;
     int nlevels;
     int lvl_cnt[TREE_MAX_LEVELS];
@@ -180,12 +187,10 @@ struct FaceTree {
 
 struct MeshView : FaceTree {
     const float4 *tri;    // [F][3]: (a.xyz, ab.x) (ab.yz, ac.xy) (ac.z, -, -, -), original face order
-    const float4 *sph;    // [F]: bounding sphere (centre xyz, radius), conservative
     const float4 *attr;   // [F][6]: normals 9, cmap 9, vis 3, pad 3
     const float4 *rbox;   // [F][2]: (ymin, ymax, zmin, zmax) (xmax, xmin, -, -)
     float *vnormals;      // [V][3] scratch
     void *vn_ws;          // area_vertex_normals' workspace
-    unsigned long long *keys;   // [F] morton << 32 | face: the sort keys of the tree
     // ray grid
     int32_t *rcount;      // [RAY_GRID^2 + 1]
     int32_t *roff;        // [RAY_GRID^2 + 1]

@@ -1,11 +1,13 @@
 // The Morton-sorted 4-ary AABB tree over a mesh's faces (FaceTree, common.cuh) and the exact nearest-face walk over
-// it, shared by the SMPL SDF block (sdf.cu, smpl.cu) and the distance-only mesh query (mesh_dist.cu).
+// it, shared by the SMPL SDF block (sdf.cu, smpl.cu), the distance-only mesh query (mesh_dist.cu) and the PRT ray cast
+// (prt.cu).  One builder, face_tree.cu, fills the tree for icon_smpl_prepare and icon_mesh_prepare alike.
 //
 // Like geom.cuh, this header is included only by translation units compiled with -fmad=false: the bounds below and the
 // exact distance are the same fp32 operations in every caller, fused multiply-adds only where fmaf() is written.
 //
-// Layout: face records (a, ab, ac) and bounding spheres in Morton order of the face centroids; leaves of 4 consecutive
-// faces, then parents of 4 consecutive nodes, level by level (leaves first, root last).
+// Layout: face records (a, ab, ac) and bounding spheres in Morton order of the face centroids (ties by face id), over
+// the frame the caller gives (TreeFrame); leaves of 4 consecutive faces, then parents of 4 consecutive nodes, level by
+// level (leaves first, root last).
 //
 // The walk (DESIGN.md 4.2): one warp serves PPW query points, each replicated on REP = 32 / PPW lanes that split the
 // candidate faces between them and merge by shuffle.
@@ -50,7 +52,16 @@ __device__ __forceinline__ float warp_min(float v) {
     return v;
 }
 
-// ---------------------------------------------------------------- building the tree
+// ---------------------------------------------------------------- building the tree (face_tree.cu)
+// The Morton frame and the sphere slack of a tree.  SMPL bodies in the query frame take the fixed cube
+// [-1.5, 1.5)^3 and the plain 1e-7 slack; any other mesh, in any unit, its own bounding cube and a slack scaled by its
+// largest |coordinate|.
+struct TreeFrame {
+    bool fit;                          // codes over the mesh's bounding cube, else over [lo, lo + 1024 / scale)^3
+    float lo, scale;
+    bool scaled_slack;                 // sphere slack 1e-7 max(1, absmax), else 1e-7
+};
+
 // level sizes and offsets of a tree over F faces; returns the total node count
 static inline size_t tree_levels(FaceTree &t, int F) {
     t.F = F;
@@ -78,20 +89,8 @@ __device__ __forceinline__ unsigned morton30(V3 p, V3 lo, float s) {
     return (expand10(qz(p.x, lo.x)) << 2) | (expand10(qz(p.y, lo.y)) << 1) | expand10(qz(p.z, lo.z));
 }
 
-// record (a, ab, ac) and bounding sphere (centroid, largest corner distance inflated by 1.0001 and `slack`: only a
-// conservative lower bound for pruning, never a reported distance) of the face (a, b, c); returns the centroid
-__device__ __forceinline__ V3 write_face_record(V3 a, V3 b, V3 c, float slack, float4 *__restrict__ tri,
-                                                float4 *__restrict__ sph) {
-    const V3 ab = sub3(b, a), ac = sub3(c, a);
-    const V3 sc = mk3((a.x + b.x + c.x) / 3.f, (a.y + b.y + c.y) / 3.f, (a.z + b.z + c.z) / 3.f);
-    const float ra = dot3(sub3(a, sc), sub3(a, sc)), rb = dot3(sub3(b, sc), sub3(b, sc)),
-                rc = dot3(sub3(c, sc), sub3(c, sc));
-    const float sr = sqrtf(fmaxf(ra, fmaxf(rb, rc))) * 1.0001f + slack;
-    tri[0] = make_float4(a.x, a.y, a.z, ab.x);
-    tri[1] = make_float4(ab.y, ab.z, ac.x, ac.y);
-    tri[2] = make_float4(ac.z, 0.f, 0.f, 0.f);
-    *sph = make_float4(sc.x, sc.y, sc.z, sr);
-    return sc;
+__device__ __forceinline__ V3 centroid(V3 a, V3 b, V3 c) {
+    return mk3((a.x + b.x + c.x) / 3.f, (a.y + b.y + c.y) / 3.f, (a.z + b.z + c.z) / 3.f);
 }
 
 // box of leaf n (its 4 sorted faces, corners a, a + ab, a + ac as the distance code forms them)
@@ -124,9 +123,33 @@ __device__ __forceinline__ void write_parent_box(const FaceTree &t, int l, int n
     t.nodes[2 * ((size_t)t.lvl_off[l] + n) + 1] = hi;
 }
 
-// the tree of a workspace icon_mesh_prepare filled, and the device address of the mesh's largest |coordinate|
-// (defined in mesh_dist.cu; the PRT ray walk of prt.cu reads the same tree)
-FaceTree mesh_ws_tree(const void *mesh_ws, int V, int F, const float **absmax);
+// The tree's arrays, then its build scratch: a workspace that holds a tree begins with them
+struct TreeWs {
+    FaceTree t;
+    unsigned long long *keys, *keys_b;  // [F] morton << 32 | face: original order, then grouped by bucket
+    int32_t *bcount, *boff;            // bucket counts / offsets (top 18 code bits)
+    void *scan_ws;
+};
+TreeWs face_tree_carve(Carver &c, int F);
+FaceTree face_tree_view(const void *ws, int F);
+// fills the tree at the start of `ws` from verts [V,3] f32, faces [F,3] i64 (stream-ordered)
+int face_tree_build(void *ws, const float *verts, const int64_t *faces, int F, TreeFrame frame, cudaStream_t stream);
+
+__device__ __forceinline__ void load_face(const float *__restrict__ verts, const int64_t *__restrict__ faces, int64_t f,
+                                          V3 &a, V3 &b, V3 &c) {
+    const int64_t i0 = faces[3 * f], i1 = faces[3 * f + 1], i2 = faces[3 * f + 2];
+    a = mk3(verts[3 * i0], verts[3 * i0 + 1], verts[3 * i0 + 2]);
+    b = mk3(verts[3 * i1], verts[3 * i1 + 1], verts[3 * i1 + 2]);
+    c = mk3(verts[3 * i2], verts[3 * i2 + 1], verts[3 * i2 + 2]);
+}
+
+// record (a, ab, ac) of the face (a, b, c), as load_tri reads it
+__device__ __forceinline__ void write_tri(V3 a, V3 b, V3 c, float4 *__restrict__ tri) {
+    const V3 ab = sub3(b, a), ac = sub3(c, a);
+    tri[0] = make_float4(a.x, a.y, a.z, ab.x);
+    tri[1] = make_float4(ab.y, ab.z, ac.x, ac.y);
+    tri[2] = make_float4(ac.z, 0.f, 0.f, 0.f);
+}
 
 // ---------------------------------------------------------------- the walk
 struct ChunkSmem {                     // phase C's staging area, one per warp

@@ -5,10 +5,10 @@
 //   trimesh.proximity.closest_point  -> icon_mesh_distance: exact squared distance + lowest-index nearest face
 //   trimesh.sample.sample_surface_even -> icon_mesh_sample: area-weighted candidates, greedy radius removal
 //
-// Any triangle mesh (no cmap / vis / normals, no sign): icon_mesh_prepare builds the same per-face records and
-// Morton-sorted 4-ary AABB tree as icon_smpl_prepare (face_tree.cuh), but with 32-bit ids, so F is bounded by memory
-// only.  The Morton code is taken over the mesh's own bounding cube (the SMPL tree uses the fixed [-1.5, 1.5]^3 of a
-// body in the query frame), its sort is a bucket sort and rank.
+// Any triangle mesh (no cmap / vis / normals, no sign): icon_mesh_prepare builds the face tree with the same builder
+// as icon_smpl_prepare (face_tree.cu), over the mesh's own bounding cube and with the sphere slack scaled by its
+// largest |coordinate|; the walk uses 32-bit ids, so F is bounded by memory only.  The rest of the prepare is the
+// sampler's: the largest face area, the fixed-point area weights and their uint64 prefix sum.
 //
 // k_mesh_dist runs face_tree.cuh's walk at one query point per warp (PPW = 1): the query sets are sparse (1000 samples
 // on a mesh), so the warp box is the point and the 32 lanes split the candidate faces.  The frontier holds 1024
@@ -26,29 +26,20 @@
 
 namespace icon {
 
-constexpr int GM_BUCKET_BITS = 18;           // sort buckets: the top 18 of the 30 Morton bits
-constexpr int GM_NBUCKET = 1 << GM_BUCKET_BITS;
 constexpr int GM_T = 128;                    // 4 warps per block, one query point per warp
 constexpr int GM_FR_CAP = 1024;              // frontier capacity per warp (node / leaf ids)
 constexpr int GM_SAMPLE_MAX = 8192;          // most samples icon_mesh_sample keeps (shared memory of the removal pass)
 constexpr int S64_T = 256, S64_I = 8, S64_B = S64_T * S64_I;   // uint64 inclusive scan: elements per block
 
 struct GMeshHeader {                         // device-resident, written by icon_mesh_prepare
-    unsigned lo[3], hi[3];                   // bounding box, order-preserving float encoding (atomicMin / atomicMax)
     unsigned long long amax;                 // largest face area (fp64 bits; areas are >= 0 so bits order like values)
     unsigned long long total;                // sum of the fixed-point face weights (sampler)
     int wbits;                               // weight_f = floor(area_f / amax * 2^wbits)
-    float absmax;                            // largest |coordinate| of the mesh (scale of the bounds' slack)
 };
 
 struct GMesh : FaceTree {
     unsigned long long *wcum;                // [F] inclusive prefix sum of the face weights, original face order
     GMeshHeader *hdr;
-    // prepare scratch
-    unsigned long long *keys;                // [F] morton << 32 | face, original order
-    unsigned long long *keys_b;              // [F] the same, grouped by bucket
-    int32_t *bcount, *boff;                  // [GM_NBUCKET + 1]
-    void *scan_ws;                           // int32 bucket scan
     unsigned long long *s64_ws;              // block totals of the uint64 scan
     int V;
 };
@@ -64,19 +55,10 @@ static size_t s64_ws_elems(int64_t n) {
 
 static GMesh carve_gmesh(Carver &c, int V, int F) {
     GMesh m{};
+    static_cast<FaceTree &>(m) = face_tree_carve(c, F).t;     // first: icon_face_tree_read finds it there
     m.V = V;
-    const size_t total_nodes = tree_levels(m, F);
-    m.tri_s = c.take<float4>((size_t)F * 3);
-    m.sph_s = c.take<float4>((size_t)F);
-    m.order = c.take<int32_t>((size_t)F);
-    m.nodes = c.take<float4>(total_nodes * 2);
     m.wcum = c.take<unsigned long long>((size_t)F);
     m.hdr = c.take<GMeshHeader>(1);
-    m.keys = c.take<unsigned long long>((size_t)F);
-    m.keys_b = c.take<unsigned long long>((size_t)F);
-    m.bcount = c.take<int32_t>(GM_NBUCKET + 1);
-    m.boff = c.take<int32_t>(GM_NBUCKET + 1);
-    m.scan_ws = c.take<char>(scan_ws_bytes(GM_NBUCKET + 1));
     m.s64_ws = c.take<unsigned long long>(s64_ws_elems(F));
     return m;
 }
@@ -87,132 +69,45 @@ static size_t gmesh_ws_bytes(int V, int F) {
     return c.total();
 }
 
-// ---------------------------------------------------------------- prepare
-__device__ __forceinline__ unsigned f2ord(float v) {
-    const unsigned b = __float_as_uint(v);
-    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float ord2f(unsigned u) {
-    return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
-
-__device__ __forceinline__ void load_face(const float *__restrict__ verts, const int64_t *__restrict__ faces, int64_t f,
-                                          V3 &a, V3 &b, V3 &c) {
-    const int64_t i0 = faces[3 * f], i1 = faces[3 * f + 1], i2 = faces[3 * f + 2];
-    a = mk3(verts[3 * i0], verts[3 * i0 + 1], verts[3 * i0 + 2]);
-    b = mk3(verts[3 * i1], verts[3 * i1 + 1], verts[3 * i1 + 2]);
-    c = mk3(verts[3 * i2], verts[3 * i2 + 1], verts[3 * i2 + 2]);
-}
-
+// ---------------------------------------------------------------- prepare: the sampler's area weights
 __global__ void k_gm_init(GMeshHeader *h, int wbits) {
-    for (int k = 0; k < 3; ++k) { h->lo[k] = 0xffffffffu; h->hi[k] = 0u; }
     h->amax = 0ull;
     h->total = 0ull;
     h->wbits = wbits;
-    h->absmax = 0.f;
 }
 
-// bounding box of the referenced vertices + largest face area (trimesh's area_faces: |(b - a) x (c - a)| / 2 in fp64)
-__global__ void __launch_bounds__(256) k_gm_bounds(const float *__restrict__ verts, const int64_t *__restrict__ faces,
-                                                   int F, GMeshHeader *h) {
+// trimesh's area_faces: |(b - a) x (c - a)| / 2 in fp64
+__device__ __forceinline__ double face_area(V3 a, V3 b, V3 c) {
+    const double abx = (double)b.x - (double)a.x, aby = (double)b.y - (double)a.y, abz = (double)b.z - (double)a.z;
+    const double acx = (double)c.x - (double)a.x, acy = (double)c.y - (double)a.y, acz = (double)c.z - (double)a.z;
+    const double cx = aby * acz - abz * acy, cy = abz * acx - abx * acz, cz = abx * acy - aby * acx;
+    return sqrt(cx * cx + cy * cy + cz * cz) * 0.5;
+}
+
+// largest face area
+__global__ void __launch_bounds__(256) k_gm_area(const float *__restrict__ verts, const int64_t *__restrict__ faces,
+                                                 int F, GMeshHeader *h) {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned lo[3] = {0xffffffffu, 0xffffffffu, 0xffffffffu}, hi[3] = {0u, 0u, 0u};
     double area = 0.0;
     if (f < F) {
         V3 a, b, c;
         load_face(verts, faces, f, a, b, c);
-        const float xs[3][3] = {{a.x, b.x, c.x}, {a.y, b.y, c.y}, {a.z, b.z, c.z}};
-        for (int k = 0; k < 3; ++k)
-            for (int j = 0; j < 3; ++j) { lo[k] = min(lo[k], f2ord(xs[k][j])); hi[k] = max(hi[k], f2ord(xs[k][j])); }
-        const double abx = (double)b.x - (double)a.x, aby = (double)b.y - (double)a.y, abz = (double)b.z - (double)a.z;
-        const double acx = (double)c.x - (double)a.x, acy = (double)c.y - (double)a.y, acz = (double)c.z - (double)a.z;
-        const double cx = aby * acz - abz * acy, cy = abz * acx - abx * acz, cz = abx * acy - aby * acx;
-        area = sqrt(cx * cx + cy * cy + cz * cz) * 0.5;
+        area = face_area(a, b, c);
     }
-    for (int o = 16; o; o >>= 1) {
-        for (int k = 0; k < 3; ++k) {
-            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
-            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
-        }
-        area = fmax(area, __shfl_xor_sync(0xffffffffu, area, o));
-    }
-    if ((threadIdx.x & 31) == 0) {
-        for (int k = 0; k < 3; ++k) { atomicMin(&h->lo[k], lo[k]); atomicMax(&h->hi[k], hi[k]); }
-        atomicMax(&h->amax, (unsigned long long)__double_as_longlong(area));
-    }
+    for (int o = 16; o; o >>= 1) area = fmax(area, __shfl_xor_sync(0xffffffffu, area, o));
+    if ((threadIdx.x & 31) == 0) atomicMax(&h->amax, (unsigned long long)__double_as_longlong(area));
 }
 
-__device__ __forceinline__ V3 centroid(V3 a, V3 b, V3 c) {
-    return mk3((a.x + b.x + c.x) / 3.f, (a.y + b.y + c.y) / 3.f, (a.z + b.z + c.z) / 3.f);
-}
-
-// per face: 30-bit Morton code of the centroid over the mesh's bounding cube, its sort bucket, and the fixed-point
-// sampling weight
-__global__ void __launch_bounds__(256) k_gm_keys(const float *__restrict__ verts, const int64_t *__restrict__ faces,
-                                                 GMesh m) {
+// per face: the fixed-point sampling weight, the area relative to the largest in wbits bits
+__global__ void __launch_bounds__(256) k_gm_weights(const float *__restrict__ verts, const int64_t *__restrict__ faces,
+                                                    GMesh m) {
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= m.F) return;
     const GMeshHeader *h = m.hdr;
     V3 a, b, c;
     load_face(verts, faces, f, a, b, c);
-    const float lx = ord2f(h->lo[0]), ly = ord2f(h->lo[1]), lz = ord2f(h->lo[2]);
-    const float ext = fmaxf(fmaxf(ord2f(h->hi[0]) - lx, ord2f(h->hi[1]) - ly), ord2f(h->hi[2]) - lz);
-    const float s = ext > 0.f ? 1024.f / ext : 0.f;
-    if (f == 0)
-        m.hdr->absmax = fmaxf(fmaxf(fmaxf(fabsf(lx), fabsf(ly)), fabsf(lz)),
-                              fmaxf(fmaxf(fabsf(ord2f(h->hi[0])), fabsf(ord2f(h->hi[1]))), fabsf(ord2f(h->hi[2]))));
-    const unsigned code = morton30(centroid(a, b, c), mk3(lx, ly, lz), s);
-    m.keys[f] = ((unsigned long long)code << 32) | (unsigned)f;
-    atomicAdd(&m.bcount[code >> (30 - GM_BUCKET_BITS)], 1);
-    // weight: the same fp64 area as k_gm_bounds, relative to the largest, in wbits fixed-point bits
-    const double abx = (double)b.x - (double)a.x, aby = (double)b.y - (double)a.y, abz = (double)b.z - (double)a.z;
-    const double acx = (double)c.x - (double)a.x, acy = (double)c.y - (double)a.y, acz = (double)c.z - (double)a.z;
-    const double cx = aby * acz - abz * acy, cy = abz * acx - abx * acz, cz = abx * acy - aby * acx;
-    const double area = sqrt(cx * cx + cy * cy + cz * cz) * 0.5;
     const double amax = __longlong_as_double((long long)h->amax);
-    m.wcum[f] = amax > 0.0 ? (unsigned long long)ldexp(area / amax, h->wbits) : 0ull;
-}
-
-__global__ void __launch_bounds__(256) k_gm_scatter(GMesh m, int32_t *__restrict__ cursor) {
-    const int f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= m.F) return;
-    const unsigned long long k = m.keys[f];
-    const int b = (int)(k >> (62 - GM_BUCKET_BITS));
-    m.keys_b[m.boff[b] + atomicAdd(&cursor[b], 1)] = k;
-}
-
-// rank within the bucket: keys are unique (the face id is in the low word), so the order is (Morton code, face id)
-// whatever order the scatter's atomics left the bucket in
-__global__ void __launch_bounds__(256) k_gm_rank(GMesh m) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m.F) return;
-    const unsigned long long k = m.keys_b[i];
-    const int b = (int)(k >> (62 - GM_BUCKET_BITS));
-    const int o0 = m.boff[b], o1 = m.boff[b + 1];
-    int r = 0;
-    for (int j = o0; j < o1; ++j) r += m.keys_b[j] < k;
-    m.order[o0 + r] = (int32_t)(k & 0xffffffffull);
-}
-
-// sorted records: tri / sphere as k_face_records (smpl.cu) computes them, the sphere's additive slack scaled by the
-// mesh's coordinate magnitude (the same 1e-7 for |coordinates| <= 1)
-__global__ void __launch_bounds__(256) k_gm_records(const float *__restrict__ verts, const int64_t *__restrict__ faces,
-                                                    GMesh m) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= m.F) return;
-    V3 a, b, c;
-    load_face(verts, faces, m.order[p], a, b, c);
-    write_face_record(a, b, c, 1e-7f * fmaxf(1.f, m.hdr->absmax), m.tri_s + 3 * (size_t)p, m.sph_s + p);
-}
-
-__global__ void __launch_bounds__(256) k_gm_leaves(GMesh m) {
-    const int n = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n < m.lvl_cnt[0]) write_leaf_box(m, n);
-}
-
-__global__ void __launch_bounds__(256) k_gm_level(GMesh m, int l) {
-    const int n = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n < m.lvl_cnt[l]) write_parent_box(m, l, n);
+    m.wcum[f] = amax > 0.0 ? (unsigned long long)ldexp(face_area(a, b, c) / amax, h->wbits) : 0ull;
 }
 
 // ---- inclusive uint64 prefix sum (the weights' cumulative sum): integer, so exact and independent of block order
@@ -263,13 +158,6 @@ static int scan64_inclusive(unsigned long long *x, int64_t n, unsigned long long
 
 __global__ void k_gm_total(GMesh m) { m.hdr->total = m.wcum[m.F - 1]; }
 
-FaceTree mesh_ws_tree(const void *mesh_ws, int V, int F, const float **absmax) {
-    Carver c((void *)mesh_ws);
-    GMesh m = carve_gmesh(c, V, F);
-    *absmax = &m.hdr->absmax;
-    return m;
-}
-
 // ---------------------------------------------------------------- nearest face, one point per warp
 using MeshDistSmem = WalkSmem<int32_t, GM_FR_CAP>;
 
@@ -282,7 +170,7 @@ __global__ void __launch_bounds__(GM_T) k_mesh_dist(const float *__restrict__ pt
     // the SMPL path's additive slacks (1e-6 on lengths, 1e-7 on the support bound) are sized for coordinates of
     // magnitude <= 1; a general mesh may be in any unit, so they scale with the largest coordinate in play (the leaf
     // boxes are built from a + ab, which may sit an ulp of that magnitude away from the vertex)
-    const float sc = fmaxf(fmaxf(1.f, m.hdr->absmax), fmaxf(fmaxf(fabsf(p.x), fabsf(p.y)), fabsf(p.z)));
+    const float sc = fmaxf(fmaxf(1.f, m.bounds->absmax), fmaxf(fmaxf(fabsf(p.x), fabsf(p.y)), fabsf(p.z)));
     const float tol = 1e-6f * sc;
     NearestFace<1> nf(p, tol, 1e-7f * sc * sc);
     // one point: the warp's box is the point inflated by tol, its radius tol
@@ -410,31 +298,17 @@ extern "C" int icon_mesh_prepare(const float *verts, const int64_t *faces, int V
     }
     Carver c(mesh_ws);
     GMesh m = carve_gmesh(c, V, F);
+    int rc = face_tree_build(mesh_ws, verts, faces, F, TreeFrame{true, 0.f, 0.f, true}, stream);
+    if (rc) return rc;
     const unsigned nb = (unsigned)((F + 255) / 256);
     int wbits = 62;                                              // F * 2^wbits < 2^62: the weight sum fits
     for (int f = F; f; f >>= 1) --wbits;
     k_gm_init<<<1, 1, 0, stream>>>(m.hdr, wbits);
     ICON_LAUNCHED();
-    k_gm_bounds<<<nb, 256, 0, stream>>>(verts, faces, F, m.hdr);
+    k_gm_area<<<nb, 256, 0, stream>>>(verts, faces, F, m.hdr);
     ICON_LAUNCHED();
-    ICON_CUDA(cudaMemsetAsync(m.bcount, 0, sizeof(int32_t) * (GM_NBUCKET + 1), stream));
-    k_gm_keys<<<nb, 256, 0, stream>>>(verts, faces, m);
+    k_gm_weights<<<nb, 256, 0, stream>>>(verts, faces, m);
     ICON_LAUNCHED();
-    int rc = scan_exclusive_i32(m.bcount, m.boff, GM_NBUCKET + 1, nullptr, m.scan_ws, stream);
-    if (rc) return rc;
-    ICON_CUDA(cudaMemsetAsync(m.bcount, 0, sizeof(int32_t) * (GM_NBUCKET + 1), stream));   // reuse as cursor
-    k_gm_scatter<<<nb, 256, 0, stream>>>(m, m.bcount);
-    ICON_LAUNCHED();
-    k_gm_rank<<<nb, 256, 0, stream>>>(m);
-    ICON_LAUNCHED();
-    k_gm_records<<<nb, 256, 0, stream>>>(verts, faces, m);
-    ICON_LAUNCHED();
-    k_gm_leaves<<<(unsigned)((m.lvl_cnt[0] + 255) / 256), 256, 0, stream>>>(m);
-    ICON_LAUNCHED();
-    for (int l = 1; l < m.nlevels; ++l) {
-        k_gm_level<<<(unsigned)((m.lvl_cnt[l] + 255) / 256), 256, 0, stream>>>(m, l);
-        ICON_LAUNCHED();
-    }
     rc = scan64_inclusive(m.wcum, F, m.s64_ws, stream);
     if (rc) return rc;
     k_gm_total<<<1, 1, 0, stream>>>(m);

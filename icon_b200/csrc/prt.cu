@@ -167,8 +167,8 @@ extern "C" int icon_prt(const void *mesh_ws, int Vm, int F, const double *origin
     const int W = (D + 31) / 32;
     const int n = (int)llround(sqrt((double)D));
     const int B = n * n == D ? n : D;                            // the reference's block of n directions
-    const float *absmax = nullptr;
-    const FaceTree t = mesh_ws_tree(mesh_ws, Vm, F, &absmax);
+    const FaceTree t = face_tree_view(mesh_ws, F);
+    const float *absmax = &t.bounds->absmax;
     for (int v0 = 0; v0 < V; v0 += chunk) {
         const int nv = std::min(chunk, V - v0);
         uint32_t *bits = hit_bits ? hit_bits + (size_t)v0 * W : (uint32_t *)ws;

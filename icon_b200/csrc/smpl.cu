@@ -1,5 +1,6 @@
-// SMPL body preparation: vertex normals (normals.cu's area-weighted rule), per-face records, Morton-ordered implicit
-// AABB tree and the yz ray grid.  Compiled with -fmad=false.
+// SMPL body preparation: vertex normals (normals.cu's area-weighted rule), per-face records in original order, the
+// face tree (face_tree.cu, over the fixed cube [-1.5, 1.5)^3 of a body in the query frame) and the yz ray grid.
+// Compiled with -fmad=false.
 //
 // Replaces the per-query preamble of cal_sdf_batch (lib/dataset/mesh_util.py:367-372):
 //   normals = Meshes(verts, faces).verts_normals_padded()          (pytorch3d)
@@ -17,17 +18,11 @@ namespace icon {
 
 static MeshView carve_mesh(Carver &c, int V, int F) {
     MeshView m{};
+    static_cast<FaceTree &>(m) = face_tree_carve(c, F).t;     // first: icon_face_tree_read finds it there
     m.V = V;
-    const size_t total_nodes = tree_levels(m, F);
     m.tri = c.take<float4>((size_t)F * 3);
-    m.sph = c.take<float4>((size_t)F);
     m.attr = c.take<float4>((size_t)F * 6);
     m.rbox = c.take<float4>((size_t)F * 2);
-    m.keys = c.take<unsigned long long>((size_t)F);
-    m.order = c.take<int32_t>((size_t)F);
-    m.tri_s = c.take<float4>((size_t)F * 3);
-    m.sph_s = c.take<float4>((size_t)F);
-    m.nodes = c.take<float4>(total_nodes * 2);
     m.rcount = c.take<int32_t>(RAY_GRID * RAY_GRID + 1);
     m.roff = c.take<int32_t>(RAY_GRID * RAY_GRID + 1);
     m.rlist = c.take<int32_t>((size_t)F * RAY_LIST_PER_FACE);
@@ -61,15 +56,13 @@ MeshView mesh_view(const void *ws, int V, int F) {
 __global__ void k_face_records(const float *__restrict__ verts, const int64_t *__restrict__ faces,
                                const float *__restrict__ vnormals, const float *__restrict__ cmap,
                                const float *__restrict__ vis, int F, float4 *__restrict__ tri,
-                               float4 *__restrict__ sph, float4 *__restrict__ attr, float4 *__restrict__ rbox,
-                               unsigned long long *__restrict__ keys) {
+                               float4 *__restrict__ attr, float4 *__restrict__ rbox) {
     int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= F) return;
     int64_t i0 = faces[3 * f], i1 = faces[3 * f + 1], i2 = faces[3 * f + 2];
-    V3 a = mk3(verts[3 * i0], verts[3 * i0 + 1], verts[3 * i0 + 2]);
-    V3 b = mk3(verts[3 * i1], verts[3 * i1 + 1], verts[3 * i1 + 2]);
-    V3 c = mk3(verts[3 * i2], verts[3 * i2 + 1], verts[3 * i2 + 2]);
-    const V3 sc = write_face_record(a, b, c, 1e-7f, tri + 3 * f, sph + f);
+    V3 a, b, c;
+    load_face(verts, faces, f, a, b, c);
+    write_tri(a, b, c, tri + 3 * f);
     const float *n0 = vnormals + 3 * i0, *n1 = vnormals + 3 * i1, *n2 = vnormals + 3 * i2;
     const float *m0 = cmap + 3 * i0, *m1 = cmap + 3 * i1, *m2 = cmap + 3 * i2;
     attr[6 * f + 0] = make_float4(n0[0], n0[1], n0[2], n1[0]);
@@ -81,61 +74,20 @@ __global__ void k_face_records(const float *__restrict__ verts, const int64_t *_
     rbox[2 * f + 0] = make_float4(fminf(a.y, fminf(b.y, c.y)), fmaxf(a.y, fmaxf(b.y, c.y)),
                                   fminf(a.z, fminf(b.z, c.z)), fmaxf(a.z, fmaxf(b.z, c.z)));
     rbox[2 * f + 1] = make_float4(fmaxf(a.x, fmaxf(b.x, c.x)), fminf(a.x, fminf(b.x, c.x)), 0.f, 0.f);
-    // Morton code of the centroid over [-1.5, 1.5]^3
-    keys[f] = ((unsigned long long)morton30(sc, mk3(-1.5f, -1.5f, -1.5f), 1024.f / 3.f) << 32) | (unsigned)f;
 }
 
-// rank sort: F is ~1e4, so F^2 comparisons from shared memory are cheaper than a radix sort's passes
-__global__ void __launch_bounds__(256) k_rank_sort(const unsigned long long *__restrict__ keys, int F,
-                                                   int32_t *__restrict__ order) {
-    __shared__ unsigned long long tile[1024];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned long long my = i < F ? keys[i] : 0ull;
-    int rank = 0;
-    for (int j0 = 0; j0 < F; j0 += 1024) {
-        const int n = min(1024, F - j0);
-        __syncthreads();
-        for (int k = threadIdx.x; k < n; k += 256) tile[k] = keys[j0 + k];
-        __syncthreads();
-        if (i < F)
-            for (int k = 0; k < n; ++k) rank += tile[k] < my;
-    }
-    if (i < F) order[rank] = i;
-}
-
-// sorted copies + leaf boxes (level 0), then the upper levels inside one CTA
-__global__ void k_sorted_copy(const int32_t *__restrict__ order, const float4 *__restrict__ tri,
-                              const float4 *__restrict__ sph, int F, float4 *__restrict__ tri_s,
-                              float4 *__restrict__ sph_s) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= F) return;
-    const int f = order[p];
-    tri_s[3 * p] = tri[3 * f]; tri_s[3 * p + 1] = tri[3 * f + 1]; tri_s[3 * p + 2] = tri[3 * f + 2];
-    float4 s = sph[f];
-    sph_s[p] = s;
-}
-
-__global__ void __launch_bounds__(1024) k_build_tree(MeshView m) {
-    for (int n = threadIdx.x; n < m.lvl_cnt[0]; n += blockDim.x) write_leaf_box(m, n);
-    for (int l = 1; l < m.nlevels; ++l) {
-        __threadfence_block();
-        __syncthreads();
-        for (int n = threadIdx.x; n < m.lvl_cnt[l]; n += blockDim.x) write_parent_box(m, l, n);
-    }
-    // ray grid frame from the root box
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const size_t root = (size_t)m.lvl_off[m.nlevels - 1];
-        float4 lo = m.nodes[2 * root], hi = m.nodes[2 * root + 1];
-        const float pad = 1e-3f;
-        MeshHeader h;
-        h.y0 = lo.y - pad; h.z0 = lo.z - pad;
-        h.inv_cy = (float)RAY_GRID / ((hi.y + pad) - h.y0);
-        h.inv_cz = (float)RAY_GRID / ((hi.z + pad) - h.z0);
-        h.ray_overflow = 0;
-        h.brick_built = h.brick_overflow = h.pad = 0;
-        *m.hdr = h;
-    }
+// ray grid frame from the tree's root box
+__global__ void k_ray_header(MeshView m) {
+    const size_t root = (size_t)m.lvl_off[m.nlevels - 1];
+    float4 lo = m.nodes[2 * root], hi = m.nodes[2 * root + 1];
+    const float pad = 1e-3f;
+    MeshHeader h;
+    h.y0 = lo.y - pad; h.z0 = lo.z - pad;
+    h.inv_cy = (float)RAY_GRID / ((hi.y + pad) - h.y0);
+    h.inv_cz = (float)RAY_GRID / ((hi.z + pad) - h.z0);
+    h.ray_overflow = 0;
+    h.brick_built = h.brick_overflow = h.pad = 0;
+    *m.hdr = h;
 }
 
 // ---- yz cell lists for the +x ray: a face is listed in every cell its (inflated) yz box overlaps
@@ -197,13 +149,11 @@ extern "C" int icon_smpl_prepare(const float *verts, const int64_t *faces, const
     int rc = area_vertex_normals(verts, V, faces, F, m.vnormals, m.vn_ws, stream);
     if (rc) return rc;
     k_face_records<<<(F + 127) / 128, 128, 0, stream>>>(verts, faces, m.vnormals, cmap, vis, F, (float4 *)m.tri,
-                                                        (float4 *)m.sph, (float4 *)m.attr, (float4 *)m.rbox, m.keys);
+                                                        (float4 *)m.attr, (float4 *)m.rbox);
     ICON_LAUNCHED();
-    k_rank_sort<<<(F + 255) / 256, 256, 0, stream>>>(m.keys, F, m.order);
-    ICON_LAUNCHED();
-    k_sorted_copy<<<(F + 127) / 128, 128, 0, stream>>>(m.order, m.tri, m.sph, F, m.tri_s, m.sph_s);
-    ICON_LAUNCHED();
-    k_build_tree<<<1, 1024, 0, stream>>>(m);
+    rc = face_tree_build(mesh_ws, verts, faces, F, TreeFrame{false, -1.5f, 1024.f / 3.f, false}, stream);
+    if (rc) return rc;
+    k_ray_header<<<1, 1, 0, stream>>>(m);
     ICON_LAUNCHED();
     ICON_CUDA(cudaMemsetAsync(m.rcount, 0, sizeof(int32_t) * (RAY_GRID * RAY_GRID + 1), stream));
     k_ray_count<<<(F + 127) / 128, 128, 0, stream>>>(m);

@@ -225,6 +225,23 @@ def sdf_brick_lists(body):
     return out
 
 
+def face_tree(mesh):
+    """The face tree of a prepared SmplBody or metrics.Mesh as CPU tensors (include/icon_b200.h: icon_face_tree_read; a
+    diagnostic tap): order [F] original face ids in sorted order, tri_s [F,12] records (a, ab, ac, 0 0 0), sph_s [F,4]
+    bounding spheres, nodes [N,2,4] boxes (min.xyz, 0) (max.xyz, 0), leaves first."""
+    n, N = mesh.F, 0
+    while True:
+        n = (n + 3) // 4
+        N += n
+        if n == 1:
+            break
+    out = {"order": torch.empty(mesh.F, dtype=torch.int32), "tri_s": torch.empty(mesh.F, 12),
+           "sph_s": torch.empty(mesh.F, 4), "nodes": torch.empty(N, 2, 4)}
+    check(lib.icon_face_tree_read(_p(mesh.ws), mesh.V, mesh.F, *(_p(out[k]) for k in ("order", "tri_s", "sph_s", "nodes"))),
+          "icon_face_tree_read")
+    return out
+
+
 # --------------------------------------------------------------------------- query
 def _point_strides(points):
     """points [1,3,N] (any strides) -> (tensor, stride_c, stride_n, N) in elements."""

@@ -53,9 +53,10 @@ int icon_profile_last_query(float *h_ms);
  * Replaces the per-call preamble of cal_sdf_batch, lib/dataset/mesh_util.py:367-372:
  * pytorch3d Meshes.verts_normals_padded (area-weighted vertex normals, deterministic
  * sequential-index_add order) and the four face_vertices gathers
- * (lib/common/render_utils.py:149-163).  Builds, into `mesh_ws`, per-face records
- * (a, ab, ac, bounding sphere), per-face attribute records (normals, cmap, vis at the three
- * corners) and the +x-ray culling boxes.  Done once per body, not once per query.
+ * (lib/common/render_utils.py:149-163).  Builds, into `mesh_ws`, the face tree (Morton-sorted
+ * records and bounding spheres, AABB levels), per-face records (a, ab, ac), per-face attribute
+ * records (normals, cmap, vis at the three corners) and the +x-ray culling boxes.  Done once per
+ * body, not once per query.
  * verts [V,3] f32, faces [F,3] i64, cmap [V,3] f32, vis [V] f32 (0/1). */
 size_t icon_smpl_workspace_bytes(int V, int F);
 int icon_smpl_prepare(const float *verts, const int64_t *faces, const float *cmap,
@@ -160,6 +161,12 @@ int icon_sdf_only(const float *points, int64_t stride_c, int64_t stride_n, int64
 int icon_sdf_bruteforce(const float *points, int64_t stride_c, int64_t stride_n, int64_t N,
                         const float *h_calib, const void *mesh_ws, int V, int F, float *rec,
                         int32_t *face, icon_stream_t stream);
+/* Read-back of the face tree at the start of a workspace icon_smpl_prepare or icon_mesh_prepare filled (diagnostics;
+ * synchronises the device).  Host arrays: order [F] original face id at each sorted position, tri_s [F][12] records
+ * (a.xyz, ab.xyz, ac.xyz, then 3 zeros) and sph_s [F][4] bounding spheres (centre, radius) in sorted order, nodes
+ * [N][2][4] boxes (min.xyz, 0) (max.xyz, 0), leaves first, N = sum over levels of the node counts ceil(F / 4),
+ * ceil(F / 16), ... down to 1. */
+int icon_face_tree_read(const void *mesh_ws, int V, int F, int32_t *order, float *tri_s, float *sph_s, float *nodes);
 /* ------------------------------------------------------------------ any triangle mesh: distance and sampling
  * The two trimesh calls of the benchmark's Chamfer / P2S metric (lib/dataset/Evaluator.py:200-230,
  * calculate_chamfer_p2s): trimesh.proximity.closest_point and trimesh.sample.sample_surface_even.

@@ -95,11 +95,13 @@ def box_dist(c, lo, hi):
     return np.sqrt((g * g).sum(-1))
 
 
-def leaf_boxes(v, f):
-    """Leaves of the body's tree as icon_smpl_prepare sorts them: 4 faces each, Morton order of the centroids."""
+def leaf_boxes(v, f, lo=np.float32(-1.5), scale=np.float32(1024) / np.float32(3)):
+    """Leaves of a mesh's face tree: 4 faces each, in Morton order of the float32 centroids over the cube
+    [lo, lo + 1024 / scale)^3 (default: the fixed cube of an SMPL body), codes clamped and truncated like morton30
+    (face_tree.cuh), ties by face id.  Returns the order and the leaves' boxes over the faces' vertices (float64)."""
     tri = v[f]                                                          # float32 [F,3,3]
     cen = (tri[:, 0] + tri[:, 1] + tri[:, 2]) / np.float32(3)
-    q = np.clip((cen.astype(np.float32) + np.float32(1.5)) * np.float32(1024.0 / 3.0), 0, 1023).astype(np.uint64)
+    q = np.clip((cen.astype(np.float32) - lo) * scale, 0, 1023).astype(np.uint64)
 
     def expand(x):
         out = np.zeros_like(x)

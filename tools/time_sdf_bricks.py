@@ -1,4 +1,5 @@
-"""Brick lists of the dense SDF path: build cost, list size, and sdf_only with the path on / off (alternating).
+"""Body preparation and the brick lists of the dense SDF path: SmplBody construction time on the 13,776-face body and a
+68k-face one, brick-list build cost, list size, and sdf_only with the path on / off (alternating).
 
     python tools/time_sdf_bricks.py [--reps 5]
 
@@ -17,10 +18,14 @@ from icon_b200 import ops, synthetic as S  # noqa: E402
 EYE = torch.eye(4)[None]
 
 
-def body(dev, seed=0):
-    v, f = S.body_mesh(seed=seed)
+def body_arrays(dev, seed=0, **mesh):
+    v, f = S.body_mesh(seed=seed, **mesh)
     cm, vi = S.body_attributes(v, seed=seed)
-    return ops.SmplBody(*(torch.from_numpy(a)[None].to(dev) for a in (v, f, cm, vi)))
+    return [torch.from_numpy(a)[None].to(dev) for a in (v, f, cm, vi)]
+
+
+def body(dev, seed=0):
+    return ops.SmplBody(*body_arrays(dev, seed))
 
 
 def ms(fn, reps=1):
@@ -46,6 +51,12 @@ def main():
     out = {"gpu": torch.cuda.get_device_name(dev)}
     ops.set_sdf_policy(32)
     ops.set_sdf_bricks(True)
+    out["prepare_ms"] = {}
+    for name, mesh in (("faces_13776", {}), ("faces_68k", {"rings": 200, "segs": 170})):
+        arrs = body_arrays(dev, 0, **mesh)
+        ms(lambda: ops.SmplBody(*arrs), 2)                                  # warm-up
+        t = [ms(lambda: ops.SmplBody(*arrs)) for _ in range(4 * args.reps)]
+        out["prepare_ms"][name] = {"F": int(arrs[1].shape[1]), "median": median(t), "min": min(t), "max": max(t)}
     tiny = S.lattice_points(4).permute(0, 2, 1).contiguous().to(dev)       # 64 points: the call is the build
     builds = []
     for seed in range(args.reps + 1):
