@@ -133,6 +133,11 @@ _SIGS = {
     "icon_mc_workspace_bytes": (_sz, [_i, _i]),
     "icon_mc_count": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _sz, _vp, _vp]),
     "icon_mc_emit": (_i, [_vp, _i, ctypes.c_double, _i, _vp, _vp, _vp, _i64, _i64, _vp]),
+    "icon_garment_labels_workspace_bytes": (_sz, [_i]),
+    "icon_garment_labels": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    "icon_garment_face_mask_workspace_bytes": (_sz, [_i, _i]),
+    "icon_garment_face_mask": (_i, [_vp, _i, _vp, _i, _vp, ctypes.c_uint32, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz,
+                                    _vp]),
 }
 
 EXPORTS = tuple(_SIGS.keys())

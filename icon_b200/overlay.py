@@ -26,7 +26,7 @@ GL renderers `PRTRender` / `ColorRender` / `initialize_GL_context`,
               `lib/dataset/TestDataset.py` an `__init__` that rebinds `get_rgb_image` / `get_silhouette_image` /
               `VF2Mesh` on the instance's `self.render` only, `lbs` in `lib/smplx/body_models.py`, `SMPLX` in
               `lib/pixielib/models/SMPLX.py`: the same class, its `forward` patched to run on the kernels,
-              `computePRT` in `lib/renderer/prt_util.py`), so
+              `computePRT` in `lib/renderer/prt_util.py`, `extract_cloth` in `lib/common/cloth_extraction.py`), so
               `from lib.common.train_util import *` (apps/ICON.py:20) still finds everything else it uses.
 
 Callers and call sites this serves: apps/ICON.py:17-22, 52-90 (HGPIFuNet, Seg3dLossless, query_func, get_visibility),
@@ -49,7 +49,9 @@ scripts/render_single.py:118 (computePRT of the dataset preparation: the rays ca
 prt/bounce.npy and prt/face.npy written),
 scripts/render_single.py:41, 97-141, 144-239 (initialize_GL_context, ColorRender and PRTRender: every render/,
 normal_F/B and T_normal_F/B image drawn on the kernels with no GL context; opengl_util's render_result, load_calib,
-make_rotate and rotateSH, Camera, load_scan and the script's RNG use stay the reference's).
+make_rotate and rotateSH, Camera, load_scan and the script's RNG use stay the reference's),
+apps/infer.py:566-605 (`-seg_dir`: extract_cloth's body-part labels and polygon test on the kernels, the mesh cut by
+the reference's own trimesh calls; load_segmentation and smpl_to_recon_labels stay the reference's).
 """
 import importlib.abc
 import importlib.machinery
@@ -78,7 +80,8 @@ def _replacements():
 
 
 def _patches():
-    from . import body_model, encoders, mesh, mesh_priors, mesh_views, metrics, net, prt, remesh, visibility, voxelize
+    from . import (body_model, encoders, garments, mesh, mesh_priors, mesh_views, metrics, net, prt, remesh, visibility,
+                   voxelize)
 
     def make_define_G(reference_define_G):
         import torch.nn as nn
@@ -113,6 +116,7 @@ def _patches():
         "lib.smplx.body_models": {"lbs": body_model.make_lbs},              # SMPL / SMPLH / SMPLX.forward's skinning
         "lib.pixielib.models.SMPLX": {"SMPLX": body_model.make_pixie_SMPLX},  # PIXIE's SMPL-X: skinning and heads
         "lib.renderer.prt_util": {"computePRT": prt.make_computePRT},       # the dataset renderer's PRT transfer
+        "lib.common.cloth_extraction": {"extract_cloth": garments.make_extract_cloth},  # -seg_dir garments
     }
 
 

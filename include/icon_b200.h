@@ -645,6 +645,28 @@ int icon_clean_mesh_count(const int64_t *faces, int64_t nv, int64_t nf, void *ws
 int icon_clean_mesh_emit(const void *verts, int verts_f64, const int64_t *faces, int64_t nv, int64_t nf, const void *ws,
                          float *out_verts, int32_t *out_faces, icon_stream_t stream);
 
+/* ---- garment extraction (csrc/garments.cu; reference lib/common/cloth_extraction.py:extract_cloth, called from
+ * apps/infer.py:566-605 with -seg_dir).  DESIGN.md 4.16.
+ * icon_garment_labels: labels[v] = h_smpl_parts[j*], j* the SMPL vertex nearest to reconstruction vertex v in the
+ *   float64 rdist ((x0-y0)^2 + (x1-y1)^2) + (x2-y2)^2, exact ties to the lowest j.  recon_verts [V,3] f64,
+ *   smpl_verts [S,3] f64, labels [V] u8 on the device; h_smpl_parts [S] u8 on the host (copied into `ws`),
+ *   ICON_EINVAL when one is 32 or more.  Brute force.
+ * icon_garment_face_mask: keep[v] = inside(v) && !(remove_parts >> labels[v] & 1), inside(v) = (x, y) of verts[v]
+ *   inside any polygon under matplotlib's crossings rule (a non-finite point is never inside; a polygon of fewer than
+ *   three vertices encloses nothing); face_mask[f] = keep of any corner of faces[f]; *kept_count = sum of face_mask.
+ *   Polygon p is poly_xy[h_poly_off[p] .. h_poly_off[p+1]) ([NP,2] f64 on the device; offsets [npoly+1] i32 on the
+ *   host, ICON_EINVAL when one decreases or leaves [0, NP]).  verts [V,3] f64, faces [F,3] i64, labels [V] u8,
+ *   face_mask [F] u8, kept_count one i32 on the device.  Synchronises `stream` before it returns: the kernels check
+ *   the labels and faces on the device and the verdict is read back; ICON_EINVAL when a label is 32 or more or a
+ *   face index is outside [0, V). */
+size_t icon_garment_labels_workspace_bytes(int S);
+int icon_garment_labels(const double *recon_verts, int V, const double *smpl_verts, int S, const uint8_t *h_smpl_parts,
+                        uint8_t *labels, void *ws, size_t ws_bytes, icon_stream_t stream);
+size_t icon_garment_face_mask_workspace_bytes(int V, int npoly);
+int icon_garment_face_mask(const double *verts, int V, const int64_t *faces, int F, const uint8_t *labels,
+                           uint32_t remove_parts, const double *poly_xy, int NP, const int32_t *h_poly_off, int npoly,
+                           uint8_t *face_mask, int32_t *kept_count, void *ws, size_t ws_bytes, icon_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
