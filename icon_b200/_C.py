@@ -138,6 +138,12 @@ _SIGS = {
     "icon_garment_face_mask_workspace_bytes": (_sz, [_i, _i]),
     "icon_garment_face_mask": (_i, [_vp, _i, _vp, _i, _vp, ctypes.c_uint32, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz,
                                     _vp]),
+    "icon_maxpool3s2_nhwc": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "icon_maf_mlp": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp]),
+    "icon_hps_gemv": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "icon_hps_rot6d": (_i, [_vp, _vp, _i, _vp]),
+    "icon_hps_regress": (_i, [_vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp]),
+    "icon_hps_tail": (_i, [_vp, _vp, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
 }
 
 EXPORTS = tuple(_SIGS.keys())

@@ -61,7 +61,7 @@ struct ActParams {
     int N, H, W, C, Cs_in, ci_off, Cp;
     int P;                   // halo (reflection) around the image in hi / lo; 0 with s2d
     int s2d;                 // 1: 4 parity planes of (H/2, W/2) -- plane = (y & 1) * 2 + (x & 1)
-    int relu;
+    int relu;                // 1: ReLU before the residual add; 2: after it (a Bottleneck's relu(bn3(conv3) + residual))
 };
 
 // one thread = one (destination pixel, 8-channel group)
@@ -115,7 +115,7 @@ __global__ void k_act_nhwc(const __grid_constant__ ActParams p) {
             }
         }
     }
-    if (p.relu) {
+    if (p.relu == 1) {
 #pragma unroll
         for (int k = 0; k < 8; ++k) v[k] = fmaxf(v[k], 0.f);
     }
@@ -129,6 +129,10 @@ __global__ void k_act_nhwc(const __grid_constant__ ActParams p) {
             for (int k = 0; k < 8; ++k)
                 if (c0 + k < p.C) v[k] += rs[k];
         }
+    }
+    if (p.relu == 2) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = fmaxf(v[k], 0.f);
     }
     if (p.f32 && interior) {
         float *fd = p.f32 + spix * p.C + c0;
@@ -536,6 +540,7 @@ extern "C" int icon_act_nhwc(const float *x, int Cs_in, int ci_off, const float 
     ICON_CHECK_ARG(ci_off >= 0 && ci_off + C <= Cs_in, "icon_act_nhwc: channel slice outside the input tensor");
     ICON_CHECK_ARG(!(scale_shift && stats), "icon_act_nhwc: scale_shift and stats are exclusive");
     ICON_CHECK_ARG((gamma == nullptr) == (beta == nullptr), "icon_act_nhwc: gamma and beta go together");
+    ICON_CHECK_ARG(relu >= 0 && relu <= 2, "icon_act_nhwc: relu %d (0 none, 1 before the residual, 2 after it)", relu);
     ActParams p{};
     p.stats = stats; p.gamma = gamma; p.beta = beta; p.eps = eps; p.cg = 1; p.inv_count = 1.0 / ((double)H * W);
     if (stats && groups > 0) {

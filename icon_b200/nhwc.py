@@ -146,7 +146,7 @@ def finalize(raw, norm=None):
 
 def act(raw, ss=None, relu=False, res=None, operand=True, halo=0, s2d=False, f32=False):
     """y = [relu]((x - mean) * scale + beta) [+ res] -> (Operand or None, fp32 NHWC tensor or None); `ss` is a NormSpec,
-    a [N, C, 3] (scale, mean, beta) table or None (identity)."""
+    a [N, C, 3] (scale, mean, beta) table or None (identity); relu = 2 applies the ReLU after the residual add."""
     dev = raw.t.device
     N, H, W, C = raw.N, raw.H, raw.W, raw.C
     Cp = _pad64(C)
@@ -175,7 +175,7 @@ def act(raw, ss=None, relu=False, res=None, operand=True, halo=0, s2d=False, f32
     else:
         table = ss
     check(lib.icon_act_nhwc(_p(raw.t), raw.Cs, raw.c_off, _p(table), _p(stats), _p(gamma), _p(beta), groups, eps, _p(res),
-                            _p(hi), _p(lo), _p(out), N, H, W, C, Cp, int(halo), 1 if s2d else 0, 1 if relu else 0,
+                            _p(hi), _p(lo), _p(out), N, H, W, C, Cp, int(halo), 1 if s2d else 0, int(relu),
                             _stream()), "icon_act_nhwc")
     op = Operand(hi, lo, N, H, W, C, Cp, halo, s2d) if operand else None
     return op, out
@@ -457,7 +457,7 @@ def conv_transpose(op, m, stats=True):
         raise NotImplementedError("conv_transpose: stride 2 on a plain operand")
     OH, OW = (op.H - 1) * s - 2 * pad + KH + opad, (op.W - 1) * s - 2 * pad + KW + opad
     if OH != 2 * op.H or OW != 2 * op.W:
-        raise NotImplementedError("conv_transpose: output must be exactly 2x (k3 s2 p1 op1)")
+        raise NotImplementedError("conv_transpose: output must be exactly 2x (k3 s2 p1 op1, k4 s2 p1 op0)")
     cpt = op.Cp // 64
     n_tile = _n_tile(Cout)
     packed = packed_weight(m, True, op.Cp, n_tile)

@@ -80,8 +80,8 @@ def _replacements():
 
 
 def _patches():
-    from . import (body_model, encoders, garments, mesh, mesh_priors, mesh_views, metrics, net, prt, remesh, visibility,
-                   voxelize)
+    from . import (body_model, encoders, garments, hps, mesh, mesh_priors, mesh_views, metrics, net, prt, remesh,
+                   visibility, voxelize)
 
     def make_define_G(reference_define_G):
         import torch.nn as nn
@@ -117,6 +117,7 @@ def _patches():
         "lib.pixielib.models.SMPLX": {"SMPLX": body_model.make_pixie_SMPLX},  # PIXIE's SMPL-X: skinning and heads
         "lib.renderer.prt_util": {"computePRT": prt.make_computePRT},       # the dataset renderer's PRT transfer
         "lib.common.cloth_extraction": {"extract_cloth": garments.make_extract_cloth},  # -seg_dir garments
+        "lib.pymaf.models.pymaf_net": {"PyMAF": hps.make_PyMAF},           # the body estimate (-hps_type pymaf)
     }
 
 

@@ -460,3 +460,266 @@ def tetra_model(kind="tiny", seed=0, folder=None):
                                               "posedirs_added", "tetrahedrons")})
     np.savetxt(paths[2], out["tets"], fmt="%d")
     return out, paths
+
+
+# ---------------------------------------------------------------- PyMAF (lib/pymaf/models/pymaf_net.py)
+
+PYMAF_DMAP_SIZES = (6890, 1723, 431)
+
+
+def pymaf_tables(seed=0):
+    """Seeded SMPL tables PyMAF reads besides the body model (float32 unless stated): J_regressor_extra [9,6890]
+    (rows of 4 nearby vertices, positive weights summing to 1), the two sparse downsampling matrices D0 [1723,6890]
+    and D1 [431,1723] (rows of 1..3 positive weights summing to 1) and their product Dmap [431,6890], 21 vertex-joint
+    ids (int64, distinct), a joint_map of 49 entries into the 54 [24 lbs, 21 vertex, 9 extra] joints (int64), and the
+    mean parameters pose [144] (6-D rotations near the identity), shape [10] and cam [3] (scale near 0.9)."""
+    rng = np.random.RandomState(seed + 7001)
+    bm = body_model("smpl", seed=seed)
+    v = bm["v_template"].astype(np.float64)
+    nv = len(v)
+    jx = np.zeros((9, nv), np.float64)
+    for r, c in enumerate(rng.choice(nv, 9, replace=False)):
+        near = np.argsort(((v - v[c]) ** 2).sum(1), kind="stable")[:4]
+        w = rng.uniform(0.5, 1.5, 4)
+        jx[r, near] = w / w.sum()
+    D = []
+    for rows, cols in ((PYMAF_DMAP_SIZES[1], PYMAF_DMAP_SIZES[0]), (PYMAF_DMAP_SIZES[2], PYMAF_DMAP_SIZES[1])):
+        d = np.zeros((rows, cols), np.float32)
+        for r in range(rows):
+            k = rng.randint(1, 4)
+            w = rng.uniform(0.5, 1.5, k)
+            d[r, rng.choice(cols, k, replace=False)] = w / w.sum()
+        D.append(d)
+    eye6 = np.tile(np.array([1, 0, 0, 1, 0, 0], np.float32), 24)
+    return dict(body=bm, J_regressor_extra=jx.astype(np.float32), D=D,
+                Dmap=(D[1].astype(np.float64) @ D[0].astype(np.float64)).astype(np.float32),
+                vertex_ids=np.sort(rng.choice(nv, 21, replace=False)).astype(np.int64),
+                joint_map=rng.choice(54, 49, replace=False).astype(np.int64),
+                pose=(eye6 + 0.1 * rng.standard_normal(144)).astype(np.float32),
+                shape=(0.5 * rng.standard_normal(10)).astype(np.float32),
+                cam=np.array([0.9, 0.05, 0.2], np.float32) + (0.02 * rng.standard_normal(3)).astype(np.float32))
+
+
+def pymaf_state_dict(seed=0, tables=None):
+    """Every key and shape of PyMAF's state_dict (res50 backbone, three k4 deconvolutions of 256 channels, three MAF
+    extractors with MLP_DIM [256, 128, 64, 5], three regressors with their SMPL, dp_head), seeded with NumPy's
+    RandomState: He-scaled convolutions; trained-like BatchNorms (running mean ~ N(0, 0.1), variance U(0.5, 1.5),
+    gamma U(0.5, 1.5) and U(0.2, 1) for the last BN of each block, beta ~ N(0, 0.1)); MAF and fc layers uniform in
+    +-1 / sqrt(fan_in) (torch's defaults); decpose / decshape / deccam xavier-uniform with gain 0.01.  The SMPL
+    buffers and mean parameters come from pymaf_tables(seed)."""
+    rng = np.random.RandomState(seed)
+    T = pymaf_tables(seed) if tables is None else tables
+    sd = {}
+
+    def t(a):
+        return torch.from_numpy(np.ascontiguousarray(a))
+
+    def conv(name, cout, cin, k):
+        sd[name] = t((rng.standard_normal((cout, cin, k, k)) * math.sqrt(2.0 / (cin * k * k))).astype(np.float32))
+
+    def bn(name, c, last=False):
+        sd[name + ".weight"] = t(rng.uniform(0.2, 1.0, c) if last else rng.uniform(0.5, 1.5, c)).float()
+        sd[name + ".bias"] = t(0.1 * rng.standard_normal(c)).float()
+        sd[name + ".running_mean"] = t(0.1 * rng.standard_normal(c)).float()
+        sd[name + ".running_var"] = t(rng.uniform(0.5, 1.5, c)).float()
+        sd[name + ".num_batches_tracked"] = torch.tensor(0, dtype=torch.int64)
+
+    def uni(shape, fan_in, gain=None, fan_out=None):
+        b = 1.0 / math.sqrt(fan_in) if gain is None else gain * math.sqrt(6.0 / (fan_in + fan_out))
+        return t(rng.uniform(-b, b, shape).astype(np.float32))
+
+    fe = "feature_extractor."
+    conv(fe + "conv1.weight", 64, 3, 7)
+    bn(fe + "bn1", 64)
+    inplanes = 64
+    for li, (planes, n) in enumerate(zip((64, 128, 256, 512), (3, 4, 6, 3))):
+        for b in range(n):
+            pre = f"{fe}layer{li + 1}.{b}."
+            conv(pre + "conv1.weight", planes, inplanes, 1)
+            bn(pre + "bn1", planes)
+            conv(pre + "conv2.weight", planes, planes, 3)
+            bn(pre + "bn2", planes)
+            conv(pre + "conv3.weight", planes * 4, planes, 1)
+            bn(pre + "bn3", planes * 4, last=True)
+            if b == 0:
+                conv(pre + "downsample.0.weight", planes * 4, inplanes, 1)
+                bn(pre + "downsample.1", planes * 4, last=True)
+            inplanes = planes * 4
+    for i in range(3):
+        cin = inplanes if i == 0 else 256
+        sd[f"deconv_layers.{3 * i}.weight"] = t((rng.standard_normal((cin, 256, 4, 4))
+                                                  * math.sqrt(2.0 / (cin * 4))).astype(np.float32))
+        bn(f"deconv_layers.{3 * i + 1}", 256)
+    bm = T["body"]
+    for i in range(3):
+        m = f"maf_extractor.{i}."
+        for k, (cout, cin) in enumerate(((128, 256), (64, 384), (5, 320))):
+            sd[m + f"conv{k}.weight"] = uni((cout, cin, 1), cin)
+            sd[m + f"conv{k}.bias"] = uni((cout,), cin)
+        sd[m + "Dmap"] = t(T["Dmap"])
+    lin = torch.linspace(-1, 1, 21)
+    xv, yv = torch.meshgrid([lin, lin], indexing="ij")
+    sd["points_grid"] = torch.stack([xv.reshape(-1), yv.reshape(-1)]).unsqueeze(0)
+    for i in range(3):
+        r = f"regressor.{i}."
+        feat = 441 * 5 if i == 0 else 431 * 5
+        for name, (cout, cin) in (("fc1", (1024, feat + 157)), ("fc2", (1024, 1024))):
+            sd[r + name + ".weight"] = uni((cout, cin), cin)
+            sd[r + name + ".bias"] = uni((cout,), cin)
+        for name, cout in (("decpose", 144), ("decshape", 10), ("deccam", 3)):
+            sd[r + name + ".weight"] = uni((cout, 1024), 1024, gain=0.01, fan_out=cout)
+            sd[r + name + ".bias"] = uni((cout,), 1024)
+        s = r + "smpl."
+        sd[s + "betas"] = torch.zeros(64, 10)
+        sd[s + "global_orient"] = torch.zeros(64, 3)
+        sd[s + "body_pose"] = torch.zeros(64, 69)
+        sd[s + "faces_tensor"] = t(bm["faces"].astype(np.int64))
+        sd[s + "v_template"] = t(bm["v_template"])
+        sd[s + "shapedirs"] = t(bm["shapedirs"])
+        sd[s + "J_regressor"] = t(bm["J_regressor"])
+        sd[s + "posedirs"] = t(bm["posedirs"])
+        sd[s + "parents"] = t(bm["parents"])
+        sd[s + "lbs_weights"] = t(bm["lbs_weights"])
+        sd[s + "vertex_joint_selector.extra_joints_idxs"] = t(T["vertex_ids"])
+        sd[s + "J_regressor_extra"] = t(T["J_regressor_extra"])
+        sd[r + "init_pose"] = t(T["pose"][None])
+        sd[r + "init_shape"] = t(T["shape"][None])
+        sd[r + "init_cam"] = t(T["cam"][None])
+    for name, cout in (("predict_u", 25), ("predict_v", 25), ("predict_ann_index", 15), ("predict_uv_index", 25)):
+        sd[f"dp_head.{name}.weight"] = uni((cout, 256, 3, 3), 256 * 9)
+        sd[f"dp_head.{name}.bias"] = uni((cout,), 256 * 9)
+    return sd
+
+
+def pymaf_image(seed=0):
+    """An ImageNet-normalised-looking [1,3,224,224] float32 image: a smooth seeded field plus noise."""
+    rng = np.random.RandomState(seed + 9100)
+    yy, xx = np.meshgrid(np.linspace(-1, 1, 224), np.linspace(-1, 1, 224), indexing="ij")
+    img = np.stack([np.sin(3 * xx + c) * np.cos(2 * yy - c) for c in range(3)])
+    img = img + 0.3 * rng.standard_normal((3, 224, 224))
+    return torch.from_numpy(img[None].astype(np.float32))
+
+
+PYMAF_PARAMETERS = ("weight", "bias", "betas", "global_orient", "body_pose")
+
+
+def pymaf_standin(state_dict, joint_map, cfg):
+    """A fresh class standing in for the reference's PyMAF where no checkout exists: a module tree whose state_dict
+    has exactly `state_dict`'s keys (`weight` / `bias` and SMPL's betas / pose are parameters that require grad, as
+    in the reference's module, every other tensor a buffer; numeric children as ModuleLists so that
+    `regressor[i].smpl.joint_map` resolves), a `forward(x, J_regressor=None)` that records its calls and returns
+    "reference", and `cfg` bound in a module of its own, as lib.pymaf.models.pymaf_net binds it."""
+    import sys
+    import types
+    from torch import nn
+
+    mod = types.ModuleType(f"icon_b200_pymaf_standin_{len([m for m in sys.modules if 'pymaf_standin' in m])}")
+    mod.cfg = cfg
+    sys.modules[mod.__name__] = mod
+
+    def tree(names):
+        kids = {}
+        for k in names:
+            head, _, rest = k.partition(".")
+            kids.setdefault(head, []).append(rest)
+        return kids
+
+    def build(m, prefix, names):
+        for head, rests in tree(names).items():
+            if rests == [""]:
+                t = state_dict[prefix + head].clone()
+                if head in PYMAF_PARAMETERS and t.is_floating_point() and "running" not in head:
+                    m.register_parameter(head, nn.Parameter(t))
+                else:
+                    m.register_buffer(head, t)
+                continue
+            sub = tree(rests)
+            if all(h.isdigit() for h in sub):
+                child = nn.ModuleList([nn.Module() for _ in range(max(int(h) for h in sub) + 1)])
+                for h, rs in sub.items():
+                    build(child[int(h)], f"{prefix}{head}.{h}.", rs)
+            else:
+                child = nn.Module()
+                build(child, f"{prefix}{head}.", rests)
+            m.add_module(head, child)
+
+    class PyMAF(nn.Module):
+        calls = []
+
+        def __init__(self):
+            super().__init__()
+            build(self, "", list(state_dict))
+            for r in self.regressor:
+                r.smpl.joint_map = torch.as_tensor(joint_map).long()
+
+        def forward(self, x, J_regressor=None):
+            PyMAF.calls.append((x, J_regressor))
+            return "reference"
+
+    PyMAF.__module__ = mod.__name__
+    mod.PyMAF = PyMAF
+    return PyMAF
+
+
+def pymaf_cfg():
+    """The shipped lib/pymaf/configs/pymaf_config.yaml values PyMAF reads, as attribute namespaces."""
+    from types import SimpleNamespace as NS
+    return NS(MODEL=NS(PyMAF=NS(BACKBONE="res50", MLP_DIM=[256, 128, 64, 5], N_ITER=3, AUX_SUPV_ON=True)),
+              RES_MODEL=NS(DECONV_WITH_BIAS=False, NUM_DECONV_LAYERS=3, NUM_DECONV_FILTERS=[256, 256, 256],
+                           NUM_DECONV_KERNELS=[4, 4, 4]),
+              LOSS=NS(POINT_REGRESSION_WEIGHTS=0.5))
+
+
+PYMAF_FILES = ("smpl_related/models/smpl/SMPL_NEUTRAL.pkl", "pymaf_data/J_regressor_extra.npy",
+               "pymaf_data/mesh_downsampling.npz", "pymaf_data/smpl_mean_params.npz")
+
+
+def pymaf_files(folder, seed=0):
+    """Write, under `folder`, the model files PyMAF loads (PYMAF_FILES), at the real sizes, from pymaf_tables(seed):
+    SMPL_NEUTRAL.pkl (plain NumPy arrays: v_template, f, J_regressor, weights, posedirs [V,3,207], shapedirs [V,3,10],
+    kintree_table with the root entry 4294967295), J_regressor_extra.npy [9,6890], mesh_downsampling.npz (D: the two
+    sparse downsampling matrices; U: their transposes; A: the adjacency of the three levels as sparse identities) and
+    smpl_mean_params.npz (pose [144], shape [10], cam [3], float32).  Returns (tables, paths)."""
+    import os
+    import pickle
+
+    import scipy.sparse as sp
+    T = pymaf_tables(seed)
+    bm = T["body"]
+    V = len(bm["v_template"])
+    paths = tuple(os.path.join(folder, n) for n in PYMAF_FILES)
+    for p in paths:
+        os.makedirs(os.path.dirname(p), exist_ok=True)
+    kin = np.stack([np.asarray(SMPL_PARENTS, np.int64), np.arange(24, dtype=np.int64)])
+    kin[0, 0] = 4294967295
+    with open(paths[0], "wb") as fh:
+        pickle.dump(dict(v_template=bm["v_template"].astype(np.float64), f=bm["faces"].astype(np.int64),
+                         J_regressor=sp.csc_matrix(bm["J_regressor"].astype(np.float64)),
+                         weights=bm["lbs_weights"].astype(np.float64),
+                         posedirs=bm["posedirs"].T.reshape(V, 3, -1).astype(np.float64),
+                         shapedirs=bm["shapedirs"].astype(np.float64), kintree_table=kin), fh, protocol=2)
+    np.save(paths[1], T["J_regressor_extra"])
+
+    def objs(xs):
+        a = np.empty(len(xs), dtype=object)
+        for i, x in enumerate(xs):
+            a[i] = x
+        return a
+    D = [sp.csr_matrix(d) for d in T["D"]]
+    np.savez(paths[2], D=objs(D), U=objs([d.T.tocsr() for d in D]),
+             A=objs([sp.identity(n, format="csr", dtype=np.float32) for n in PYMAF_DMAP_SIZES]))
+    np.savez(paths[3], pose=T["pose"], shape=T["shape"], cam=T["cam"])
+    return T, paths
+
+
+def pymaf_sha256(state_dict):
+    """SHA-256 over the state dict's keys, dtypes, shapes and bytes in key order: seed drift fails loudly."""
+    import hashlib
+    h = hashlib.sha256()
+    for k in sorted(state_dict):
+        t = state_dict[k].detach().cpu().contiguous()
+        h.update(k.encode())
+        h.update(str(t.dtype).encode())
+        h.update(str(tuple(t.shape)).encode())
+        h.update(t.numpy().tobytes())
+    return h.hexdigest()

@@ -593,7 +593,8 @@ int icon_conv3d(const float *x, const float *w, const float *scale, const float 
  *   same.
  * icon_norm_finalize: stats -> [N][C][3] (scale, mean, beta) for InstanceNorm2d (groups = 0) / GroupNorm(groups) with
  *   affine; a consumer computes y = (x - mean) * scale + beta, so a constant channel gives exactly beta.
- * icon_act_nhwc: y = [relu]((x - mean) * scale + beta) [+ res], from the `scale_shift` table or folded in from the
+ * icon_act_nhwc: y = [relu]((x - mean) * scale + beta) [+ res] (relu = 1), or relu(... + res) (relu = 2: the ReLU
+ *   after the residual add that ends a ResNet Bottleneck), from the `scale_shift` table or folded in from the
  *   producer's `stats` (+ GroupNorm gamma / beta, groups = 0: instance norm; 1, 2, 4 or 8 channels per group)
  *   -> hi / lo operand tensors (halo > 0: reflection halo;
  *   s2d = 1: four parity planes for a stride-2 consumer; channels padded to Cp with zeros) and / or fp32 NHWC.
@@ -666,6 +667,34 @@ size_t icon_garment_face_mask_workspace_bytes(int V, int npoly);
 int icon_garment_face_mask(const double *verts, int V, const int64_t *faces, int F, const uint8_t *labels,
                            uint32_t remove_parts, const double *poly_xy, int NP, const int32_t *h_poly_off, int npoly,
                            uint8_t *face_mask, int32_t *kept_count, void *ws, size_t ws_bytes, icon_stream_t stream);
+
+/* ---- PyMAF's body estimate (csrc/hps.cu; reference lib/pymaf/models/pymaf_net.py, maf_extractor.py, smpl.py,
+ * utils/geometry.py).  DESIGN.md 4.17.  All buffers fp32 on the device; dot products accumulate in float64.
+ * icon_maxpool3s2_nhwc: MaxPool2d(3, 2, 1) of x [N,H,W,C] (of relu(x) when relu != 0) -> the plain hi / lo operand
+ *   [N,OH,OW,Cp] (Cp % 64 == 0, channels >= C written 0), OH = (H - 1) / 2 + 1.
+ * icon_maf_mlp: per point n of pts [2,N] (x row, y row): bilinear grid_sample (align_corners, zero padding) of the
+ *   256 channels of feat [H,W,256], then Conv1d 256->128 + leaky 0.01, [., feature] 384->64 + leaky,
+ *   [., feature] 320->5 + ReLU (w1 [128,256], w2 [64,384], w3 [5,320]) -> xc[c * N + n]; xc[5N .. 5N + nprev) = prev.
+ * icon_hps_gemv: y [R] = w [R,K] x [K] + b [+ add], K <= 12288.
+ * icon_hps_rot6d: rot6d_to_rotmat of pose [J,6] -> rotmat [J,3,3].
+ * icon_hps_regress: extra [E,3] = jextra [E,V] verts [V,3]; for Dmap in CSR (row_off [M+1], col, val), the
+ *   projection of Dmap verts with cam [3] -> pts [2,M].
+ * icon_hps_tail: kp_3d [NJ,3] = [jlbs [Jl,3], verts[vid] [NV,3], extra [E,3]][jmap], kp_2d [NJ,2] its projection with
+ *   the cam at par[npose + nshape], theta = [cam, par[npose .. npose + nshape), angle-axis of rotmat [Jl,3,3]]
+ *   (kornia's quaternion route, NaN -> 0).  vid and jmap are checked by the caller. */
+int icon_maxpool3s2_nhwc(const float *x, void *hi, void *lo, int N, int H, int W, int C, int Cp, int relu,
+                         icon_stream_t stream);
+int icon_maf_mlp(const float *feat, int H, int W, int C, const float *pts, int N, const float *w1, const float *b1,
+                 const float *w2, const float *b2, const float *w3, const float *b3, const float *prev, int nprev,
+                 float *xc, icon_stream_t stream);
+int icon_hps_gemv(const float *w, const float *x, const float *b, const float *add, float *y, int R, int K,
+                  icon_stream_t stream);
+int icon_hps_rot6d(const float *pose, float *rotmat, int J, icon_stream_t stream);
+int icon_hps_regress(const float *verts, int V, const float *jextra, int E, float *extra, const int *row_off,
+                     const int *col, const float *val, int M, const float *cam, float *pts, icon_stream_t stream);
+int icon_hps_tail(const float *verts, const float *jlbs, int Jl, const int *vid, int NV, const float *extra, int E,
+                  const int *jmap, int NJ, const float *rotmat, const float *par, int npose, int nshape, float *kp3d,
+                  float *kp2d, float *theta, icon_stream_t stream);
 
 #ifdef __cplusplus
 }
