@@ -11,10 +11,12 @@
 //   * barycentrics w0 = e(p, v1, v2) / (area + 1e-8), w1 = e(p, v2, v0) / .., w2 = e(p, v0, v1) / ..; the pixel is
 //     covered when all three are > 0; depth uses the perspective-corrected weights
 //     (w0 z1 z2, z0 w1 z2, z0 z1 w2) / (their sum + 1e-8), pz = sum w_i z_i, pixels with pz < 0 are dropped;
-//   * the nearest pz wins, ties go to the lowest face index (scan order of the naive rasteriser).
+//   * the nearest pz wins, ties go to the lowest face index (scan order of the naive rasteriser); -0 ties with +0,
+//     and pz = +inf (the background's depth) or NaN never takes a pixel.
 // Bug-compatibility: `faces[torch.unique(pix_to_face)]` also indexes with the background value -1, i.e. the LAST
 // face, whenever some pixel is empty (mesh_util.py:310) -- its three vertices are then marked visible too.
-// Coverage / depth are compared bit for bit with oracle/visibility.py, hence -fmad=false for this file.
+// pix_to_face, the depth of every pixel (read back from the workspace, include/icon_b200.h) and the mask are compared
+// bit for bit with oracle/visibility.py, hence -fmad=false for this file.
 #include "common.cuh"
 
 namespace icon {
@@ -43,11 +45,14 @@ __global__ void k_vis_raster(const float *__restrict__ xyz, const int64_t *__res
     if (zmax < 0.f || area < 0.f || (area <= 1e-8f && area >= -1e-8f)) return;
     const float xmin = fminf(fminf(v[0][0], v[1][0]), v[2][0]), xmax = fmaxf(fmaxf(v[0][0], v[1][0]), v[2][0]);
     const float ymin = fminf(fminf(v[0][1], v[1][1]), v[2][1]), ymax = fmaxf(fmaxf(v[0][1], v[1][1]), v[2][1]);
-    // pixel index ranges whose centres can fall inside [min, max]: x_ndc = 1 - (2 xi + 1) / S (conservative by 1)
+    // pixel index ranges whose centres can fall inside [min, max]: x_ndc = 1 - (2 xi + 1) / S (conservative by 1),
+    // clamped in float before the int conversion -- a vertex far off screen must not saturate it and wrap the count
+    // -- and so that a NaN bound (all three coordinates NaN) spans the whole image, as the oracle evaluates it
     const float Sf = (float)S;
-    int xi0 = (int)floorf(((1.f - xmax) * Sf - 1.f) * 0.5f) - 1, xi1 = (int)ceilf(((1.f - xmin) * Sf - 1.f) * 0.5f) + 1;
-    int yi0 = (int)floorf(((1.f - ymax) * Sf - 1.f) * 0.5f) - 1, yi1 = (int)ceilf(((1.f - ymin) * Sf - 1.f) * 0.5f) + 1;
-    xi0 = max(xi0, 0); yi0 = max(yi0, 0); xi1 = min(xi1, S - 1); yi1 = min(yi1, S - 1);
+    const int xi0 = (int)fminf(fmaxf(floorf(((1.f - xmax) * Sf - 1.f) * 0.5f) - 1.f, 0.f), Sf);
+    const int xi1 = (int)fmaxf(fminf(ceilf(((1.f - xmin) * Sf - 1.f) * 0.5f) + 1.f, Sf - 1.f), -1.f);
+    const int yi0 = (int)fminf(fmaxf(floorf(((1.f - ymax) * Sf - 1.f) * 0.5f) - 1.f, 0.f), Sf);
+    const int yi1 = (int)fmaxf(fminf(ceilf(((1.f - ymin) * Sf - 1.f) * 0.5f) + 1.f, Sf - 1.f), -1.f);
     const int nx = xi1 - xi0 + 1, ny = yi1 - yi0 + 1;
     if (nx <= 0 || ny <= 0) return;
     const float den = area + 1e-8f;
@@ -63,8 +68,12 @@ __global__ void k_vis_raster(const float *__restrict__ xyz, const int64_t *__res
         const float t0 = w0 * z1 * z2, t1 = z0 * w1 * z2, t2 = z0 * z1 * w2;
         const float dsum = (t0 + t1 + t2) + 1e-8f;
         const float pz = (t0 / dsum) * z0 + (t1 / dsum) * z1 + (t2 / dsum) * z2;
-        if (!(pz >= 0.f)) continue;
-        const unsigned long long key = ((unsigned long long)__float_as_uint(pz) << 32) | (unsigned)f;
+        // the oracle takes a pixel on a strictly nearer depth only: NaN, pz < 0 and pz = +inf (the background's
+        // depth) never take one
+        if (!(pz >= 0.f && pz < INFINITY)) continue;
+        // pz is +0 .. +FLT_MAX or -0 here: clearing the sign makes -0 the key of +0, so -0 ties with +0 (lowest face
+        // wins) and is nearer than every positive depth, as `pz < zbuf` orders them
+        const unsigned long long key = ((unsigned long long)(__float_as_uint(pz) & 0x7fffffffu) << 32) | (unsigned)f;
         atomicMin(&zbuf[(size_t)yi * S + xi], key);
     }
 }

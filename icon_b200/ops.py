@@ -475,9 +475,7 @@ def voxelize(verts, n_surface, codes, tets, res, sigma):
 
 
 # --------------------------------------------------------------------------- vertex visibility
-def visibility(xyz, faces, image_size=4096):
-    """xyz [V,3] f32 screen-space vertices ((cat(xy, -z) + 1) / 2), faces [F,3] int64 -> vis [V] f32 (0/1), CUDA;
-    include/icon_b200.h: icon_visibility."""
+def _visibility(xyz, faces, image_size):
     _need_cuda(xyz)
     v = xyz.detach().float().contiguous()
     f = faces.detach().to(device=v.device, dtype=torch.int64).contiguous()
@@ -488,4 +486,24 @@ def visibility(xyz, faces, image_size=4096):
     ws = torch.empty(nbytes, dtype=torch.uint8, device=v.device)
     check(lib.icon_visibility(_p(v), v.shape[0], _p(f), f.shape[0], int(image_size), _p(vis), _p(ws), nbytes,
                               _stream()), "icon_visibility")
-    return vis
+    return vis, ws
+
+
+def visibility(xyz, faces, image_size=4096):
+    """xyz [V,3] f32 screen-space vertices ((cat(xy, -z) + 1) / 2), faces [F,3] int64 -> vis [V] f32 (0/1), CUDA;
+    include/icon_b200.h: icon_visibility."""
+    return _visibility(xyz, faces, image_size)[0]
+
+
+def visibility_zbuffer(xyz, faces, image_size=4096):
+    """The z-buffer icon_visibility leaves in its workspace, decoded: same inputs as `visibility` ->
+    (pix_to_face int64 [S,S] with -1 for background, depth float32 [S,S] with +inf for background), CUDA.
+    Row r, column c is the pixel centred at NDC (1 - (2c + 1)/S, 1 - (2r + 1)/S), as oracle/visibility.py."""
+    S = int(image_size)
+    _, ws = _visibility(xyz, faces, S)
+    key = ws[:S * S * 8].view(torch.int64).view(S, S)
+    empty = key == -1                                   # all ones: the cleared buffer
+    p2f = torch.where(empty, -1, key & 0xffffffff)
+    depth = (key >> 32).to(torch.int32).view(torch.float32)
+    depth = torch.where(empty, float("inf"), depth)
+    return p2f, depth

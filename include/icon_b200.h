@@ -275,7 +275,10 @@ int icon_voxelize(const float *verts, int NV, int NVsurf, const float *codes, co
  * Replaces get_visibility (lib/dataset/mesh_util.py:280-316): z-buffer rasterisation of the body at
  * image_size^2 (4096 in the reference) with pytorch3d's conventions (csrc/visibility.cu header; parity unpinned),
  * vis[v] = 1 for the vertices of every face that owns a pixel (plus the last face's, as faces[-1] does upstream).
- * xyz [V,3] f32 = (cat(xy, -z) + 1) / 2 as the reference builds it, faces [F,3] i64, vis [V] f32. */
+ * xyz [V,3] f32 = (cat(xy, -z) + 1) / 2 as the reference builds it, faces [F,3] i64, vis [V] f32.
+ * On return the first image_size^2 * 8 bytes of ws hold the z-buffer, row-major [S][S] u64: all ones for an
+ * empty pixel, else (bits of the owner's depth, sign cleared) << 32 | owner's face index; row r, column c is the
+ * pixel centred at NDC (1 - (2c + 1)/S, 1 - (2r + 1)/S). */
 size_t icon_visibility_workspace_bytes(int image_size);
 int icon_visibility(const float *xyz, int V, const int64_t *faces, int F, int image_size, float *vis,
                     void *ws, size_t ws_bytes, icon_stream_t stream);
